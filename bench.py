@@ -8,7 +8,7 @@
 One "step" = one pass of the hot path over one batch of synthetic search regions — the whole frame of
 `siamese_track` (tools/test.py:201-261): `track_mask` (backbone -> depthwise xcorr -> cls/loc/mask heads) ->
 score/box post-processing + argmax ON THE DEVICE -> `track_refine` at the selected position, for B paired tracker
-streams per GPU (BASELINE.json configs[1]: "batch=64 synthetic search regions, 1xB200, full track() path with mask
+streams per GPU (BASELINE.json configs[1]: "batch=64 synthetic search regions, 1xH100, full track() path with mask
 refine"); templates are cached per slot (configs[3]).  N>1: one process per GPU (torchrun), streams are sharded, the
 packed weights are broadcast ONCE over NCCL at init, no per-frame collective ("weak" scaling).
 
@@ -17,8 +17,8 @@ the same frame through the host-buffer call `sm_step_host_async` (H2D of every f
 records and refine logits inside the timed region, SAME flags as `value`); `roofline` = the tensor-core conv family
 (dominant kernel) timed per launch with CUDA events; `cpu_baseline` = the oracle port of the reference timed on all of
 this box's host cores; `parity_check` = max relative error of this run's outputs against the CPU oracle.
-The timed region is at least --min-seconds long (default 2 s): every reported step is repeated `passes_per_step`
-times inside it and all per-step figures are per pass.
+The timed region of `value` is exactly --steps steps; the other legs (e2e, loop, roofline) size their own regions.
+--dump-outputs DIR writes what the last timed step returned (see dump_outputs).
 """
 from __future__ import annotations
 
@@ -49,11 +49,12 @@ def load_peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tflops": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "tflops_burst": d["bf16_tflops"], "src": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "tflops": 1400.0, "tflops_burst": 1590.0, "src": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense fp16 / bf16
+    return {"hbm_gbs": 3350.0, "tflops": 989.0, "tflops_burst": 989.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md).  The process is
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region.  The process is
     started (and its first sample awaited) before the warm-up, so its start-up cost never lands inside the timed
     region; a reader thread time-stamps every sample and `stop()` keeps those inside [t0, t1]."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -248,7 +249,7 @@ def workload_config(args, batch_per_gpu, world):
                            "no per-frame collective; inside a GPU the batch runs as two concurrent lanes of "
                            "batch_per_gpu/2 streams (batches >= 16)",
             "l2": "inputs rotate over 4 device buffers (4 x 50 MB at B=64) and every step streams > 5 GB of "
-                  "activations (>> 126 MB L2)"}
+                  "activations (>> 50 MB L2)"}
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -352,10 +353,13 @@ def run_gpu(args, rank, local_rank, world):
     m.template(z, slot0=0)
     m.template(z, slot0=B)
 
+    last = {}
+
     def step(i, mask_head=True):
         # the whole frame of siamese_track (tools/test.py:201-261) in one engine call, nothing leaves the device
-        return m.step(xs[i % 4], anchors_dev, window_dev, tsz_dev, PENALTY_K, WINDOW_INFLUENCE, refine=sharp,
+        last["out"] = m.step(xs[i % 4], anchors_dev, window_dev, tsz_dev, PENALTY_K, WINDOW_INFLUENCE, refine=sharp,
                       mask_head=sharp and mask_head)
+        return last["out"]
 
     def barrier():
         torch.cuda.synchronize()
@@ -377,14 +381,8 @@ def run_gpu(args, rank, local_rank, world):
     warm = max(args.warmup, 3)
     for i in range(warm):
         step(i)
-    # size the timed region: at least --min-seconds, every reported step = `passes` passes over a batch
     est_ms = timed(step, 3) / 3
-    passes = max(1, math.ceil(args.min_seconds * 1e3 / (est_ms * args.steps)))
-    if world > 1:
-        t = torch.tensor([passes], device=dev)
-        dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        passes = int(t.item())
-    n_pass = args.steps * passes
+    n_pass = args.steps
     l0 = m.launch_count
     t_start = time.perf_counter()
     ms = timed(step, n_pass)
@@ -392,6 +390,8 @@ def run_gpu(args, rank, local_rank, world):
     launches = m.launch_count - l0
     clocks = sampler.stop(t_start, t_end) if sampler else None
     fps = world * B * n_pass / (ms * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["out"])
     fps_skip = None
     if sharp:
         n_skip = max(3, n_pass // 4)
@@ -498,17 +498,10 @@ def run_gpu(args, rank, local_rank, world):
             for name, cat, t, fl, by in rows[:len(rows) // nprof]:
                 f.write(f"{name}\t{cat}\t{t:.4f}\t{fl / 1e9:.2f}\t{by / 1e6:.1f}\t{fl / (t * 1e-3) / 1e12:.1f}\t"
                         f"{by / (t * 1e-3) / 1e9:.0f}\n")
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", args.traffic_file)
-    if os.path.exists(tpath) and args.precision == "exact" and B == 64 and S == 255 and sharp:
-        tj = json.load(open(tpath))           # ncu dram__bytes_read+write of the family's launches in one step
-        traffic = {"bytes_per_step": tj["conv_gemm_traffic_bytes_per_step"],
-                   "launches_per_step": tj["conv_gemm_launches_per_step"], "measured_in_run": False,
-                   "source": f"profiles/{args.traffic_file} (committed ncu capture of this command, not measured in this run)"}
     roofline = {
-        "bound": "tensor", "kernel": "conv_gemm_kernel (tcgen05 implicit-GEMM conv family, all layers of one step)",
+        "bound": "tensor", "kernel": "conv_gemm_kernel (wgmma implicit-GEMM conv family, all layers of one step)",
         "achieved": achieved, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": achieved / peaks["tflops"],
-        "peak_source": peaks["src"] + ", sustained cuBLAS bf16", "traffic": traffic,
+        "peak_source": peaks["src"],
         "algorithmic_bytes_per_step": gemm["bytes"],
         # the parity mode issues 3 fp16 MMAs per algorithmic MAC: tensor-pipe work actually executed vs the same peak
         "mma_issued_frac": (3.0 if args.precision == "exact" else 1.0) * achieved / peaks["tflops"],
@@ -548,13 +541,11 @@ def run_gpu(args, rank, local_rank, world):
         "metric": metric_name(args), "value": fps, "unit": "frames/s", "n_gpus": world, "steps": args.steps,
         "warmup": warm, "ms_per_step": ms / n_pass, "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None,
-        "dtype": "f16x3 (hi+lo split fp16 operands on tcgen05, f32 accumulate; f32 CUDA-core stem/xcorr/refine)"
-                 if args.precision == "exact" else "f16 (single-pass tcgen05, f32 accumulate)",
+        "dtype": "f16x3 (hi+lo split fp16 operands on wgmma, f32 accumulate; f32 CUDA-core xcorr/refine)"
+                 if args.precision == "exact" else "f16 (single-pass wgmma, f32 accumulate)",
         "data": "synthetic", "config": workload_config(args, B, world),
         "precision_mode": args.precision,
-        "passes_per_step": passes, "timed_region_s": ms * 1e-3,
-        "timing_note": f"the timed region covers steps x passes_per_step = {n_pass} passes over a batch "
-                       f"(>= {args.min_seconds} s); ms_per_step and value are per pass",
+        "timed_region_s": ms * 1e-3,
         "algorithmic_tflops": fps * gfl / 1e3,
         "value_skip_dead_mask_head": fps_skip,
         "e2e": {"value": e2e_fps, "unit": "frames/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
@@ -585,6 +576,22 @@ def run_gpu(args, rank, local_rank, world):
     print(json.dumps(result))
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(path, out):
+    """What the last timed step handed its caller (Custom.step's dict): cls, loc, best, pos, records, refine as float32 /
+    float64 (int32 indices) arrays; the B x 3969 x R x R mask-head tensor as a fixed seeded sample of 2^20 of its
+    elements (mask_sample.npy, flat indices from numpy's default_rng(0), sorted)."""
+    os.makedirs(path, exist_ok=True)
+    for name, t in out.items():
+        if t is None:
+            continue
+        a = t.detach().cpu().numpy()
+        if name == "mask":
+            flat = a.reshape(-1)
+            idx = np.sort(np.random.default_rng(0).integers(0, flat.size, size=min(flat.size, 1 << 20)))
+            a, name = flat[idx], "mask_sample"
+        np.save(os.path.join(path, name + ".npy"), a.astype(np.float64 if a.dtype.kind in "iu" else np.float32))
 
 
 def tracker_loop_rate(args, m, B, dev, seconds=1.5):
@@ -676,7 +683,8 @@ def main():
     ap.add_argument("--precision", default="exact", choices=["exact", "fast"])
     ap.add_argument("--rpn-only", action="store_true", default=None,
                     help="SiamRPN-only engine (experiments/siamrpn_resnet): step = track -> cls/loc")
-    ap.add_argument("--min-seconds", type=float, default=2.0, help="minimum length of every timed region")
+    ap.add_argument("--min-seconds", type=float, default=2.0,
+                    help="minimum length of the e2e and loop timed regions (value times exactly --steps steps)")
     ap.add_argument("--ref-batch", type=int, default=2, help="frames per step of each CPU reference worker")
     ap.add_argument("--cpu-threads", type=int, default=0, help="torch threads per CPU worker (0 = pick)")
     ap.add_argument("--cpu-seconds", type=float, default=10.0, help="length of the cpu_baseline sample")
@@ -684,7 +692,8 @@ def main():
     ap.add_argument("--no-context", action="store_true", help="skip the PyTorch/cuDNN context leg")
     ap.add_argument("--no-loop", action="store_true", help="skip the whole-tracker-loop leg")
     ap.add_argument("--no-verify", dest="verify", action="store_false", help="skip the oracle parity check")
-    ap.add_argument("--traffic-file", default="r02_traffic.json")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs to DIR/<name>.npy (seeded inputs: identical every run)")
     ap.add_argument("--dump-layers", default=None, help="write the per-launch CUDA-event table of one step here")
     # internal (cpu worker processes)
     ap.add_argument("--threads", type=int, default=8)

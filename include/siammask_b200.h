@@ -1,4 +1,4 @@
-/* siammask_b200 — C ABI of the B200-native SiamMask per-frame inference hot path.
+/* siammask_b200 — C ABI of the H100-native SiamMask per-frame inference hot path.
  *
  * The reference (foolwood/SiamMask) has no FFI for this path: the boundary is the duck-typed Python
  * object `state['net']` used by tools/test.py (siamese_init :155, siamese_track :201,203,257).  The entry
@@ -27,7 +27,7 @@ typedef struct sm_engine sm_engine;
 
 enum { SM_PRECISION_EXACT = 0, /* fp16 hi+lo operands, 3 tensor-core MMAs per k-step: fp32-class results */
        SM_PRECISION_FAST = 1   /* single fp16 MMA per k-step */ };
-enum { SM_BACKEND_TENSOR = 0,  /* tcgen05 implicit-GEMM convolutions */
+enum { SM_BACKEND_TENSOR = 0,  /* wgmma implicit-GEMM convolutions */
        SM_BACKEND_SIMT = 1     /* CUDA-core reference convolutions (debug / bisecting only) */ };
 enum { SM_TRACK_MASK_FEATURES = 1, /* keep p0/p1/p2 + mask corr feature for sm_refine (track_mask) */
        SM_TRACK_MASK_HEAD = 2      /* also evaluate the 256->3969 mask head (dead under --refine) */ };

@@ -22,8 +22,7 @@ The reference holds no tests and no golden vectors for this path (SURVEY §4),
 so the oracle is pinned the other way round: `oracle/make_golden.py` imports
 the *unmodified* reference model from /root/reference, runs it on a seeded
 checkpoint and commits its outputs under `tests/golden/`; `tests/test_oracle.py`
-checks this restatement against those vectors (and, when /root/reference is
-present, against the live reference model).
+checks this restatement against those vectors.
 
 The arithmetic itself (conv / batch-norm / max-pool / nearest upsample) lives
 in PyTorch, which the reference pins as torch==0.4.1 (requirements.txt); here it

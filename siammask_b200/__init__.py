@@ -1,4 +1,4 @@
-"""siammask_b200 — B200-native (sm_100a) implementation of SiamMask's per-frame inference hot path.
+"""siammask_b200 — H100-native (sm_90a) implementation of SiamMask's per-frame inference hot path.
 
 Public surface mirrors the reference's model object for that path:
     Custom.template / track / track_mask / track_refine   (experiments/siammask_sharp/custom.py:173-190)

@@ -91,7 +91,7 @@ def load():
         return _lib
     from . import build as _build
     if not os.path.exists(LIB_PATH):
-        # a fresh checkout has sources only: compile the extension in-tree (nvcc, sm_100a) — there is no other
+        # a fresh checkout has sources only: compile the extension in-tree (nvcc, sm_90a) — there is no other
         # implementation to fall back to, so a failed build is a hard error
         try:
             _build.build(force=True)

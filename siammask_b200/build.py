@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA extension: nvcc -> siammask_b200/libsiammask_b200.so (sm_100a only)."""
+"""In-tree build of the CUDA extension: nvcc -> siammask_b200/libsiammask_b200.so (sm_90a only)."""
 from __future__ import annotations
 
 import os
@@ -9,9 +9,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsiammask_b200.so")
-SOURCES = ["conv_gemm_sm100.cu", "conv3x3_patch_sm100.cu", "stem_sm100.cu", "simt_kernels.cu", "xcorr_bulk_sm100.cu", "engine.cu"]
+SOURCES = ["conv_gemm_sm90.cu", "conv3x3_patch_sm90.cu", "stem_sm90.cu", "simt_kernels.cu", "xcorr_bulk.cu", "engine.cu"]
 HEADERS = ["common.cuh", "ptx.cuh", os.path.join("..", "..", "include", "siammask_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 

@@ -1,4 +1,4 @@
-// Shared types for the SiamMask hot-path kernels (sm_100a).
+// Shared types for the SiamMask hot-path kernels (sm_90a).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -50,7 +50,7 @@ __device__ __forceinline__ void flag_if_out_of_range(float absmax, int* ovf) {
   if (ovf != nullptr && !(absmax <= 65504.f)) atomicOr(ovf, 1);
 }
 
-// One K-segment of the implicit GEMM (see conv_gemm_sm100.cu).
+// One K-segment of the implicit GEMM (see conv_gemm_sm90.cu).
 struct GemmSegment {
   CUtensorMap tmA[2];  // hi / lo plane.  kind 0, mode 0: 2D [M][Cin]; mode 1: im2col over NHWC; kind 1: residual [M][Cout]
   int kind;            // 0: convolution segment, 1: identity (residual) segment
@@ -60,17 +60,14 @@ struct GemmSegment {
   int b_col0;          // first column of this segment inside the packed weight matrix
 };
 
-// Parameters of the tcgen05 implicit-GEMM convolution kernel (passed by value, __grid_constant__).
+// Parameters of the wgmma implicit-GEMM convolution kernel (passed by value, __grid_constant__).
 struct GemmParams {
   GemmSegment seg[2];
   int nseg;
   CUtensorMap tmB[2];   // weights: hi / lo, 2D [Cout_pad][w_ld], K-major
-  CUtensorMap tmOut[2]; // staged epilogue: output planes [M][Cout], box 32 cols x 32 rows, 64B swizzle
   int M, Cout, Ho, Wo;
   int n_tiles, m_tiles;
-  int staged;           // 1: epilogue goes smem -> TMA store (NHWC split outputs)
   int reverse_m;        // 1: walk the M tiles from the last to the first (see Engine::conv_into: L2 reuse)
-  int ncat;             // 1: exact mode issues A_hi x [B_hi; B_lo] as ONE MMA of N = 2*BLOCK_N (A_hi read from smem once)
   Epilogue ep;
 };
 
@@ -118,7 +115,7 @@ inline void ensure_dynamic_smem(K kernel, int bytes, unsigned long long& done_ma
 
 // ---- launchers (defined in the .cu files) ---------------------------------------------------
 
-// conv_gemm_sm100.cu : tensor-core implicit GEMM. nsplit = 1 (fast) or 2 planes (exact, 3 MMAs).
+// conv_gemm_sm90.cu : tensor-core implicit GEMM. nsplit = 1 (fast) or 2 planes (exact, 3 MMAs).
 bool gemm_conv_supported(const ConvGeom& g);
 void launch_gemm_conv(const Act& in, const ConvGeom& g, const __half* w_hi, const __half* w_lo, int cout_pad,
                       const Epilogue& ep, int nsplit, int num_sms, cudaStream_t st);
@@ -131,13 +128,13 @@ void launch_gemm_multi(const GemmInput* convs, int nconv, const Act* residual, i
 CUtensorMap make_map_tiled_nd(const __half* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                               const uint32_t* box, int swizzle_bytes);
 
-// conv3x3_patch_sm100.cu : 3x3 / s1 / p1 / Cin == Cout in {64, 128} on a resident input patch (no im2col traffic)
+// conv3x3_patch_sm90.cu : 3x3 / s1 / p1 / Cin == Cout in {64, 128} on a resident input patch (no im2col traffic)
 int patch_conv_mode();
 bool patch_conv_supported(const Act& in, const ConvGeom& g);
 void launch_conv3x3_patch(const Act& in, const ConvGeom& g, const __half* w_hi, const __half* w_lo, int w_ld,
                           const Epilogue& ep, int nsplit, int num_sms, cudaStream_t st);
 
-// stem_sm100.cu : 7x7/2 stem on the tensor cores (weights [64][192] K-major, k = (r*7+s)*3+c, pow2-scaled)
+// stem_sm90.cu : 7x7/2 stem on the tensor cores (weights [64][192] K-major, k = (r*7+s)*3+c, pow2-scaled)
 void launch_stem_tc(const float* x_nchw, int B, int S, const __half* w_hi, const __half* w_lo, const float* alpha,
                     const float* beta, Act out, int num_sms, cudaStream_t st, int* ovf = nullptr);
 

@@ -187,7 +187,7 @@ class Engine {
 
   sm_config cfg_;
   bool exact_;
-  int num_sms_ = 148;
+  int num_sms_ = 132;
   int R_ = 0;                          // response size (score_size)
   std::map<std::string, ConvW> layers_;
   std::vector<std::string> layer_order_;
@@ -536,8 +536,8 @@ void Engine::construct(const sm_config& cfg) {
   SMK_CUDA(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   SMK_CUDA(cudaGetDeviceProperties(&prop, dev));
-  SMK_CHECK(prop.major == 10, "siammask_b200 kernels are built for sm_100a only (found sm_" +
-                                  std::to_string(prop.major) + std::to_string(prop.minor) + ")");
+  SMK_CHECK(prop.major == 9 && prop.minor == 0, "siammask_b200 kernels are built for sm_90a only (found sm_" +
+                                                    std::to_string(prop.major) + std::to_string(prop.minor) + ")");
   num_sms_ = prop.multiProcessorCount;
   R_ = (cfg.search_size - 127) / 8 + 1 + 8;   // utils/tracker_config.py:23,46 with base_size 8
 
@@ -1765,7 +1765,7 @@ static void conv2d_op(const float* x, const float* w, const float* scale, const 
   ep.relu = relu;
   ep.out_mode = OUT_NCHW_F32;
   ep.out_f32 = out;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   SMK_CUDA(cudaGetDevice(&dev));
   SMK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   (void)Ho; (void)Wo;
@@ -1815,7 +1815,7 @@ struct sm_engine {
 extern "C" {
 
 const char* sm_last_error(void) { return smk::g_last_error.c_str(); }
-const char* sm_version(void) { return "siammask_b200 0.1 (sm_100a)"; }
+const char* sm_version(void) { return "siammask_b200 0.1 (sm_90a)"; }
 
 int sm_engine_create(const sm_config* cfg, sm_engine** out) {
   SM_API_BEGIN

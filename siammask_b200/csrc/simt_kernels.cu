@@ -1,7 +1,7 @@
-// CUDA-core kernels of the SiamMask hot path (sm_100a): everything that is not a dense contraction
+// CUDA-core kernels of the SiamMask hot path (sm_90a): everything that is not a dense contraction
 // large enough for the tensor pipe — the 3-channel 7x7 stem, max-pool, the bandwidth-bound depthwise
 // cross-correlation, the crops/gathers of the refine stage, its 1-32 channel 3x3 convs and the
-// 1x1 -> 15x15 transposed conv — plus a plain reference convolution used to bisect the tcgen05 path.
+// 1x1 -> 15x15 transposed conv — plus a plain reference convolution used to bisect the tensor-core path.
 #include "common.cuh"
 
 #include <cmath>
@@ -189,7 +189,7 @@ __global__ void maxpool_kernel(Act in, Act out) {
 // fp32 in shared memory once (each element is read from L2 exactly once), then every thread (channel, output
 // row) slides a KHxKW window along the row out of smem.  Lanes are consecutive channels: conflict-free LDS and
 // contiguous 64-byte stores per plane.
-// Register-blocked variant (same mapping idea as xcorr_bulk_sm100.cu): lane = channel (32 consecutive channels of one
+// Register-blocked variant (same mapping idea as xcorr_bulk.cu): lane = channel (32 consecutive channels of one
 // stream: every shared-memory access of a warp is one conflict-free 128-byte row), and a thread owns a
 // (row block x column strip) task of NR x SW outputs: per input row SW+KW-1 loads feed NR..KH*SW*KW FMAs.  The tile
 // is reconstructed to fp32 in shared memory once; 2 blocks per SM so one block's load phase overlaps the other's math.
@@ -683,6 +683,28 @@ __global__ void __launch_bounds__(256) small_conv3x3_kernel(const float* __restr
 // the penalty is evaluated in fp64 (numpy promotes those expressions to float64 through the float64 target size).
 // np.argmax semantics incl. NaN: the first NaN wins over every number (a NaN/Inf network output or a 0/0 target
 // size must not leave `besti` unset: rec/pos are always in range).  rec[7] = best index (exact in fp32).
+// float32 exp evaluated the way numpy's SIMD float32 np.exp does it: Cody-Waite reduction by round(x*log2(e))*ln2,
+// a (5,2) rational polynomial with FMAs, one division, scaling by 2^q.  The reference's box sizes are np.exp of the
+// float32 loc values (:211-212) and the tracker feeds them back into every later crop scale, so they must round the
+// same way: CUDA's expf differs from it by an ulp on ~40 % of inputs, and a jump of a few hundred pixels turns that
+// into a 1e-5 px position error.
+__device__ __forceinline__ float np_expf(float x) {
+  if (x != x) return x;
+  if (x >= 88.72283935546875f) return INFINITY;
+  if (x <= -103.97208404541015625f) return 0.f;
+  const float q = rintf(__fmul_rn(x, 1.442695040888963407359924681001892137f));
+  float r = __fmaf_rn(q, -6.93145752e-1f, x);
+  r = __fmaf_rn(q, -1.42860677e-6f, r);
+  float n = __fmaf_rn(5.082762527590693718096e-04f, r, 6.757896990527504603057e-03f);
+  n = __fmaf_rn(n, r, 5.114512081637298353406e-02f);
+  n = __fmaf_rn(n, r, 2.473615434895520810817e-01f);
+  n = __fmaf_rn(n, r, 7.257664613233124478488e-01f);
+  n = __fmaf_rn(n, r, 9.999999999980870924916e-01f);
+  float d = __fmaf_rn(2.159509375685829852307e-02f, r, -2.742335390411667452936e-01f);
+  d = __fmaf_rn(d, r, 1.0f);
+  return ldexpf(__fdiv_rn(n, d), static_cast<int>(q));
+}
+
 constexpr int SEL_THREADS = 512;   // latency-bound (fp64 exp / divides per candidate): more threads, fewer serial candidates each
 __global__ void __launch_bounds__(SEL_THREADS) select_kernel(const float* __restrict__ cls, const float* __restrict__ loc,
                                                      const float* __restrict__ anchors,
@@ -714,8 +736,8 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(const float* __rest
     const float e0 = expf(s0 - m), e1 = expf(s1 - m);
     const float score = e1 / (e0 + e1);
     const float aw = anchors[4 * idx + 2], ah = anchors[4 * idx + 3];
-    const float w = expf(l[(size_t)(2 * A + a) * RR + p]) * aw;
-    const float h = expf(l[(size_t)(3 * A + a) * RR + p]) * ah;
+    const float w = __fmul_rn(np_expf(l[(size_t)(2 * A + a) * RR + p]), aw);
+    const float h = __fmul_rn(np_expf(l[(size_t)(3 * A + a) * RR + p]), ah);
     const float pad = (w + h) * 0.5f;
     const float sz = sqrtf((w + pad) * (h + pad));
     double sc = (double)sz / tsz_c;
@@ -754,16 +776,18 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(const float* __rest
     const float m = fmaxf(s0, s1);
     const float e0 = expf(s0 - m), e1 = expf(s1 - m);
     const float score = e1 / (e0 + e1);
-    const float w = expf(l[(size_t)(2 * A + a) * RR + p]) * aw;
-    const float h = expf(l[(size_t)(3 * A + a) * RR + p]) * ah;
+    const float w = __fmul_rn(np_expf(l[(size_t)(2 * A + a) * RR + p]), aw);
+    const float h = __fmul_rn(np_expf(l[(size_t)(3 * A + a) * RR + p]), ah);
     const float pad = (w + h) * 0.5f;
     double sc = (double)sqrtf((w + pad) * (h + pad)) / tsz_c;
     sc = fmax(sc, 1.0 / sc);
     double rc = tratio / (double)(w / h);
     rc = fmax(rc, 1.0 / rc);
     float* o = rec + 8 * b;
-    o[0] = l[(size_t)a * RR + p] * aw + ax;
-    o[1] = l[(size_t)(A + a) * RR + p] * ah + ay;
+    // delta * anchor_wh + anchor_xy with the product rounded before the add, as numpy evaluates it (:209-210); a
+    // contracted FMA rounds once and moves the box centre by up to one float32 ulp
+    o[0] = __fadd_rn(__fmul_rn(l[(size_t)a * RR + p], aw), ax);
+    o[1] = __fadd_rn(__fmul_rn(l[(size_t)(A + a) * RR + p], ah), ay);
     o[2] = w;
     o[3] = h;
     o[4] = score;
@@ -930,7 +954,9 @@ __global__ void tracker_update_kernel(int B, double* __restrict__ state, const f
   const double lr = penalty * (double)score * hp.lr;            // :241
   const double p0 = (double)r[0] / scale_x, p1 = (double)r[1] / scale_x, p2 = (double)w / scale_x, p3 = (double)h / scale_x;
   double res_x = p0 + px, res_y = p1 + py;
-  double res_w = sw * (1.0 - lr) + p2 * lr, res_h = sh * (1.0 - lr) + p3 * lr;
+  // both products rounded before the sum, as numpy evaluates them (:245-246; no FMA contraction)
+  double res_w = __dadd_rn(__dmul_rn(sw, 1.0 - lr), __dmul_rn(p2, lr));
+  double res_h = __dadd_rn(__dmul_rn(sh, 1.0 - lr), __dmul_rn(p3, lr));
   const double im_w = imsize[2 * b], im_h = imsize[2 * b + 1];
   if (maps != nullptr) {
     // crop_back mapping of the refined / head mask into the frame (:263-282)
@@ -1052,9 +1078,9 @@ small_conv3x3_tiled_kernel(const float* __restrict__ a, const float* __restrict_
 inline int device_sms() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   int& c = cached[dev & 63];
-  if (c == 0 && cudaDeviceGetAttribute(&c, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) c = 148;
+  if (c == 0 && cudaDeviceGetAttribute(&c, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) c = 132;
   return c;
 }
 inline int grid_for(size_t total, int block) {
@@ -1110,7 +1136,7 @@ void launch_xcorr_nhwc(const Act& x, int c_off, const __half* k_hi, const __half
 void launch_xcorr_nchw_f32(const float* x, const float* k, float* out, int planes, int H, int W, int kh, int kw,
                            cudaStream_t st) {
   SMK_CHECK(H >= kh && W >= kw && planes > 0, "xcorr shapes");
-  // bulk-copy pipeline (xcorr_bulk_sm100.cu) for whole tiles of planes; the one-warp-per-plane kernel takes the rest
+  // bulk-copy pipeline (xcorr_bulk.cu) for whole tiles of planes; the one-warp-per-plane kernel takes the rest
   static const bool no_bulk = getenv("SMB200_XCORR_NO_BULK") != nullptr;
   const int done = no_bulk ? 0 : launch_xcorr_bulk_f32(x, k, out, planes, H, W, kh, kw, st);
   if (done >= planes) return;

@@ -8,7 +8,7 @@ experiments/siamrpn_resnet/custom.py:81-93) as used by the tracker loop in tools
     main          :560-569   Custom(anchors=cfg['anchors']); load_pretrain(model, path); model.eval().to(device)
 
 Python here is plumbing only: tensors in, tensors out, every FLOP happens in libsiammask_b200.so
-(hand-written sm_100a kernels) reached through the C ABI in include/siammask_b200.h.
+(hand-written sm_90a kernels) reached through the C ABI in include/siammask_b200.h.
 
 Batched extension (not in the reference, SURVEY §8b): every method accepts B>1 *paired* templates/searches
 bound to engine slots slot0..slot0+B-1, and `track_refine` additionally accepts an int tensor/array [B,2]
@@ -100,7 +100,7 @@ class Custom:
     def to(self, device):
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("siammask_b200 runs on CUDA (sm_100a) devices only; there is no CPU path")
+            raise RuntimeError("siammask_b200 runs on CUDA (sm_90a) devices only; there is no CPU path")
         if device.index is None:
             device = torch.device("cuda", torch.cuda.current_device())
         if self._engine.value and self._device == device:

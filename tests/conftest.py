@@ -13,7 +13,7 @@ warnings.filterwarnings("ignore", category=UserWarning)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_100a) device")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_90a) device")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -1,4 +1,4 @@
-"""Parity at the shapes the benchmark actually runs (VERDICT r01 "missing 1"): the B=64 default tile / CTA-pair /
+"""Parity at the shapes the benchmark actually runs (VERDICT r01 "missing 1"): the B=64 default tile /
 two-lane path, the sharp path at search 383 (R=41), SiamRPN-only at B=256, and the fused frame entry points
 `sm_step` / `sm_step_host_async`.  All against the CPU oracle / the reference goldens, tolerance 1e-3."""
 import ctypes as C
@@ -57,8 +57,8 @@ def _check_stream(o, out, b, z, x, a, w, tsz, sharp=True, mask_head=True):
 
 
 def test_b64_default_path_matches_oracle(calib_sd):
-    """BASELINE configs[1] exactly as bench.py runs it: B=64, default env (wide / CTA-pair tiles where the launcher
-    picks them, two lanes of 32), one `sm_step` per frame incl. the mask head; streams at both ends of both lanes."""
+    """BASELINE configs[1] exactly as bench.py runs it: B=64, default env (the tiles the launcher
+    picks, two lanes of 32), one `sm_step` per frame incl. the mask head; streams at both ends of both lanes."""
     B = 64
     z, x = synthetic_inputs(71, B)
     a, w, tsz = _consts(25, B)

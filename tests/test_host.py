@@ -26,7 +26,7 @@ def test_library_exports_every_declared_symbol():
     for s in syms:
         assert hasattr(lib, s), f"{s} declared in include/siammask_b200.h but not exported"
     assert set(syms) == set(_lib.SIGNATURES), "ctypes prototypes out of sync with the header"
-    assert b"sm_100a" in _lib.load().sm_version()
+    assert b"sm_90a" in _lib.load().sm_version()
 
 
 def test_ctypes_struct_layouts_match_the_header(tmp_path):

@@ -1,7 +1,6 @@
 """The oracle against (i) the golden vectors produced by the unmodified reference (oracle/make_golden.py),
-(ii) the live reference model when /root/reference is present, (iii) independent plain-loop restatements."""
+(ii) independent plain-loop restatements."""
 import os
-import sys
 
 import numpy as np
 import pytest
@@ -12,7 +11,6 @@ from conftest import GOLDEN, assert_close
 from oracle.calibrate import synthetic_inputs
 from oracle.siammask_oracle import Oracle, nearest_upsample_index, xcorr_depthwise_loops
 
-REF = "/root/reference"
 # The golden vectors were produced on the build container's CPU.  The calibrated checkpoint is regenerated
 # from its seed wherever the tests run; a different CPU (other conv kernels in the calibration pass) moves
 # BN statistics by ~1e-7 and this seeded network amplifies perturbations ~100x, hence 1e-3 here.
@@ -108,18 +106,16 @@ def test_per_stream_refine_equals_per_sample_loop(calib_sd):
         assert_close(both[b:b + 1], o1.track_refine(pos), 1e-4, f"refine stream {b}")
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present on this box")
 def test_oracle_matches_live_reference(calib_sd):
-    sys.path[:0] = [REF, os.path.join(REF, "experiments", "siammask_sharp")]
-    from custom import Custom
-    m = Custom(anchors={"stride": 8, "ratios": [0.33, 0.5, 1, 2, 3], "scales": [8], "round_dight": 0}).eval()
-    m.load_state_dict(calib_sd, strict=False)
+    """Against the reference model's outputs on a further seed (oracle/make_golden.py::live_reference_golden).  Kept at
+    the 1e-4 this comparison had when it ran the reference model live; a host whose calibration pass moves the BN
+    statistics (see GOLDEN_TOL) would show up here first."""
+    g = _g("sharp_b1_s255_seed11.npz")
     z, x = synthetic_inputs(11, 1)
     o = Oracle(calib_sd)
     with torch.no_grad():
-        m.template(z); o.template(z)
-        ref = m.track_mask(x)
-        got = o.track_mask(x)
-        for a, b, n in zip(got, ref, ("cls", "loc", "mask")):
+        o.template(z)
+        cls, loc, mask = o.track_mask(x)
+        for a, b, n in ((cls, g["cls"], "cls"), (loc, g["loc"], "loc"), (mask[:, MASK_CH], g["mask_sub"], "mask")):
             assert_close(a, b, 1e-4, n + " vs live reference")
-        assert_close(o.track_refine((0, 24)), m.track_refine((0, 24)), 1e-4, "refine vs live reference")
+        assert_close(o.track_refine((0, 24)), g["refine_0_24"], 1e-4, "refine vs live reference")
