@@ -129,7 +129,6 @@ CUtensorMap make_map_tiled_nd(const __half* base, int rank, const uint64_t* dims
                               const uint32_t* box, int swizzle_bytes);
 
 // conv3x3_patch_sm90.cu : 3x3 / s1 / p1 / Cin == Cout in {64, 128} on a resident input patch (no im2col traffic)
-int patch_conv_mode();
 bool patch_conv_supported(const Act& in, const ConvGeom& g);
 void launch_conv3x3_patch(const Act& in, const ConvGeom& g, const __half* w_hi, const __half* w_lo, int w_ld,
                           const Epilogue& ep, int nsplit, int num_sms, cudaStream_t st);

@@ -266,12 +266,6 @@ void launch_patch(const PatchParams& p, int num_sms, cudaStream_t st) {
 
 }  // namespace
 
-// SMB200_PATCH3X3: 0 = off (im2col kernel everywhere), 1 = on (default)
-int patch_conv_mode() {
-  static const int mode = [] { const char* e = getenv("SMB200_PATCH3X3"); return e ? atoi(e) : 1; }();
-  return mode;
-}
-
 bool patch_conv_supported(const Act& in, const ConvGeom& g) {
   if (!(g.KH == 3 && g.KW == 3 && g.stride == 1 && g.pad == 1 && g.dil == 1 && g.Cin == g.Cout)) return false;
   if (!(g.Cin == 64 || g.Cin == 128)) return false;

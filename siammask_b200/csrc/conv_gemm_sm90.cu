@@ -334,8 +334,6 @@ template <typename F>
 CUtensorMap cached_map(const MapKey& key, F&& encode) {
   static std::mutex mu;
   static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> cache;
-  static const bool off = getenv("SMB200_NO_MAP_CACHE") != nullptr;
-  if (off) return encode();
   int dev = 0;
   cudaGetDevice(&dev);
   MapKey k = key;

@@ -85,17 +85,17 @@ struct Arena {
   }
 };
 
-// One execution lane: its own workspace, stream set and cached per-step tensors.  A batch of >= 2 * kLaneMinB streams
-// is split over two (SMB200_LANES: up to kMaxLanes) lanes that run concurrently (streams are independent): the persistent GEMM kernels of one lane
-// fill the SMs the other lane's kernels leave idle in their last wave and in the low-occupancy refine tail.
+// One execution lane: its own workspace and stream set.  A batch of >= 2 * kLaneMinB streams is split over two lanes
+// that run concurrently (streams are independent): the persistent GEMM kernels of one lane fill the SMs the other
+// lane's kernels leave idle in their last wave and in the low-occupancy refine tail.
 struct Lane {
+  int id = 0;                                  // index of the lane's tensors in CallState::named
   Arena search, refine;
-  std::map<std::string, Act> named;            // p0, p1, p2, search, corr_* of the lane's last track
   cudaStream_t own = nullptr;                  // the lane's main stream (lane 0 runs on the caller's stream in the device-pointer API)
   cudaStream_t aux[3] = {nullptr, nullptr, nullptr};
   int cap_B = 0;                               // largest batch this lane's arenas were sized for
 };
-constexpr int kMaxLanes = 4;
+constexpr int kMaxLanes = 2;
 constexpr int kLaneMinB = 8;                   // a lane gets at least this many streams (below 2 x 8: one lane)
 
 }  // namespace
@@ -142,6 +142,7 @@ class Engine {
   int64_t launches() const { return launches_; }
   size_t bytes() const { return total_bytes_; }
   const sm_config& cfg() const { return cfg_; }
+  int score_size() const { return R_; }
 
  private:
   // ---- construction
@@ -149,8 +150,7 @@ class Engine {
   ConvW& add_layer(const std::string& conv_key, const std::string& bn_key, ConvGeom g);
   void build_layer_table();
   void assign_blob_layout();
-  size_t measure_arena(int B, int S, bool search);
-  size_t refine_arena_bytes(int B) const;
+  void size_arenas();
   // ---- packing
   void fold_layer(ConvW& L, const std::map<std::string, const sm_tensor_desc*>& sd, uint8_t* host);
   void quantize_layer(ConvW& L, uint8_t* host);
@@ -171,7 +171,7 @@ class Engine {
   void conv_into(const Act& in, const ConvW& L, Epilogue ep, cudaStream_t st, const Act* res = nullptr,
                  const Act* in2 = nullptr);
   F32T conv_f32(const Act& in, const ConvW& L, bool relu, Arena& ar, cudaStream_t st);
-  Act backbone(const float* x, int B, int S, Arena& ar, bool keep, cudaStream_t st);
+  Act backbone(const float* x, int B, int S, Arena& ar, std::map<std::string, Act>* keep, cudaStream_t st);
   F32T small(const F32T& a, const F32T* b, int Ho, const ConvW& L, bool relu, float* out_override, Arena& ar,
              cudaStream_t st);
   const ConvW& L(const std::string& k) const {
@@ -215,10 +215,7 @@ class Engine {
 
   Arena templ_arena_;
   Lane lanes_[kMaxLanes];
-  Lane* cur_ = &lanes_[0];             // lane whose schedule is being enqueued
-  int n_lanes_ = 1;                    // SMB200_LANES (default 2), capped by max_batch / kLaneMinB
-  int split_n_ = 1;                    // how the last track divided its batch: lane l got streams
-  int split_off_[kMaxLanes + 1] = {0, 0, 0, 0, 0};   //   [split_off_[l], split_off_[l + 1])
+  int n_lanes_ = 1;                    // kMaxLanes, capped by max_batch / kLaneMinB
   // per-slot template caches: [branch][slot][5][5][256] split planes, and zf for export
   __half* kcache_hi_ = nullptr;
   __half* kcache_lo_ = nullptr;
@@ -235,20 +232,26 @@ class Engine {
   int32_t* stage_best_[2] = {nullptr, nullptr};
   float* stage_maskcol_[2] = {nullptr, nullptr};
   float* mask_raw_ = nullptr;          // [max_batch][3969][R][R] raw mask-head output of the host-buffer step (lazy)
-  void step_lane(int slot0, int B, const StepIO& io, cudaStream_t st);
+  void step_lane(Lane& ln, int slot0, int B, const StepIO& io, cudaStream_t st);
   void release();
   cudaStream_t h2d_stream_ = nullptr, d2h_stream_ = nullptr;
-  cudaEvent_t h2d_done_[2] = {nullptr, nullptr}, compute_done_[2] = {nullptr, nullptr}, d2h_done_[2] = {nullptr, nullptr};
+  cudaEvent_t h2d_done_[2] = {nullptr, nullptr}, d2h_done_[2] = {nullptr, nullptr};
   bool set_busy_[2] = {false, false};
   uint64_t host_calls_ = 0;
   int* maps_dev_ = nullptr;
   std::map<int, const int*> maps_;
 
-  // state of the last track (Custom.feature / .search / .corr_feature, custom.py:182-184)
   Act zf_;                             // template feature of the last sm_template (export)
   bool have_zf_ = false;
-  int last_B_ = 0;
-  bool have_mask_feats_ = false;
+  // state of the last track (Custom.feature / .search / .corr_feature, custom.py:182-184), read by refine / export
+  struct CallState {
+    std::map<std::string, Act> named[kMaxLanes];   // per lane: p0, p1, p2, search, corr_* of its share of the batch
+    int split_n = 1;                               // lane l got streams [split_off[l], split_off[l + 1])
+    int split_off[kMaxLanes + 1] = {};
+    int last_B = 0;
+    bool have_mask_feats = false;
+  };
+  CallState state_;
 
   int64_t launches_ = 0;
   size_t total_bytes_ = 0;
@@ -269,21 +272,14 @@ class Engine {
   struct GraphEntry {
     int seen = 0;
     cudaGraphExec_t exec = nullptr;
-    std::map<std::string, Act> named[kMaxLanes];
-    int split_n = 1;
-    int split_off[kMaxLanes + 1] = {0, 0, 0, 0, 0};
-    int last_B = 0;
-    bool have_mask_feats = false;
+    CallState state;
     int64_t launches = 0;
   };
   bool use_graphs_ = false;
   std::map<std::vector<uint64_t>, GraphEntry> graphs_;
-  void track_impl(int slot0, int B, const float* x, float* cls, float* loc, float* mask, int flags, cudaStream_t st);
-  void track_lane(int slot0, int B, const float* x, float* cls, float* loc, float* mask, int flags, cudaStream_t st);
-  void refine_impl(int B, const int32_t* pos, float* out, cudaStream_t st);
-  void refine_lane(int B, const int32_t* pos, float* out, cudaStream_t st);
-  bool defer_join_ = false;            // host-buffer path: lane 1 stays forked between its track and its refine
-  bool lane1_forked_ = false;          // lanes 1.. are forked from the caller's stream and not joined back yet
+  void track_lane(Lane& ln, int slot0, int B, const float* x, float* cls, float* loc, float* mask, int flags,
+                  cudaStream_t st);
+  void refine_lane(Lane& ln, int B, const int32_t* pos, float* out, cudaStream_t st);
   // host-buffer path with two lanes: both lanes run on their own streams and are never joined into the caller's
   // stream — each only waits for its inputs, the D2H waits for both — so consecutive steps of the two lanes slide
   // against each other.  The next stream-ordered entry point (template / track / refine / export) joins them.
@@ -300,45 +296,29 @@ class Engine {
     // per-launch profiling (bench.py roofline) times every layer as ONE launch over the whole batch: per-kernel
     // durations are not defined while two lanes interleave, and half-batch launches timed back to back would charge
     // each kernel the idle last wave that the other lane fills in the real schedule
-    split_n_ = (profiling_ || calibrating_) ? 1 : lanes_for(n_lanes_, B);
-    split_off_[0] = 0;
-    for (int l = 0; l < split_n_; ++l) {
-      split_off_[l + 1] = split_off_[l] + chunk(B, split_n_, l);
-      SMK_CHECK(chunk(B, split_n_, l) <= lanes_[l].cap_B, "lane workspace too small for this batch");
+    CallState& s = state_;
+    s.split_n = (profiling_ || calibrating_) ? 1 : lanes_for(n_lanes_, B);
+    s.split_off[0] = 0;
+    for (int l = 0; l < s.split_n; ++l) {
+      s.split_off[l + 1] = s.split_off[l] + chunk(B, s.split_n, l);
+      SMK_CHECK(chunk(B, s.split_n, l) <= lanes_[l].cap_B, "lane workspace too small for this batch");
     }
   }
-  void fork_lanes(cudaStream_t st) {
-    if (split_n_ < 2 || !concurrent() || lane1_forked_) return;
-    for (int l = 1; l < split_n_; ++l) order_after(st, lanes_[l].own);
-    lane1_forked_ = true;
-  }
-  void join_forked(cudaStream_t st) {
-    if (!lane1_forked_) return;
-    for (int l = 1; l < n_lanes_; ++l) order_after(lanes_[l].own, st);
-    lane1_forked_ = false;
-  }
-  // if a schedule throws half way (arena exhausted, launch error), leave the lanes joined and lane 0 current
-  struct LaneGuard {
-    Engine* e; cudaStream_t st; bool armed = true;
-    ~LaneGuard() {
-      if (!armed) return;
-      e->cur_ = &e->lanes_[0];
-      e->defer_join_ = false;
-      try { e->join_forked(st); } catch (...) {}
-    }
-  };
+  static constexpr int kJoined = -1;   // run_lanes mode: joined into the caller's stream (else: decoupled, staging set)
+  template <typename F>
+  void run_lanes(cudaStream_t st, int set, F&& body);
+  struct Copy { void* dst; const void* src; size_t bytes; };   // one transfer of a host-buffer call (null: skipped)
+  int next_set();
+  template <typename Coupled, typename F>
+  int host_call(int t, int B, bool mask_feats, cudaStream_t st, std::initializer_list<Copy> h2d,
+                std::initializer_list<Copy> d2h, Coupled&& coupled, F&& body);
   template <typename F>
   void run_with_graph(const std::vector<uint64_t>& key, cudaStream_t st, F&& body) {
     if (!use_graphs_ || profiling_ || calibrating_) { body(); return; }
     GraphEntry& ge = graphs_[key];
     if (ge.exec != nullptr) {
       SMK_CUDA(cudaGraphLaunch(ge.exec, st));
-      for (int l = 0; l < kMaxLanes; ++l)
-        for (auto& kv : ge.named[l]) lanes_[l].named[kv.first] = kv.second;
-      split_n_ = ge.split_n;
-      for (int l = 0; l <= kMaxLanes; ++l) split_off_[l] = ge.split_off[l];
-      last_B_ = ge.last_B;
-      have_mask_feats_ = ge.have_mask_feats;
+      state_ = ge.state;
       launches_ += ge.launches;
       return;
     }
@@ -356,11 +336,7 @@ class Engine {
     SMK_CUDA(cudaStreamEndCapture(st, &graph));
     SMK_CUDA(cudaGraphInstantiate(&ge.exec, graph, 0));
     SMK_CUDA(cudaGraphDestroy(graph));
-    for (int l = 0; l < kMaxLanes; ++l) ge.named[l] = lanes_[l].named;
-    ge.split_n = split_n_;
-    for (int l = 0; l <= kMaxLanes; ++l) ge.split_off[l] = split_off_[l];
-    ge.last_B = last_B_;
-    ge.have_mask_feats = have_mask_feats_;
+    ge.state = state_;
     ge.launches = launches_ - l0;
     SMK_CUDA(cudaGraphLaunch(ge.exec, st));
   }
@@ -378,7 +354,7 @@ class Engine {
   bool concurrent() const { return !profiling_ && !calibrating_; }
   // make `to` wait for everything enqueued on `from` so far
   void order_after(cudaStream_t from, cudaStream_t to) {
-    if (from == to) return;
+    if (from == to || measuring_) return;
     cudaEvent_t e = next_sync_event();
     SMK_CUDA(cudaEventRecord(e, from));
     SMK_CUDA(cudaStreamWaitEvent(to, e, 0));
@@ -394,20 +370,24 @@ class Engine {
     SMK_CUDA(cudaEventCreate(&e));
     return e;
   }
-  struct Scope {
-    Engine* eng; cudaStream_t st; size_t idx; bool on;
-    Scope(Engine* e, const std::string& name, const char* cat, double flops, double bytes, cudaStream_t s)
-        : eng(e), st(s), idx(0), on(e->profiling_ && !e->measuring_) {
-      if (!on) return;
-      ProfRec r;
-      r.name = name; r.cat = cat; r.flops = flops; r.bytes = bytes;
-      r.e0 = eng->get_event(); r.e1 = eng->get_event();
-      cudaEventRecord(r.e0, st);
-      idx = eng->prof_.size();
-      eng->prof_.push_back(r);
+  // enqueue() issues n kernel launches on st.  Nothing happens while measuring (the arena dry runs); when profiling,
+  // the launches are timed as one row (name, category, flops, bytes) — an empty name means no row.
+  template <typename F>
+  void launch(cudaStream_t st, int n, const std::string& name, const char* cat, double flops, double bytes,
+              F&& enqueue) {
+    if (measuring_) return;
+    const bool row = profiling_ && !name.empty();
+    const size_t idx = prof_.size();
+    if (row) {
+      prof_.push_back(ProfRec{name, cat, flops, bytes, get_event(), get_event()});
+      cudaEventRecord(prof_[idx].e0, st);
     }
-    ~Scope() { if (on) cudaEventRecord(eng->prof_[idx].e1, st); }
-  };
+    enqueue();
+    if (row) cudaEventRecord(prof_[idx].e1, st);
+    launches_ += n;
+  }
+  template <typename F>
+  void launch(cudaStream_t st, int n, F&& enqueue) { launch(st, n, std::string(), nullptr, 0, 0, enqueue); }
 };
 
 // ================================================================================================
@@ -566,12 +546,7 @@ void Engine::construct(const sm_config& cfg) {
     deconv_b_ = reinterpret_cast<float*>(blob_ + off_deconv_b_);
   }
 
-  // workspace sizes: dry-run the schedule with a measuring arena
-  {
-    const char* e = std::getenv("SMB200_LANES");
-    const int want = e != nullptr ? std::max(1, std::min(kMaxLanes, atoi(e))) : 2;
-    n_lanes_ = lanes_for(want, cfg.max_batch);
-  }
+  n_lanes_ = lanes_for(kMaxLanes, cfg.max_batch);
   // the largest chunk each lane can be handed over all batch sizes this engine accepts (lane 0: the whole batch,
   // when profiling)
   lanes_[0].cap_B = cfg.max_batch;
@@ -579,16 +554,13 @@ void Engine::construct(const sm_config& cfg) {
     const int nl = lanes_for(n_lanes_, B);
     for (int l = 0; l < nl; ++l) lanes_[l].cap_B = std::max(lanes_[l].cap_B, chunk(B, nl, l));
   }
-  templ_arena_.cap = measure_arena(cfg.max_batch, 127, false);
+  size_arenas();
   SMK_CUDA(cudaMalloc(&templ_arena_.base, templ_arena_.cap));
   for (int l = 0; l < n_lanes_; ++l) {
     Lane& ln = lanes_[l];
-    ln.search.cap = measure_arena(ln.cap_B, cfg.search_size, true);
+    ln.id = l;
     SMK_CUDA(cudaMalloc(&ln.search.base, ln.search.cap));
-    if (cfg_.with_mask) {
-      ln.refine.cap = refine_arena_bytes(ln.cap_B);
-      SMK_CUDA(cudaMalloc(&ln.refine.base, ln.refine.cap));
-    }
+    if (cfg_.with_mask) SMK_CUDA(cudaMalloc(&ln.refine.base, ln.refine.cap));
     for (int i = 0; i < kAux; ++i) SMK_CUDA(cudaStreamCreateWithFlags(&ln.aux[i], cudaStreamNonBlocking));
     SMK_CUDA(cudaStreamCreateWithFlags(&ln.own, cudaStreamNonBlocking));
   }
@@ -610,7 +582,6 @@ void Engine::construct(const sm_config& cfg) {
     SMK_CUDA(cudaMalloc(&stage_best_[i], B * sizeof(int32_t)));
     if (cfg_.with_mask) SMK_CUDA(cudaMalloc(&stage_maskcol_[i], B * 3969 * sizeof(float)));
     SMK_CUDA(cudaEventCreateWithFlags(&h2d_done_[i], cudaEventDisableTiming));
-    SMK_CUDA(cudaEventCreateWithFlags(&compute_done_[i], cudaEventDisableTiming));
     SMK_CUDA(cudaEventCreateWithFlags(&d2h_done_[i], cudaEventDisableTiming));
     for (int l = 0; l < kMaxLanes; ++l) SMK_CUDA(cudaEventCreateWithFlags(&lane_done_[i][l], cudaEventDisableTiming));
   }
@@ -653,7 +624,6 @@ void Engine::release() {
     cudaFree(stage_x_[i]); cudaFree(stage_cls_[i]); cudaFree(stage_loc_[i]); cudaFree(stage_mask_[i]); cudaFree(stage_pos_[i]);
     cudaFree(stage_tsz_[i]); cudaFree(stage_rec_[i]); cudaFree(stage_best_[i]); cudaFree(stage_maskcol_[i]);
     if (h2d_done_[i]) cudaEventDestroy(h2d_done_[i]);
-    if (compute_done_[i]) cudaEventDestroy(compute_done_[i]);
     if (d2h_done_[i]) cudaEventDestroy(d2h_done_[i]);
     for (int l = 0; l < kMaxLanes; ++l) if (lane_done_[i][l]) cudaEventDestroy(lane_done_[i][l]);
   }
@@ -668,38 +638,28 @@ void Engine::release() {
   for (auto& kv : graphs_) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
 }
 
-// every allocation refine_lane makes, in its order (the window sizes 15 / 31 / 61 / 127 are fixed by custom.py:131-152)
-size_t Engine::refine_arena_bytes(int B) const {
-  size_t off = 0;
-  auto add = [&](size_t bytes) { off = align_up(off) + bytes; };
-  auto act = [&](int hw, int c) { add((size_t)B * hw * hw * c * sizeof(__half)); if (exact_) add((size_t)B * hw * hw * c * sizeof(__half)); };
-  auto f32 = [&](int hw, int c) { add((size_t)B * hw * hw * c * sizeof(float)); };
-  act(15, 512); act(15, 128); f32(15, 32);          // c2, v2.0, v2.2
-  act(31, 256); act(31, 64); f32(31, 16);           // c1, v1.0, v1.2
-  act(61, 64); f32(61, 16); f32(61, 4);             // c0, v0.0, v0.2
-  add((size_t)B * 256 * sizeof(float)); f32(15, 32);// p3, deconv
-  f32(15, 32); f32(15, 32); f32(31, 16);            // h2.0, h2.2, post0
-  f32(31, 16); f32(31, 16); f32(61, 4);             // h1.0, h1.2, post1
-  f32(61, 4); f32(61, 4);                           // h0.0, h0.2 (post2 writes the caller's buffer)
-  return align_up(off + (1u << 16));
-}
-
-size_t Engine::measure_arena(int B, int S, bool search) {
-  Arena ar;
-  ar.measure = true;
+// Workspace sizes from the schedule itself: dry runs (measuring_: the arenas only count, nothing is enqueued) of the
+// template backbone and, per lane, of track_lane under every flag combination it accepts and of refine_lane.
+void Engine::size_arenas() {
   measuring_ = true;
-  Act xf = backbone(nullptr, B, S, ar, search, nullptr);
-  if (search) {
-    // heads: conv_search, corr, head.0 per branch
-    alloc_act(ar, B, xf.H - 2, xf.W - 2, 256 * n_branches_);      // conv_search of all branches (one GEMM or one each)
-    for (int br = 0; br < n_branches_; ++br) {
-      alloc_act(ar, B, R_, R_, 256);
-      alloc_act(ar, B, R_, R_, 256);
-    }
+  Arena templ;
+  templ.measure = true;
+  backbone(nullptr, cfg_.max_batch, 127, templ, nullptr, nullptr);
+  templ_arena_.cap = align_up(templ.peak + (1u << 20));
+  const int max_flags = cfg_.with_mask ? (SM_TRACK_MASK_FEATURES | SM_TRACK_MASK_HEAD) : 0;
+  for (int l = 0; l < n_lanes_; ++l) {
+    Lane probe;
+    probe.search.measure = probe.refine.measure = true;
+    const int B = lanes_[l].cap_B;
+    for (int flags = 0; flags <= max_flags; ++flags)
+      track_lane(probe, 0, B, nullptr, nullptr, nullptr, nullptr, flags, nullptr);
+    float out;                         // refine_lane's last layer writes the caller's buffer, not the arena
+    if (cfg_.with_mask) refine_lane(probe, B, nullptr, &out, nullptr);
+    lanes_[l].search.cap = align_up(probe.search.peak + (1u << 20));
+    if (cfg_.with_mask) lanes_[l].refine.cap = align_up(probe.refine.peak + (1u << 16));
   }
   measuring_ = false;
-  cur_->named.clear();
-  return align_up(ar.peak + (1u << 20));
+  state_ = CallState();
 }
 
 // ================================================================================================
@@ -1063,9 +1023,7 @@ F32T Engine::alloc_f32(Arena& ar, int B, int H, int W, int C) {
 
 void Engine::conv_into(const Act& in, const ConvW& Lw, Epilogue ep, cudaStream_t st, const Act* res,
                        const Act* in2) {
-  if (measuring_) return;
   ep.beta = Lw.beta;
-  ++launches_;
   const double M = (double)in.B * Lw.g.out_size(in.H) * Lw.g.out_size(in.W);
   double K = (double)Lw.g.KH * Lw.g.KW * Lw.g.Cin;
   const bool tc = cfg_.backend == SM_BACKEND_TENSOR && Lw.gemm_ok;
@@ -1087,47 +1045,48 @@ void Engine::conv_into(const Act& in, const ConvW& Lw, Epilogue ep, cudaStream_t
             "activation scale mismatch at " + Lw.conv_key + " (weights were packed for other scales: re-run calibrate)");
   SMK_CHECK(ep.out_mode == OUT_NHWC_SPLIT || Lw.s_out == 0, "fp32 outputs are unscaled");
   if (ep.out_mode == OUT_NHWC_SPLIT) ep.ovf = ovf_flag_;
-  Scope sc(this, Lw.conv_key, tc ? "conv_gemm" : "conv_simt", 2.0 * M * K * Lw.g.Cout,
-           4.0 * ((double)in.numel() + (in2 ? (double)in2->numel() : 0.0) + M * Lw.g.Cout * (res ? 2 : 1) +
-                  K * Lw.g.Cout), st);
-  if (tc) {
-    ep.alpha = Lw.alpha;
-    // start where the biggest input was touched last
-    const Act* big = &in;
-    if (in2 != nullptr && in2->numel() > big->numel()) big = in2;
-    if (res != nullptr && res->numel() > big->numel()) big = res;
-    static const bool no_reverse = std::getenv("SMB200_NO_REVERSE") != nullptr;   // A/B switch for measurements
-    // bottleneck conv2 (3x3 / s1 / p1, 64 or 128 channels): resident-patch kernel, walks its tiles front to back
-    const bool use_patch = patch_conv_mode() != 0 && in2 == nullptr && res == nullptr &&
-                           ep.out_mode == OUT_NHWC_SPLIT && patch_conv_supported(in, Lw.g);
-    const bool reverse = !use_patch && !no_reverse && end_of(*big) > 0;
+  const double flops = 2.0 * M * K * Lw.g.Cout;
+  const double bytes = 4.0 * ((double)in.numel() + (in2 ? (double)in2->numel() : 0.0) + M * Lw.g.Cout * (res ? 2 : 1) +
+                              K * Lw.g.Cout);
+  if (!tc) {
+    SMK_CHECK(Lw.s_in == 0 && Lw.s_out == 0, "the SIMT backend runs unscaled activations only");
+    ep.alpha = ones_;
+    if (res != nullptr) { ep.res_hi = res->hi; ep.res_lo = res->lo; }
+    launch(st, 1, Lw.conv_key, "conv_simt", flops, bytes, [&] { launch_ref_conv(in, Lw.g, Lw.w_ref, ep, st); });
+    return;
+  }
+  ep.alpha = Lw.alpha;
+  // start where the biggest input was touched last
+  const Act* big = &in;
+  if (in2 != nullptr && in2->numel() > big->numel()) big = in2;
+  if (res != nullptr && res->numel() > big->numel()) big = res;
+  // bottleneck conv2 (3x3 / s1 / p1, 64 or 128 channels): resident-patch kernel, walks its tiles front to back
+  const bool use_patch = in2 == nullptr && res == nullptr && ep.out_mode == OUT_NHWC_SPLIT &&
+                         patch_conv_supported(in, Lw.g);
+  const bool reverse = !use_patch && end_of(*big) > 0;
+  GemmInput gi[2] = {{in, Lw.g, 0}, {in, Lw.g, 0}};
+  int nconv = 1;
+  const Act* ident = nullptr;
+  if (in2 != nullptr) {
+    gi[1] = {*in2, Lw.g2, Lw.col2};
+    nconv = 2;
+    ep.beta = Lw.beta2;
+  } else if (res != nullptr) {
+    if (Lw.has_diag) ident = res;                                  // residual through the MMA pipeline
+    else { ep.res_hi = res->hi; ep.res_lo = res->lo; }             // epilogue-side add
+  }
+  launch(st, 1, Lw.conv_key, "conv_gemm", flops, bytes, [&] {
     const int now_end = reverse ? -1 : +1;
     last_end_[in.hi] = now_end;
     if (in2 != nullptr) last_end_[in2->hi] = now_end;
     if (res != nullptr) last_end_[res->hi] = now_end;
     if (ep.out_mode == OUT_NHWC_SPLIT) last_end_[ep.out_hi] = now_end;
-    GemmInput gi[2] = {{in, Lw.g, 0}, {in, Lw.g, 0}};
-    int nconv = 1;
-    const Act* ident = nullptr;
-    if (in2 != nullptr) {
-      gi[1] = {*in2, Lw.g2, Lw.col2};
-      nconv = 2;
-      ep.beta = Lw.beta2;
-    } else if (res != nullptr) {
-      if (Lw.has_diag) ident = res;                                  // residual through the MMA pipeline
-      else { ep.res_hi = res->hi; ep.res_lo = res->lo; }             // epilogue-side add
-    }
     if (use_patch)
       launch_conv3x3_patch(in, Lw.g, Lw.w_hi, Lw.w_lo, Lw.w_ld, ep, exact_ ? 2 : 1, num_sms_, st);
     else
       launch_gemm_multi(gi, nconv, ident, Lw.col_diag, Lw.w_hi, Lw.w_lo, Lw.cout_pad, Lw.w_ld, ep, exact_ ? 2 : 1,
                         num_sms_, st, reverse);
-  } else {
-    SMK_CHECK(Lw.s_in == 0 && Lw.s_out == 0, "the SIMT backend runs unscaled activations only");
-    ep.alpha = ones_;
-    if (res != nullptr) { ep.res_hi = res->hi; ep.res_lo = res->lo; }
-    launch_ref_conv(in, Lw.g, Lw.w_ref, ep, st);
-  }
+  });
 }
 
 // calibration pass: remember which tensor lives in this buffer and fold its max |value| into the tensor's slot
@@ -1169,32 +1128,26 @@ F32T Engine::conv_f32(const Act& in, const ConvW& Lw, bool relu, Arena& ar, cuda
 }
 
 // ResDown.forward / forward_all (custom.py:58-66): ResNet (resnet.py:217-227) + ResDownS (custom.py:19-25)
-Act Engine::backbone(const float* x, int B, int S, Arena& ar, bool keep, cudaStream_t st) {
+Act Engine::backbone(const float* x, int B, int S, Arena& ar, std::map<std::string, Act>* keep, cudaStream_t st) {
   const std::string F = "features.features.";
   const int So = (S - 7) / 2 + 1;
   Act p0 = alloc_act(ar, B, So, So, 64);
   const ConvW& stem = L(F + "conv1");
-  if (!measuring_) {
-    Scope sc(this, "stem", "stem", 2.0 * B * So * So * 64 * 147, 4.0 * B * (3.0 * S * S + 64.0 * So * So), st);
+  launch(st, 1, "stem", "stem", 2.0 * B * So * So * 64 * 147, 4.0 * B * (3.0 * S * S + 64.0 * So * So), [&] {
     if (cfg_.backend == SM_BACKEND_TENSOR)
       launch_stem_tc(x, B, S, stem_whi_, stem_wlo_, stem_alpha_, stem.beta, p0, num_sms_, st, ovf_flag_);
     else launch_stem(x, B, S, stem.w_ref, ones_, stem.beta, p0, st);
-    ++launches_;
-  }
+  });
   p0.sexp = stem.s_out;
   note_tensor(p0, "stem", st);
   const int Sp = (So + 2 - 3) / 2 + 1;
   Act y = alloc_act(ar, B, Sp, Sp, 64);
   y.sexp = p0.sexp;                    // max-pool commutes with a positive scale
-  if (calibrating_ && !measuring_) tensor_name_[y.hi] = "stem";
-  if (!measuring_) {
-    Scope sc(this, "maxpool", "pool", 0, 4.0 * (p0.numel() + y.numel()), st);
-    launch_maxpool3s2(p0, y, st);
-    ++launches_;
-  }
+  if (calibrating_) tensor_name_[y.hi] = "stem";
+  launch(st, 1, "maxpool", "pool", 0, 4.0 * (p0.numel() + y.numel()), [&] { launch_maxpool3s2(p0, y, st); });
   last_end_[p0.hi] = +1;       // stem and pool write front to back
   last_end_[y.hi] = +1;
-  if (keep) cur_->named["p0"] = p0;
+  if (keep) (*keep)["p0"] = p0;
   const char* names[3] = {"layer1", "layer2", "layer3"};
   const int blocks[3] = {3, 4, 6};
   for (int l = 0; l < 3; ++l) {
@@ -1211,14 +1164,14 @@ Act Engine::backbone(const float* x, int B, int S, Arena& ar, bool keep, cudaStr
         y = conv(t2, c3, true, &res, ar, st);
       }
     }
-    if (keep) cur_->named[std::string("p") + std::to_string(l + 1)] = y;
+    if (keep) (*keep)[std::string("p") + std::to_string(l + 1)] = y;
   }
   Act xf = conv(y, L("features.downsample.downsample.0"), false, nullptr, ar, st);
   if (xf.W < 20) {   // custom.py:21-24
     Act c = alloc_act(ar, B, xf.H - 8, xf.W - 8, xf.C);
     c.sexp = xf.sexp;
-    if (calibrating_ && !measuring_) tensor_name_[c.hi] = tensor_name_[xf.hi];
-    if (!measuring_) { launch_crop_center(xf, 4, c, st); ++launches_; }
+    if (calibrating_) tensor_name_[c.hi] = tensor_name_[xf.hi];
+    launch(st, 1, [&] { launch_crop_center(xf, 4, c, st); });
     xf = c;
   }
   return xf;
@@ -1232,7 +1185,7 @@ void Engine::do_template(int slot0, int B, const float* z, cudaStream_t st) {
   SMK_CHECK(B >= 1 && B <= cfg_.max_batch && slot0 >= 0 && slot0 + B <= cfg_.num_slots, "template batch/slot range");
   join_lanes(st);
   templ_arena_.reset();
-  Act zf = backbone(z, B, 127, templ_arena_, false, st);
+  Act zf = backbone(z, B, 127, templ_arena_, nullptr, st);
   SMK_CHECK(zf.H == 7 && zf.W == 7, "template feature must be 7x7");
   zf_ = zf;
   have_zf_ = true;
@@ -1253,16 +1206,45 @@ void Engine::do_template(int slot0, int B, const float* z, cudaStream_t st) {
   }
 }
 
-void Engine::do_track(int slot0, int B, const float* x, float* cls, float* loc, float* mask, int flags,
-                      cudaStream_t st) {
-  join_lanes(st);
-  const std::vector<uint64_t> key = {1, (uint64_t)slot0, (uint64_t)B, (uint64_t)x, (uint64_t)cls, (uint64_t)loc,
-                                     (uint64_t)mask, (uint64_t)flags, (uint64_t)st};
-  run_with_graph(key, st, [&] { track_impl(slot0, B, x, cls, loc, mask, flags, st); });
+// Runs body(lane, b0, nbat, stream) for every lane's block [b0, b0 + nbat) of the batch split_batch() divided, last
+// lane first.  set == kJoined (device-pointer calls, coupled host path): lanes >= 1 are forked from `st` before
+// anything of this call is enqueued on it, so the lanes really run side by side, lane 0 runs on `st`, and all are
+// joined back into `st` before returning (also when the body throws).  Otherwise (host path with decoupled lanes,
+// staging set `set`): every lane runs on its own stream, ordered once after `st` and after the set's H2D, and the
+// D2H stream waits for each lane's lane_done_ event.
+template <typename F>
+void Engine::run_lanes(cudaStream_t st, int set, F&& body) {
+  const CallState& s = state_;
+  if (set != kJoined) {
+    lanes_dirty_ = true;
+    for (int l = s.split_n - 1; l >= 0; --l) {
+      Lane& ln = lanes_[l];
+      order_after(st, ln.own);
+      SMK_CUDA(cudaStreamWaitEvent(ln.own, h2d_done_[set], 0));
+      body(ln, s.split_off[l], s.split_off[l + 1] - s.split_off[l], ln.own);
+      SMK_CUDA(cudaEventRecord(lane_done_[set][l], ln.own));
+      SMK_CUDA(cudaStreamWaitEvent(d2h_stream_, lane_done_[set][l], 0));
+    }
+    return;
+  }
+  const int nl = s.split_n;
+  const bool fork = nl > 1 && concurrent();
+  auto join = [&] {
+    if (fork) for (int l = 1; l < nl; ++l) order_after(lanes_[l].own, st);
+  };
+  if (fork) for (int l = 1; l < nl; ++l) order_after(st, lanes_[l].own);
+  try {
+    for (int l = nl - 1; l >= 0; --l)
+      body(lanes_[l], s.split_off[l], s.split_off[l + 1] - s.split_off[l], fork && l > 0 ? lanes_[l].own : st);
+  } catch (...) {
+    try { join(); } catch (...) {}
+    throw;
+  }
+  join();
 }
 
-void Engine::track_impl(int slot0, int B, const float* x, float* cls, float* loc, float* mask, int flags,
-                        cudaStream_t st) {
+void Engine::do_track(int slot0, int B, const float* x, float* cls, float* loc, float* mask, int flags,
+                      cudaStream_t st) {
   SMK_CHECK(weights_ready_, "weights not loaded");
   SMK_CHECK(B >= 1 && B <= cfg_.max_batch && slot0 >= 0 && slot0 + B <= cfg_.num_slots, "track batch/slot range");
   SMK_CHECK(cls != nullptr && loc != nullptr, "cls/loc outputs required");
@@ -1270,64 +1252,56 @@ void Engine::track_impl(int slot0, int B, const float* x, float* cls, float* loc
   const bool want_mask_head = (flags & SM_TRACK_MASK_HEAD) != 0;
   SMK_CHECK(!(want_feats || want_mask_head) || cfg_.with_mask, "engine was built without the mask branch");
   SMK_CHECK(!want_mask_head || mask != nullptr, "mask output buffer required");
-  // split the streams over the two lanes; lane 1 forks from / joins back into the caller's stream
-  split_batch(B);
-  const int nl = split_n_;
-  LaneGuard guard{this, st};
+  join_lanes(st);
+  const std::vector<uint64_t> key = {1, (uint64_t)slot0, (uint64_t)B, (uint64_t)x, (uint64_t)cls, (uint64_t)loc,
+                                     (uint64_t)mask, (uint64_t)flags, (uint64_t)st};
   const size_t S = cfg_.search_size, A = cfg_.anchor_num, RR = (size_t)R_ * R_;
-  // fork before anything of this call is enqueued on `st`, so the lanes really run side by side
-  fork_lanes(st);
-  for (int l = nl - 1; l >= 0; --l) {
-    cur_ = &lanes_[l];
-    const int b0 = split_off_[l], nbat = split_off_[l + 1] - split_off_[l];
-    cudaStream_t ls = (l == 0 || !concurrent()) ? st : lanes_[l].own;
-    track_lane(slot0 + b0, nbat, x + b0 * 3 * S * S, cls + b0 * 2 * A * RR, loc + b0 * 4 * A * RR,
-               mask != nullptr ? mask + (size_t)b0 * 63 * 63 * RR : nullptr, flags, ls);
-  }
-  cur_ = &lanes_[0];
-  guard.armed = false;
-  if (!defer_join_) join_forked(st);
-  last_B_ = B;
-  have_mask_feats_ = want_feats || want_mask_head;
+  run_with_graph(key, st, [&] {
+    split_batch(B);
+    run_lanes(st, kJoined, [&](Lane& ln, int b0, int nbat, cudaStream_t ls) {
+      track_lane(ln, slot0 + b0, nbat, x + b0 * 3 * S * S, cls + b0 * 2 * A * RR, loc + b0 * 4 * A * RR,
+                 mask != nullptr ? mask + (size_t)b0 * 63 * 63 * RR : nullptr, flags, ls);
+    });
+    state_.last_B = B;
+    state_.have_mask_feats = want_feats || want_mask_head;
+  });
 }
 
-void Engine::track_lane(int slot0, int B, const float* x, float* cls, float* loc, float* mask, int flags,
+void Engine::track_lane(Lane& ln, int slot0, int B, const float* x, float* cls, float* loc, float* mask, int flags,
                         cudaStream_t st) {
   const bool want_feats = (flags & SM_TRACK_MASK_FEATURES) != 0;
   const bool want_mask_head = (flags & SM_TRACK_MASK_HEAD) != 0;
-  Arena& search_arena = cur_->search;
+  Arena& search_arena = ln.search;
   search_arena.reset();
-  cur_->named.clear();
-  Act xf = backbone(x, B, cfg_.search_size, search_arena, true, st);
-  cur_->named["search"] = xf;
+  std::map<std::string, Act>& named = state_.named[ln.id];
+  named.clear();
+  Act xf = backbone(x, B, cfg_.search_size, search_arena, &named, st);
+  named["search"] = xf;
   const int nb = (want_feats || want_mask_head) ? 3 : 2;
   float* outs[3] = {cls, loc, mask};
   // all branches wanted: their conv_search layers run as ONE GEMM over xf (N = 256 x branches)
-  static const bool no_cat = std::getenv("SMB200_NO_SEARCH_CAT") != nullptr;
-  const bool use_cat = nb == n_branches_ && cfg_.backend == SM_BACKEND_TENSOR && !no_cat;
+  const bool use_cat = nb == n_branches_ && cfg_.backend == SM_BACKEND_TENSOR;
   Act cs_all;
   if (use_cat) cs_all = conv(xf, L(kSearchCat), true, nullptr, search_arena, st);
   for (int br = 0; br < nb; ++br) {
     // the branches only share their input: run them side by side (their 1x1 heads and the xcorr do not fill
     // the GPU on their own)
-    cudaStream_t bs = (concurrent() && br > 0) ? cur_->aux[br - 1] : st;
+    cudaStream_t bs = (concurrent() && br > 0) ? ln.aux[br - 1] : st;
     order_after(st, bs);
     const std::string P = kBranch[br];
     Act cs = use_cat ? cs_all : conv(xf, L(P + "conv_search.0"), true, nullptr, search_arena, bs);
     Act corr = alloc_act(search_arena, B, cs.H - 4, cs.W - 4, 256);
     const size_t off = ((size_t)br * cfg_.num_slots + slot0) * 25 * 256;
-    {
-      Scope sc(this, std::string(kCorrName[br]), "xcorr", 2.0 * 25 * corr.numel(),
-               4.0 * (2.0 * corr.numel() + (double)B * cs.H * cs.W * 256 + (double)B * 25 * 256), bs);
-      corr.sexp = tscale(kCorrName[br]);
-      const int s_kc = L(P + "conv_kernel.0").s_out;
+    corr.sexp = tscale(kCorrName[br]);
+    const int s_kc = L(P + "conv_kernel.0").s_out;
+    launch(bs, 1, kCorrName[br], "xcorr", 2.0 * 25 * corr.numel(),
+           4.0 * (2.0 * corr.numel() + (double)B * cs.H * cs.W * 256 + (double)B * 25 * 256), [&] {
       launch_xcorr_nhwc(cs, use_cat ? 256 * br : 0, kcache_hi_ + off, exact_ ? kcache_lo_ + off : nullptr, 5, 5, corr,
                         std::ldexp(1.f, corr.sexp - cs.sexp - s_kc), ovf_flag_, bs);
-      ++launches_;
       last_end_[corr.hi] = +1;
-    }
+    });
     note_tensor(corr, kCorrName[br], bs);
-    cur_->named[kCorrName[br]] = corr;
+    named[kCorrName[br]] = corr;
     if (!(br == 2 && !want_mask_head)) {
       Act h = conv(corr, L(P + "head.0"), true, nullptr, search_arena, bs);
       Epilogue ep;
@@ -1337,7 +1311,7 @@ void Engine::track_lane(int slot0, int B, const float* x, float* cls, float* loc
       conv_into(h, L(P + "head.3"), ep, bs);
     }
   }
-  for (int br = 1; br < nb; ++br) order_after((concurrent()) ? cur_->aux[br - 1] : st, st);
+  for (int br = 1; br < nb; ++br) order_after((concurrent()) ? ln.aux[br - 1] : st, st);
 }
 
 F32T Engine::small(const F32T& a, const F32T* b, int Ho, const ConvW& Lw, bool relu, float* out_override, Arena& ar,
@@ -1347,97 +1321,84 @@ F32T Engine::small(const F32T& a, const F32T* b, int Ho, const ConvW& Lw, bool r
   out.p = out_override != nullptr ? out_override
                                   : static_cast<float*>(ar.alloc((size_t)a.B * Ho * Ho * Lw.g.Cout * sizeof(float)));
   SMK_CHECK(a.C == Lw.g.Cin && (b == nullptr || (b->C == a.C && b->H == a.H)), "small conv operand shapes");
-  const int* map = updown_map(Ho, a.H);
-  Scope sc(this, Lw.conv_key, "refine_small", 2.0 * a.B * Ho * Ho * 9.0 * a.C * Lw.g.Cout,
-           4.0 * a.B * ((double)a.H * a.W * a.C * (b ? 2 : 1) + (double)Ho * Ho * Lw.g.Cout), st);
-  launch_small_conv3x3_maps(a.p, b ? b->p : nullptr, a.B, a.H, a.W, Ho, Ho, a.C, Lw.g.Cout, map, map, Lw.w_ref, Lw.beta,
-                            relu ? 1 : 0, out.p, st);
-  ++launches_;
+  launch(st, 1, Lw.conv_key, "refine_small", 2.0 * a.B * Ho * Ho * 9.0 * a.C * Lw.g.Cout,
+         4.0 * a.B * ((double)a.H * a.W * a.C * (b ? 2 : 1) + (double)Ho * Ho * Lw.g.Cout), [&] {
+    const int* map = updown_map(Ho, a.H);
+    launch_small_conv3x3_maps(a.p, b ? b->p : nullptr, a.B, a.H, a.W, Ho, Ho, a.C, Lw.g.Cout, map, map, Lw.w_ref,
+                              Lw.beta, relu ? 1 : 0, out.p, st);
+  });
   return out;
 }
 
 // Refine.forward(test=True), custom.py:131-154, one (dy,dx) per stream
 void Engine::do_refine(int B, const int32_t* pos, float* out, cudaStream_t st) {
-  SMK_CHECK(have_mask_feats_ && B == last_B_, "sm_refine must follow sm_track(..., SM_TRACK_MASK_FEATURES) with the same B");
+  SMK_CHECK(state_.have_mask_feats && B == state_.last_B,
+            "sm_refine must follow sm_track(..., SM_TRACK_MASK_FEATURES) with the same B");
+  SMK_CHECK(cfg_.with_mask, "engine was built without the mask branch");
   join_lanes(st);
   const std::vector<uint64_t> key = {2, (uint64_t)B, (uint64_t)pos, (uint64_t)out, (uint64_t)st,
-                                     (uint64_t)lanes_[0].named["p0"].hi};
-  run_with_graph(key, st, [&] { refine_impl(B, pos, out, st); });
-}
-
-void Engine::refine_impl(int B, const int32_t* pos, float* out, cudaStream_t st) {
-  SMK_CHECK(cfg_.with_mask, "engine was built without the mask branch");
-  SMK_CHECK(have_mask_feats_ && B == last_B_, "sm_refine must follow sm_track(..., SM_TRACK_MASK_FEATURES) with the same B");
+                                     (uint64_t)state_.named[0]["p0"].hi};
   // same split as the track that cached the features
-  LaneGuard guard{this, st};
-  fork_lanes(st);
-  for (int l = split_n_ - 1; l >= 0; --l) {
-    cur_ = &lanes_[l];
-    const int b0 = split_off_[l], nbat = split_off_[l + 1] - split_off_[l];
-    cudaStream_t ls = (l == 0 || !concurrent()) ? st : lanes_[l].own;
-    refine_lane(nbat, pos + 2 * b0, out + (size_t)b0 * 127 * 127, ls);
-  }
-  cur_ = &lanes_[0];
-  guard.armed = false;
-  join_forked(st);
+  run_with_graph(key, st, [&] {
+    run_lanes(st, kJoined, [&](Lane& ln, int b0, int nbat, cudaStream_t ls) {
+      refine_lane(ln, nbat, pos + 2 * b0, out + (size_t)b0 * 127 * 127, ls);
+    });
+  });
 }
 
-void Engine::refine_lane(int B, const int32_t* pos, float* out, cudaStream_t st) {
-  Arena& ar = cur_->refine;
+void Engine::refine_lane(Lane& ln, int B, const int32_t* pos, float* out, cudaStream_t st) {
+  Arena& ar = ln.refine;
   ar.reset();
   const std::string R = "refine_model.";
-  const Act& p0 = cur_->named["p0"];
-  const Act& p1 = cur_->named["p1"];
-  const Act& p2 = cur_->named["p2"];
-  const Act& corr = cur_->named["corr_mask"];
+  std::map<std::string, Act>& named = state_.named[ln.id];
+  const Act& p0 = named["p0"];
+  const Act& p1 = named["p1"];
+  const Act& p2 = named["p2"];
+  const Act& corr = named["corr_mask"];
   // The three v-branches (crop -> conv -> conv on p2 / p1 / p0) depend only on the cached pyramid: they run on
   // auxiliary streams while the main stream walks deconv -> h2 -> post0 -> h1 -> post1 -> h0 -> post2.
-  cudaStream_t s2 = concurrent() ? cur_->aux[0] : st, s1 = concurrent() ? cur_->aux[1] : st,
-               s0 = concurrent() ? cur_->aux[2] : st;
+  cudaStream_t s2 = concurrent() ? ln.aux[0] : st, s1 = concurrent() ? ln.aux[1] : st,
+               s0 = concurrent() ? ln.aux[2] : st;
   order_after(st, s2);
   order_after(st, s1);
   order_after(st, s0);
   // level 2 branch (15x15)
   Act c2 = alloc_act(ar, B, 15, 15, 512);
-  {
-    Scope sc(this, "crop_p2", "refine_misc", 0, 8.0 * c2.numel(), s2);
+  c2.sexp = p2.sexp;
+  if (calibrating_) tensor_name_[c2.hi] = tensor_name_[p2.hi];
+  launch(s2, 1, "crop_p2", "refine_misc", 0, 8.0 * c2.numel(), [&] {
     last_end_[c2.hi] = +1;
-    c2.sexp = p2.sexp;
-    if (calibrating_) tensor_name_[c2.hi] = tensor_name_[p2.hi];
-    launch_refine_crop(p2, pos, R_ - 1, 1, 4, 15, c2, s2); ++launches_;
-  }
+    launch_refine_crop(p2, pos, R_ - 1, 1, 4, 15, c2, s2);
+  });
   Act v2a = conv(c2, L(R + "v2.0"), true, nullptr, ar, s2);
   F32T v2b = conv_f32(v2a, L(R + "v2.2"), true, ar, s2);
   // level 1 branch (31x31)
   Act c1 = alloc_act(ar, B, 31, 31, 256);
-  {
-    Scope sc(this, "crop_p1", "refine_misc", 0, 8.0 * c1.numel(), s1);
+  c1.sexp = p1.sexp;
+  if (calibrating_) tensor_name_[c1.hi] = tensor_name_[p1.hi];
+  launch(s1, 1, "crop_p1", "refine_misc", 0, 8.0 * c1.numel(), [&] {
     last_end_[c1.hi] = +1;
-    c1.sexp = p1.sexp;
-    if (calibrating_) tensor_name_[c1.hi] = tensor_name_[p1.hi];
-    launch_refine_crop(p1, pos, R_ - 1, 2, 8, 31, c1, s1); ++launches_;
-  }
+    launch_refine_crop(p1, pos, R_ - 1, 2, 8, 31, c1, s1);
+  });
   Act v1a = conv(c1, L(R + "v1.0"), true, nullptr, ar, s1);
   F32T v1b = conv_f32(v1a, L(R + "v1.2"), true, ar, s1);
   // level 0 branch (61x61)
   Act c0 = alloc_act(ar, B, 61, 61, 64);
-  {
-    Scope sc(this, "crop_p0", "refine_misc", 0, 8.0 * c0.numel(), s0);
+  c0.sexp = p0.sexp;
+  if (calibrating_) tensor_name_[c0.hi] = tensor_name_[p0.hi];
+  launch(s0, 1, "crop_p0", "refine_misc", 0, 8.0 * c0.numel(), [&] {
     last_end_[c0.hi] = +1;
-    c0.sexp = p0.sexp;
-    if (calibrating_) tensor_name_[c0.hi] = tensor_name_[p0.hi];
-    launch_refine_crop(p0, pos, R_ - 1, 4, 16, 61, c0, s0); ++launches_;
-  }
+    launch_refine_crop(p0, pos, R_ - 1, 4, 16, 61, c0, s0);
+  });
   F32T v0a = conv_f32(c0, L(R + "v0.0"), true, ar, s0);
   F32T v0b = small(v0a, nullptr, 61, L(R + "v0.2"), true, nullptr, ar, s0);
   // main chain: p3 = corr_feature[:, :, dy, dx]; out = deconv(p3)
   float* p3 = static_cast<float*>(ar.alloc((size_t)B * 256 * sizeof(float)));
   F32T d = alloc_f32(ar, B, 15, 15, 32);
-  {
-    Scope sc(this, "deconv", "refine_misc", 2.0 * B * 256 * 7200, 4.0 * (256.0 * 7200 + B * 7200.0), st);
-    launch_gather_corr(corr, pos, p3, std::ldexp(1.f, -corr.sexp), st); ++launches_;
-    launch_deconv(p3, deconv_w_, deconv_b_, d.p, B, 256, 7200, 32, st); ++launches_;
-  }
+  launch(st, 2, "deconv", "refine_misc", 2.0 * B * 256 * 7200, 4.0 * (256.0 * 7200 + B * 7200.0), [&] {
+    launch_gather_corr(corr, pos, p3, std::ldexp(1.f, -corr.sexp), st);
+    launch_deconv(p3, deconv_w_, deconv_b_, d.p, B, 256, 7200, 32, st);
+  });
   F32T h2a = small(d, nullptr, 15, L(R + "h2.0"), true, nullptr, ar, st);
   F32T h2b = small(h2a, nullptr, 15, L(R + "h2.2"), true, nullptr, ar, st);
   order_after(s2, st);
@@ -1452,66 +1413,68 @@ void Engine::refine_lane(int B, const int32_t* pos, float* out, cudaStream_t st)
   small(h0b, &v0b, 127, L(R + "post2"), false, out, ar, st);                // (B,127,127,1) == (B,127*127)
 }
 
-// Host-buffer step, asynchronous: H2D on a copy stream, compute on the caller's stream, D2H on a second copy
-// stream, chained by events.  Two staging sets alternate, so submitting step k+1 before waiting for step k overlaps
-// its input transfer (and step k's result transfer) with compute.  Returns the ticket to pass to host_wait().
-int Engine::track_host_async(int slot0, int B, const float* xh, float* clsh, float* loch, const int32_t* posh,
-                             float* maskh, cudaStream_t st) {
-  const size_t S = cfg_.search_size, A = cfg_.anchor_num;
-  const size_t nx = (size_t)B * 3 * S * S, ncls = (size_t)B * 2 * A * R_ * R_, nloc = 2 * ncls;
-  SMK_CHECK(B >= 1 && B <= cfg_.max_batch, "batch");
+int Engine::next_set() {
   const int t = (int)(host_calls_++ & 1);
   if (set_busy_[t]) host_wait(t);                 // the staging set is still owned by an un-waited ticket
-  const bool refine = posh != nullptr && maskh != nullptr;
-  SMK_CUDA(cudaMemcpyAsync(stage_x_[t], xh, nx * sizeof(float), cudaMemcpyHostToDevice, h2d_stream_));
-  if (refine)
-    SMK_CUDA(cudaMemcpyAsync(stage_pos_[t], posh, (size_t)B * 2 * sizeof(int32_t), cudaMemcpyHostToDevice, h2d_stream_));
+  return t;
+}
+
+// Host-buffer call on staging set t, asynchronous: H2D on a copy stream, compute, D2H on a second copy stream,
+// chained by events.  Two staging sets alternate, so submitting call k+1 before waiting for call k overlaps its input
+// transfer (and call k's result transfer) with compute.  A batch split over two lanes (graphs off) runs body on
+// decoupled lanes (see lanes_dirty_: ordered after the caller's stream once, for the templates written there, then
+// each lane only depends on its inputs); otherwise coupled() runs the whole call on `st` through the device-pointer
+// entry points.  Returns the ticket to pass to host_wait().
+template <typename Coupled, typename F>
+int Engine::host_call(int t, int B, bool mask_feats, cudaStream_t st, std::initializer_list<Copy> h2d,
+                      std::initializer_list<Copy> d2h, Coupled&& coupled, F&& body) {
+  for (const Copy& c : h2d)
+    if (c.src != nullptr) SMK_CUDA(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyHostToDevice, h2d_stream_));
   SMK_CUDA(cudaEventRecord(h2d_done_[t], h2d_stream_));
   if (lanes_for(n_lanes_, B) >= 2 && !use_graphs_ && concurrent()) {
-    // decoupled lanes (see lanes_dirty_): order them after the caller's stream once (templates written there), then
-    // each lane only depends on its inputs
-    SMK_CHECK(weights_ready_, "weights not loaded");
-    SMK_CHECK(slot0 >= 0 && slot0 + B <= cfg_.num_slots, "track batch/slot range");
-    SMK_CHECK(!refine || cfg_.with_mask, "engine was built without the mask branch");
     split_batch(B);
-    for (int l = split_n_ - 1; l >= 0; --l) {
-      cur_ = &lanes_[l];
-      cudaStream_t ls = cur_->own;
-      const int b0 = split_off_[l], nbat = split_off_[l + 1] - split_off_[l];
-      order_after(st, ls);
-      SMK_CUDA(cudaStreamWaitEvent(ls, h2d_done_[t], 0));
-      track_lane(slot0 + b0, nbat, stage_x_[t] + b0 * 3 * S * S, stage_cls_[t] + b0 * 2 * A * R_ * R_,
-                 stage_loc_[t] + b0 * 4 * A * R_ * R_, nullptr, refine ? SM_TRACK_MASK_FEATURES : 0, ls);
-      if (refine) refine_lane(nbat, stage_pos_[t] + 2 * b0, stage_mask_[t] + (size_t)b0 * 127 * 127, ls);
-      SMK_CUDA(cudaEventRecord(lane_done_[t][l], ls));
-      SMK_CUDA(cudaStreamWaitEvent(d2h_stream_, lane_done_[t][l], 0));
-    }
-    cur_ = &lanes_[0];
-    last_B_ = B;
-    have_mask_feats_ = refine;
-    lanes_dirty_ = true;
+    run_lanes(st, t, body);
+    state_.last_B = B;
+    state_.have_mask_feats = mask_feats;
   } else {
-  SMK_CUDA(cudaStreamWaitEvent(st, h2d_done_[t], 0));
-  // lane 1 stays forked between its track and its refine (nobody reads cls/loc on `st` in between)
-  defer_join_ = refine && !use_graphs_;
-  try {
-    do_track(slot0, B, stage_x_[t], stage_cls_[t], stage_loc_[t], nullptr, refine ? SM_TRACK_MASK_FEATURES : 0, st);
-  } catch (...) {
-    defer_join_ = false;
-    throw;
+    SMK_CUDA(cudaStreamWaitEvent(st, h2d_done_[t], 0));
+    coupled();
+    SMK_CUDA(cudaEventRecord(lane_done_[t][0], st));
+    SMK_CUDA(cudaStreamWaitEvent(d2h_stream_, lane_done_[t][0], 0));
   }
-  defer_join_ = false;
-  if (refine) do_refine(B, stage_pos_[t], stage_mask_[t], st);
-  SMK_CUDA(cudaEventRecord(compute_done_[t], st));
-  SMK_CUDA(cudaStreamWaitEvent(d2h_stream_, compute_done_[t], 0));
-  }
-  SMK_CUDA(cudaMemcpyAsync(clsh, stage_cls_[t], ncls * sizeof(float), cudaMemcpyDeviceToHost, d2h_stream_));
-  SMK_CUDA(cudaMemcpyAsync(loch, stage_loc_[t], nloc * sizeof(float), cudaMemcpyDeviceToHost, d2h_stream_));
-  if (refine)
-    SMK_CUDA(cudaMemcpyAsync(maskh, stage_mask_[t], (size_t)B * 127 * 127 * sizeof(float), cudaMemcpyDeviceToHost, d2h_stream_));
+  for (const Copy& c : d2h)
+    if (c.dst != nullptr) SMK_CUDA(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost, d2h_stream_));
   SMK_CUDA(cudaEventRecord(d2h_done_[t], d2h_stream_));
   set_busy_[t] = true;
   return t;
+}
+
+int Engine::track_host_async(int slot0, int B, const float* xh, float* clsh, float* loch, const int32_t* posh,
+                             float* maskh, cudaStream_t st) {
+  const size_t S = cfg_.search_size, A = cfg_.anchor_num, RR = (size_t)R_ * R_;
+  SMK_CHECK(B >= 1 && B <= cfg_.max_batch, "batch");
+  SMK_CHECK(weights_ready_, "weights not loaded");
+  SMK_CHECK(slot0 >= 0 && slot0 + B <= cfg_.num_slots, "track batch/slot range");
+  const bool refine = posh != nullptr && maskh != nullptr;
+  SMK_CHECK(!refine || cfg_.with_mask, "engine was built without the mask branch");
+  const int flags = refine ? SM_TRACK_MASK_FEATURES : 0;
+  const int t = next_set();
+  return host_call(
+      t, B, refine, st,
+      {{stage_x_[t], xh, (size_t)B * 3 * S * S * sizeof(float)},
+       {stage_pos_[t], refine ? posh : nullptr, (size_t)B * 2 * sizeof(int32_t)}},
+      {{clsh, stage_cls_[t], (size_t)B * 2 * A * RR * sizeof(float)},
+       {loch, stage_loc_[t], (size_t)B * 4 * A * RR * sizeof(float)},
+       {refine ? maskh : nullptr, stage_mask_[t], (size_t)B * 127 * 127 * sizeof(float)}},
+      [&] {
+        do_track(slot0, B, stage_x_[t], stage_cls_[t], stage_loc_[t], nullptr, flags, st);
+        if (refine) do_refine(B, stage_pos_[t], stage_mask_[t], st);
+      },
+      [&](Lane& ln, int b0, int nbat, cudaStream_t ls) {
+        track_lane(ln, slot0 + b0, nbat, stage_x_[t] + b0 * 3 * S * S, stage_cls_[t] + b0 * 2 * A * RR,
+                   stage_loc_[t] + b0 * 4 * A * RR, nullptr, flags, ls);
+        if (refine) refine_lane(ln, nbat, stage_pos_[t] + 2 * b0, stage_mask_[t] + (size_t)b0 * 127 * 127, ls);
+      });
 }
 
 void Engine::host_wait(int ticket) {
@@ -1548,19 +1511,15 @@ Engine::StepIO slice_io(const Engine::StepIO& io, int b0, size_t S, size_t A, si
 }
 }  // namespace
 
-void Engine::step_lane(int slot0, int B, const StepIO& io, cudaStream_t st) {
-  track_lane(slot0, B, io.x, io.cls, io.loc, io.mask, io.flags, st);
-  {
-    Scope sc(this, "select", "select", 0, 4.0 * B * 6.0 * cfg_.anchor_num * R_ * R_, st);
+void Engine::step_lane(Lane& ln, int slot0, int B, const StepIO& io, cudaStream_t st) {
+  track_lane(ln, slot0, B, io.x, io.cls, io.loc, io.mask, io.flags, st);
+  launch(st, 1, "select", "select", 0, 4.0 * B * 6.0 * cfg_.anchor_num * R_ * R_, [&] {
     launch_select(io.cls, io.loc, io.anchors, io.window, io.tsz, B, cfg_.anchor_num, R_, io.penalty_k,
                   io.window_influence, io.best, io.pos, io.rec, st);
-    ++launches_;
-  }
-  if (io.refine != nullptr) refine_lane(B, io.pos, io.refine, st);
-  if (io.mask_col != nullptr) {
-    launch_gather_mask_col(io.mask, io.pos, B, 3969, R_, io.mask_col, st);
-    ++launches_;
-  }
+  });
+  if (io.refine != nullptr) refine_lane(ln, B, io.pos, io.refine, st);
+  if (io.mask_col != nullptr)
+    launch(st, 1, [&] { launch_gather_mask_col(io.mask, io.pos, B, 3969, R_, io.mask_col, st); });
 }
 
 void Engine::do_step(int slot0, int B, const StepIO& io, cudaStream_t st) {
@@ -1577,28 +1536,20 @@ void Engine::do_step(int slot0, int B, const StepIO& io, cudaStream_t st) {
                                      (uint64_t)io.loc, (uint64_t)io.mask, (uint64_t)io.flags, (uint64_t)io.pos,
                                      (uint64_t)io.rec, (uint64_t)io.refine, (uint64_t)io.mask_col, (uint64_t)st,
                                      (uint64_t)io.anchors, (uint64_t)io.window};
+  const size_t S = cfg_.search_size, A = cfg_.anchor_num, RR = (size_t)R_ * R_;
   run_with_graph(key, st, [&] {
     split_batch(B);
-    LaneGuard guard{this, st};
-    const size_t S = cfg_.search_size, A = cfg_.anchor_num, RR = (size_t)R_ * R_;
-    fork_lanes(st);
-    for (int l = split_n_ - 1; l >= 0; --l) {
-      cur_ = &lanes_[l];
-      const int b0 = split_off_[l], nbat = split_off_[l + 1] - split_off_[l];
-      cudaStream_t ls = (l == 0 || !concurrent()) ? st : lanes_[l].own;
-      step_lane(slot0 + b0, nbat, slice_io(io, b0, S, A, RR), ls);
-    }
-    cur_ = &lanes_[0];
-    guard.armed = false;
-    join_forked(st);
-    last_B_ = B;
-    have_mask_feats_ = want_feats || want_head;
+    run_lanes(st, kJoined, [&](Lane& ln, int b0, int nbat, cudaStream_t ls) {
+      step_lane(ln, slot0 + b0, nbat, slice_io(io, b0, S, A, RR), ls);
+    });
+    state_.last_B = B;
+    state_.have_mask_feats = want_feats || want_head;
   });
 }
 
 // Host-buffer form of do_step (pinned buffers recommended): H2D of the frames and of target_sz*scale_x, the whole
 // frame on the device, D2H of the per-stream records (+ refine logits / mask column / cls / loc when asked for).
-// Same ticket / staging-set protocol as track_host_async.
+// Same ticket / staging-set protocol as track_host_async (host_call).
 int Engine::step_host_async(int slot0, int B, const sm_step_io& h, cudaStream_t st) {
   const size_t S = cfg_.search_size, A = cfg_.anchor_num, RR = (size_t)R_ * R_;
   SMK_CHECK(B >= 1 && B <= cfg_.max_batch, "batch");
@@ -1611,11 +1562,7 @@ int Engine::step_host_async(int slot0, int B, const sm_step_io& h, cudaStream_t 
   SMK_CHECK(h.mask_col_host == nullptr || want_head, "mask column needs SM_TRACK_MASK_HEAD");
   if (want_head && mask_raw_ == nullptr)
     SMK_CUDA(cudaMalloc(&mask_raw_, (size_t)cfg_.max_batch * 3969 * RR * sizeof(float)));
-  const int t = (int)(host_calls_++ & 1);
-  if (set_busy_[t]) host_wait(t);
-  SMK_CUDA(cudaMemcpyAsync(stage_x_[t], h.x_host, (size_t)B * 3 * S * S * sizeof(float), cudaMemcpyHostToDevice, h2d_stream_));
-  SMK_CUDA(cudaMemcpyAsync(stage_tsz_[t], h.tsz_host, (size_t)B * 2 * sizeof(double), cudaMemcpyHostToDevice, h2d_stream_));
-  SMK_CUDA(cudaEventRecord(h2d_done_[t], h2d_stream_));
+  const int t = next_set();
   StepIO io;
   io.x = stage_x_[t]; io.tsz = stage_tsz_[t]; io.anchors = h.anchors_dev; io.window = h.window_dev;
   io.penalty_k = h.penalty_k; io.window_influence = h.window_influence; io.flags = h.flags;
@@ -1623,40 +1570,19 @@ int Engine::step_host_async(int slot0, int B, const sm_step_io& h, cudaStream_t 
   io.best = stage_best_[t]; io.pos = stage_pos_[t]; io.rec = stage_rec_[t];
   io.refine = h.refine_host != nullptr ? stage_mask_[t] : nullptr;
   io.mask_col = h.mask_col_host != nullptr ? stage_maskcol_[t] : nullptr;
-  if (lanes_for(n_lanes_, B) >= 2 && !use_graphs_ && concurrent()) {
-    split_batch(B);
-    for (int l = split_n_ - 1; l >= 0; --l) {
-      cur_ = &lanes_[l];
-      cudaStream_t ls = cur_->own;
-      const int b0 = split_off_[l], nbat = split_off_[l + 1] - split_off_[l];
-      order_after(st, ls);
-      SMK_CUDA(cudaStreamWaitEvent(ls, h2d_done_[t], 0));
-      step_lane(slot0 + b0, nbat, slice_io(io, b0, S, A, RR), ls);
-      SMK_CUDA(cudaEventRecord(lane_done_[t][l], ls));
-      SMK_CUDA(cudaStreamWaitEvent(d2h_stream_, lane_done_[t][l], 0));
-    }
-    cur_ = &lanes_[0];
-    last_B_ = B;
-    have_mask_feats_ = want_feats || want_head;
-    lanes_dirty_ = true;
-  } else {
-    SMK_CUDA(cudaStreamWaitEvent(st, h2d_done_[t], 0));
-    do_step(slot0, B, io, st);
-    SMK_CUDA(cudaEventRecord(compute_done_[t], st));
-    SMK_CUDA(cudaStreamWaitEvent(d2h_stream_, compute_done_[t], 0));
-  }
-  SMK_CUDA(cudaMemcpyAsync(h.records_host, stage_rec_[t], (size_t)B * 8 * sizeof(float), cudaMemcpyDeviceToHost, d2h_stream_));
-  if (h.refine_host)
-    SMK_CUDA(cudaMemcpyAsync(h.refine_host, stage_mask_[t], (size_t)B * 127 * 127 * sizeof(float), cudaMemcpyDeviceToHost, d2h_stream_));
-  if (h.mask_col_host)
-    SMK_CUDA(cudaMemcpyAsync(h.mask_col_host, stage_maskcol_[t], (size_t)B * 3969 * sizeof(float), cudaMemcpyDeviceToHost, d2h_stream_));
-  if (h.cls_host)
-    SMK_CUDA(cudaMemcpyAsync(h.cls_host, stage_cls_[t], (size_t)B * 2 * A * RR * sizeof(float), cudaMemcpyDeviceToHost, d2h_stream_));
-  if (h.loc_host)
-    SMK_CUDA(cudaMemcpyAsync(h.loc_host, stage_loc_[t], (size_t)B * 4 * A * RR * sizeof(float), cudaMemcpyDeviceToHost, d2h_stream_));
-  SMK_CUDA(cudaEventRecord(d2h_done_[t], d2h_stream_));
-  set_busy_[t] = true;
-  return t;
+  return host_call(
+      t, B, want_feats || want_head, st,
+      {{stage_x_[t], h.x_host, (size_t)B * 3 * S * S * sizeof(float)},
+       {stage_tsz_[t], h.tsz_host, (size_t)B * 2 * sizeof(double)}},
+      {{h.records_host, stage_rec_[t], (size_t)B * 8 * sizeof(float)},
+       {h.refine_host, stage_mask_[t], (size_t)B * 127 * 127 * sizeof(float)},
+       {h.mask_col_host, stage_maskcol_[t], (size_t)B * 3969 * sizeof(float)},
+       {h.cls_host, stage_cls_[t], (size_t)B * 2 * A * RR * sizeof(float)},
+       {h.loc_host, stage_loc_[t], (size_t)B * 4 * A * RR * sizeof(float)}},
+      [&] { do_step(slot0, B, io, st); },
+      [&](Lane& ln, int b0, int nbat, cudaStream_t ls) {
+        step_lane(ln, slot0 + b0, nbat, slice_io(io, b0, S, A, RR), ls);
+      });
 }
 
 void Engine::do_export(const char* what, float* out, int64_t* shape4, cudaStream_t st) {
@@ -1664,19 +1590,18 @@ void Engine::do_export(const char* what, float* out, int64_t* shape4, cudaStream
   if (std::string(what) == "zf") {
     SMK_CHECK(have_zf_, "no cached tensor named 'zf'");
     if (shape4 != nullptr) { shape4[0] = zf_.B; shape4[1] = zf_.C; shape4[2] = zf_.H; shape4[3] = zf_.W; }
-    if (out != nullptr) { launch_split_to_f32(zf_, out, st, std::ldexp(1.f, -zf_.sexp)); ++launches_; }
+    if (out != nullptr) launch(st, 1, [&] { launch_split_to_f32(zf_, out, st, std::ldexp(1.f, -zf_.sexp)); });
     return;
   }
   int total_B = 0;
-  for (int l = 0; l < split_n_; ++l) {       // the lanes hold consecutive blocks of streams
-    auto it = lanes_[l].named.find(what);
-    SMK_CHECK(it != lanes_[l].named.end(), std::string("no cached tensor named '") + what + "'");
+  for (int l = 0; l < state_.split_n; ++l) {       // the lanes hold consecutive blocks of streams
+    const std::map<std::string, Act>& named = state_.named[l];
+    auto it = named.find(what);
+    SMK_CHECK(it != named.end(), std::string("no cached tensor named '") + what + "'");
     const Act& a = it->second;
     if (shape4 != nullptr) { shape4[1] = a.C; shape4[2] = a.H; shape4[3] = a.W; }
-    if (out != nullptr) {
-      launch_split_to_f32(a, out + (size_t)total_B * a.C * a.H * a.W, st, std::ldexp(1.f, -a.sexp));
-      ++launches_;
-    }
+    if (out != nullptr)
+      launch(st, 1, [&] { launch_split_to_f32(a, out + (size_t)total_B * a.C * a.H * a.W, st, std::ldexp(1.f, -a.sexp)); });
     total_B += a.B;
   }
   if (shape4 != nullptr) shape4[0] = total_B;
@@ -1769,7 +1694,7 @@ static void conv2d_op(const float* x, const float* w, const float* scale, const 
   SMK_CUDA(cudaGetDevice(&dev));
   SMK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   (void)Ho; (void)Wo;
-  if (use_gemm && patch_conv_mode() != 0 && patch_conv_supported(in, g)) {
+  if (use_gemm && patch_conv_supported(in, g)) {
     // the engine runs this geometry on the resident-patch kernel (NHWC split output): same here, then export
     Act o;
     o.B = B; o.H = Ho; o.W = Wo; o.C = Cout;
@@ -1812,6 +1737,11 @@ struct sm_engine {
     return -1;                                      \
   }
 
+static void require_device() {
+  int ndev = 0;
+  SMK_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0, "no CUDA device: siammask_b200 has no CPU fallback");
+}
+
 extern "C" {
 
 const char* sm_last_error(void) { return smk::g_last_error.c_str(); }
@@ -1820,9 +1750,7 @@ const char* sm_version(void) { return "siammask_b200 0.1 (sm_90a)"; }
 int sm_engine_create(const sm_config* cfg, sm_engine** out) {
   SM_API_BEGIN
   SMK_CHECK(cfg != nullptr && out != nullptr, "null argument");
-  int ndev = 0;
-  cudaError_t err = cudaGetDeviceCount(&ndev);
-  SMK_CHECK(err == cudaSuccess && ndev > 0, "no CUDA device: siammask_b200 has no CPU fallback");
+  require_device();
   auto* e = new sm_engine;
   try {
     e->impl.reset(new smk::Engine(*cfg));
@@ -1943,8 +1871,7 @@ int sm_xcorr_depthwise(const float* x, const float* k, float* out, int32_t B, in
                        int32_t kw, void* stream) {
   SM_API_BEGIN
   SMK_CHECK(x && k && out, "null argument");
-  int ndev = 0;
-  SMK_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0, "no CUDA device: siammask_b200 has no CPU fallback");
+  require_device();
   smk::launch_xcorr_nchw_f32(x, k, out, B * C, H, W, kh, kw, static_cast<cudaStream_t>(stream));
   SM_API_END
 }
@@ -1954,8 +1881,7 @@ int sm_conv2d(const float* x, const float* w, const float* scale, const float* s
               int32_t relu, int32_t backend, int32_t precision, void* stream) {
   SM_API_BEGIN
   SMK_CHECK(x && w && out, "null argument");
-  int ndev = 0;
-  SMK_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0, "no CUDA device: siammask_b200 has no CPU fallback");
+  require_device();
   smk::conv2d_op(x, w, scale, shift, out, B, Cin, H, W, Cout, KH, KW, stride, pad, dil, relu, backend, precision,
                  static_cast<cudaStream_t>(stream));
   SM_API_END
@@ -1965,8 +1891,7 @@ int sm_crop_resize(const uint8_t* frames, size_t frame_stride, int32_t H, int32_
                    int32_t model_size, float* out, void* stream) {
   SM_API_BEGIN
   SMK_CHECK(frames && boxes && out && B >= 1 && H > 0 && W > 0 && model_size > 0, "bad argument");
-  int ndev = 0;
-  SMK_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0, "no CUDA device: siammask_b200 has no CPU fallback");
+  require_device();
   smk::launch_crop_resize(frames, frame_stride, H, W, boxes, B, model_size, out, static_cast<cudaStream_t>(stream));
   SM_API_END
 }
@@ -1975,8 +1900,7 @@ int sm_warp_affine(const float* src, int32_t src_h, int32_t src_w, const double*
                    int32_t dst_w, float border_value, int32_t B, void* stream) {
   SM_API_BEGIN
   SMK_CHECK(src && maps && dst && B >= 1 && src_h > 0 && src_w > 0 && dst_h > 0 && dst_w > 0, "bad argument");
-  int ndev = 0;
-  SMK_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0, "no CUDA device: siammask_b200 has no CPU fallback");
+  require_device();
   smk::launch_warp_affine(src, src_h, src_w, maps, dst, dst_h, dst_w, border_value, B, static_cast<cudaStream_t>(stream));
   SM_API_END
 }
@@ -1993,8 +1917,7 @@ int sm_tracker_prepare(int32_t B, const double* state, const int32_t* avg_chans,
                        double* target_sz_in_crop, double* aux, void* stream) {
   SM_API_BEGIN
   SMK_CHECK(state && avg_chans && hp && boxes && target_sz_in_crop && aux && B >= 1, "bad argument");
-  int ndev = 0;
-  SMK_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0, "no CUDA device: siammask_b200 has no CPU fallback");
+  require_device();
   smk::launch_tracker_prepare(B, state, avg_chans, to_hp(hp), boxes, target_sz_in_crop, aux, static_cast<cudaStream_t>(stream));
   SM_API_END
 }
@@ -2004,8 +1927,7 @@ int sm_tracker_update(int32_t B, double* state, const float* records, const doub
                       void* stream) {
   SM_API_BEGIN
   SMK_CHECK(state && records && aux && im_wh && hp && B >= 1 && score_size >= 1, "bad argument");
-  int ndev = 0;
-  SMK_CHECK(cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0, "no CUDA device: siammask_b200 has no CPU fallback");
+  require_device();
   smk::launch_tracker_update(B, state, records, aux, im_wh, to_hp(hp), anchor_num, score_size, maps, out,
                              static_cast<cudaStream_t>(stream));
   SM_API_END
@@ -2017,9 +1939,9 @@ int sm_select(sm_engine* e, int32_t B, const float* cls, const float* loc, const
   SM_API_BEGIN
   SMK_CHECK(e && cls && loc && anchors && window && target_sz_in_crop && best_idx && pos && records, "null argument");
   SMK_CHECK(B >= 1, "batch");
-  const sm_config& c = e->impl->cfg();
-  const int R = (c.search_size - 127) / 8 + 9;
-  smk::launch_select(cls, loc, anchors, window, target_sz_in_crop, B, c.anchor_num, R, penalty_k, window_influence,
+  const smk::Engine& eng = *e->impl;
+  smk::launch_select(cls, loc, anchors, window, target_sz_in_crop, B, eng.cfg().anchor_num, eng.score_size(), penalty_k,
+                     window_influence,
                      best_idx, pos, records, static_cast<cudaStream_t>(stream));
   SM_API_END
 }

@@ -87,7 +87,7 @@ def test_batched_streams_and_slots(calib_sd):
 def test_two_lane_batch_matches_single_stream_runs(calib_sd):
     """B=17 (>= 16) is split 9 + 8 over the engine's two concurrent lanes: every stream must equal its own
     single-stream run (B=1 engine = one lane, already pinned to the oracle), intermediates are gathered across the
-    lanes, the graph-replay and host-buffer paths (lane 1 stays forked between track and refine) agree."""
+    lanes, the graph-replay and host-buffer paths (each lane runs its track and refine back to back) agree."""
     import ctypes as C
     from siammask_b200 import _lib
     B = 17
