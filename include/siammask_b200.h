@@ -74,7 +74,9 @@ int sm_engine_adopt_weights(sm_engine* e);
  * free at run time and results are unchanged.  Needs the weights to have come through sm_engine_load_weights on this
  * engine; the scales travel inside the weight arena (broadcast / packed file).
  * sm_engine_status: synchronises and returns flags; bit 0 = some activation left fp16's range since the last calibrate /
- * engine creation (results invalid: calibrate with representative data). */
+ * engine creation (results invalid: calibrate with representative data); bit 1 = a slot table passed to
+ * sm_template_slots / sm_step_slots held an entry outside [0, num_slots): that stream was skipped and its outputs are
+ * undefined. */
 int sm_engine_calibrate(sm_engine* e, int32_t B, const float* z_nchw, const float* x_nchw, void* stream);
 int sm_engine_status(sm_engine* e, int32_t* flags);
 
@@ -82,6 +84,11 @@ int sm_engine_status(sm_engine* e, int32_t* flags);
  * slot0..slot0+B-1, the template feature and the three conv_kernel outputs (models/rpn.py:64),
  * which the reference recomputes every frame. */
 int sm_template(sm_engine* e, int32_t slot0, int32_t B, const float* z_nchw, void* stream);
+
+/* sm_template with a slot table: stream b's kernels are cached in slot slots[b].  slots: device int32 [B], owned by the
+ * caller; precondition: entries distinct and in [0, num_slots) (an entry out of range skips that stream and sets bit 1
+ * of sm_engine_status).  Lets tracker streams join a running batch in any free slots. */
+int sm_template_slots(sm_engine* e, int32_t B, const int32_t* slots, const float* z_nchw, void* stream);
 
 /* Custom.track / Custom.track_mask — custom.py:176-186.  x: device f32 [B,3,S,S] paired with slots
  * slot0..slot0+B-1.  cls: f32 [B,2A,R,R], loc: f32 [B,4A,R,R], mask: f32 [B,3969,R,R] or NULL.
@@ -102,11 +109,40 @@ int sm_refine(sm_engine* e, int32_t B, const int32_t* pos, float* out, void* str
 int sm_crop_resize(const uint8_t* frames, size_t frame_stride, int32_t H, int32_t W, const int32_t* boxes, int32_t B,
                    int32_t model_size, float* out, void* stream);
 
+/* sm_crop_resize where stream b crops frame frame_idx[b] (device int32 [B]; each entry indexes a frame that exists):
+ * K objects of G videos read the G frames in place instead of a per-stream copy. */
+int sm_crop_resize_indexed(const uint8_t* frames, size_t frame_stride, int32_t H, int32_t W, const int32_t* frame_idx,
+                           const int32_t* boxes, int32_t B, int32_t model_size, float* out, void* stream);
+
 /* Mask paste-back — crop_back() in siamese_track, tools/test.py:263-282: cv2.warpAffine(src f32 [B][src_h][src_w],
  * maps f64 [B][6] (forward 2x3 maps, device), (dst_w, dst_h), INTER_LINEAR, BORDER_CONSTANT, border_value), bit-exact
  * with OpenCV's fixed-point coordinate generation.  dst f32 [B][dst_h][dst_w].  All device pointers. */
 int sm_warp_affine(const float* src, int32_t src_h, int32_t src_w, const double* maps, float* dst, int32_t dst_h,
                    int32_t dst_w, float border_value, int32_t B, void* stream);
+
+/* Multi-object label map of track_vos — tools/test.py:480-523 — fused with the paste-back, for G videos of one frame
+ * size H x W.  The objects of video g are entries obj_offsets[g] .. obj_offsets[g+1]-1 (device int32 [G+1]) of objects
+ * (device int32 [n][2] = {kind, arg}):
+ *   SM_OBJ_TRACKED: arg = row of masks f32 [rows][side][side] (sigmoid masks) and maps f64 [rows][6] (forward maps of
+ *                   sm_tracker_update); value = cv2.warpAffine(mask, map, (W, H), INTER_LINEAR, BORDER_CONSTANT, -1),
+ *                   bit for bit with sm_warp_affine;
+ *   SM_OBJ_INIT:    arg = label id; value = anno[g] == id ? 1 : 0 (anno uint8 [G][H][W]; may be NULL without such objects);
+ *   SM_OBJ_IDLE:    value = -1.
+ * labels uint8 [G][H][W] = (first argmax over the video's objects + 1) * (max > seg_thr), compared in double like the
+ * reference's float64 pred_masks; label k+1 is the video's k-th object, not its annotation id.  Precondition: at most
+ * 255 objects per video (a video with more is labelled 0 everywhere instead of with wrapped labels).  Per-object
+ * frames are never materialised.  Objects whose four taps all miss the mask are skipped at that pixel, which is exact
+ * for seg_thr >= -1 (required). */
+enum { SM_OBJ_IDLE = 0, SM_OBJ_TRACKED = 1, SM_OBJ_INIT = 2 };
+int sm_paste_labels(const float* masks, int32_t side, const double* maps, const uint8_t* anno, const int32_t* obj_offsets,
+                    const int32_t* objects, int32_t G, int32_t H, int32_t W, double seg_thr, uint8_t* labels,
+                    void* stream);
+
+/* Init boxes of track_vos (tools/test.py:483-496): for each query q = (video g, label id) of queries (device int32
+ * [Q][2]), boxes[q] (device int32 [Q][4]) = x, y, w, h = cv2.boundingRect(anno[g] == id); (0, 0, 0, 0) when no pixel
+ * carries the id. */
+int sm_label_boxes(const uint8_t* anno, int32_t G, int32_t H, int32_t W, const int32_t* queries, int32_t Q, int32_t* boxes,
+                   void* stream);
 
 /* Score / box post-processing + argmax of siamese_track — tools/test.py:205-254 — on the device, so that
  * sm_track -> sm_select -> sm_refine needs no host round trip.  All pointers are device pointers:
@@ -148,6 +184,14 @@ int sm_step(sm_engine* e, int32_t slot0, int32_t B, const float* x_nchw, const d
             const float* anchors, const float* window, double penalty_k, double window_influence, int32_t flags,
             float* cls, float* loc, float* mask, int32_t* best_idx, int32_t* pos, float* records, float* refine_out,
             float* mask_col, void* stream);
+
+/* sm_step with a slot table: stream b correlates with the template cached in slot slots[b] (device int32 [B], caller
+ * owned, entries in [0, num_slots); out-of-range entries as in sm_template_slots).  Under graph replay the table's
+ * contents are read at run time, so a caller may rewrite it between calls that reuse the same pointer. */
+int sm_step_slots(sm_engine* e, int32_t B, const int32_t* slots, const float* x_nchw, const double* target_sz_in_crop,
+                  const float* anchors, const float* window, double penalty_k, double window_influence, int32_t flags,
+                  float* cls, float* loc, float* mask, int32_t* best_idx, int32_t* pos, float* records, float* refine_out,
+                  float* mask_col, void* stream);
 
 /* The same frame through HOST buffers: H2D of x and target_sz_in_crop, sm_step on staging buffers, D2H of the
  * records (always) and of whichever of refine / mask_col / cls / loc are non-NULL.  anchors / window stay device

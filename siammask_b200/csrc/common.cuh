@@ -49,6 +49,8 @@ struct Epilogue {
 __device__ __forceinline__ void flag_if_out_of_range(float absmax, int* ovf) {
   if (ovf != nullptr && !(absmax <= 65504.f)) atomicOr(ovf, 1);
 }
+// the same status word, bit 1: a slot table entry outside [0, num_slots) was skipped (sm_engine_status)
+constexpr int kStatusBadSlot = 2;
 
 // One K-segment of the implicit GEMM (see conv_gemm_sm90.cu).
 struct GemmSegment {
@@ -143,8 +145,18 @@ void launch_ref_conv(const Act& in, const ConvGeom& g, const float* w_krsc_cout,
 void launch_stem(const float* x_nchw, int B, int S, const float* w, const float* alpha, const float* beta, Act out,
                  cudaStream_t st);
 void launch_maxpool3s2(const Act& in, Act out, cudaStream_t st);
+// slots == nullptr: stream b correlates with the kernel at k + b * kh*kw*C; else with the kernel at k + slots[b] * ...,
+// and an entry outside [0, num_slots) skips the stream and sets kStatusBadSlot in *ovf
 void launch_xcorr_nhwc(const Act& x, int c_off, const __half* k_hi, const __half* k_lo, int kh, int kw, Act out,
-                       float mul, int* ovf, cudaStream_t st);
+                       float mul, int* ovf, cudaStream_t st, const int32_t* slots = nullptr, int num_slots = 0);
+// sm_template_slots: src [B][n] split planes -> dst + slots[b] * n (guarded like launch_xcorr_nhwc)
+void launch_scatter_slots(const __half* src_hi, const __half* src_lo, __half* dst_hi, __half* dst_lo,
+                          const int32_t* slots, int B, int num_slots, int n, int* status, cudaStream_t st);
+// sm_paste_labels / sm_label_boxes (include/siammask_b200.h)
+void launch_paste_labels(const float* masks, int side, const double* maps, const uint8_t* anno, const int32_t* obj_off,
+                         const int32_t* objects, int G, int H, int W, double seg_thr, uint8_t* labels, cudaStream_t st);
+void launch_label_boxes(const uint8_t* anno, int G, int H, int W, const int32_t* queries, int Q, int32_t* boxes,
+                        cudaStream_t st);
 void launch_absmax(const Act& a, float* slot, cudaStream_t st);
 void launch_xcorr_nchw_f32(const float* x, const float* k, float* out, int planes, int H, int W, int kh, int kw,
                            cudaStream_t st);
@@ -165,8 +177,9 @@ void launch_tracker_prepare(int B, const double* state, const int32_t* avg, cons
                             double* tsz, double* aux, cudaStream_t st);
 void launch_tracker_update(int B, double* state, const float* rec, const double* aux, const int32_t* imsize,
                            const TrackerHp& hp, int A, int R, double* maps, double* out, cudaStream_t st);
+// frame_idx == nullptr: stream b crops frames + b * frame_stride; else frames + frame_idx[b] * frame_stride
 void launch_crop_resize(const uint8_t* frames, size_t frame_stride, int H, int W, const int32_t* box, int B, int model,
-                        float* out, cudaStream_t st);
+                        float* out, cudaStream_t st, const int32_t* frame_idx = nullptr);
 void launch_select(const float* cls, const float* loc, const float* anchors, const float* window, const double* tsz,
                    int B, int A, int R, double penalty_k, double window_influence, int32_t* best_idx, int32_t* pos,
                    float* rec, cudaStream_t st);

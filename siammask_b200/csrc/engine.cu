@@ -111,7 +111,8 @@ class Engine {
   int status();
   void weight_blob(void** p, size_t* bytes) { *p = blob_; *bytes = blob_bytes_; }
 
-  void do_template(int slot0, int B, const float* z, cudaStream_t st);
+  // slots == nullptr: streams b -> slot0 + b; else the device table slots[b] (sm_template_slots / sm_step_slots)
+  void do_template(int slot0, int B, const float* z, cudaStream_t st, const int32_t* slots = nullptr);
   void do_track(int slot0, int B, const float* x, float* cls, float* loc, float* mask, int flags, cudaStream_t st);
   void do_refine(int B, const int32_t* pos, float* out, cudaStream_t st);
   void set_graphs(bool on) { use_graphs_ = on; }
@@ -133,7 +134,7 @@ class Engine {
     float* refine = nullptr;             // [B][127*127] or null
     float* mask_col = nullptr;           // [B][3969] = mask[b, :, dy, dx] or null
   };
-  void do_step(int slot0, int B, const StepIO& io, cudaStream_t st);
+  void do_step(int slot0, int B, const StepIO& io, cudaStream_t st, const int32_t* slots = nullptr);
   int step_host_async(int slot0, int B, const sm_step_io& io, cudaStream_t st);
   void do_export(const char* what, float* out, int64_t* shape4, cudaStream_t st);
 
@@ -219,6 +220,9 @@ class Engine {
   // per-slot template caches: [branch][slot][5][5][256] split planes, and zf for export
   __half* kcache_hi_ = nullptr;
   __half* kcache_lo_ = nullptr;
+  // contiguous conv_kernel outputs of a sm_template_slots call, [branch][B][5][5][256] hi then lo, scattered into the
+  // per-slot cache through the slot table (allocated on first use)
+  __half* kscatter_ = nullptr;
   int n_branches_ = 2;
   // host-path staging
   // two sets (ping-pong) so the H2D of step k+1 and the D2H of step k overlap the compute of the other step
@@ -232,7 +236,7 @@ class Engine {
   int32_t* stage_best_[2] = {nullptr, nullptr};
   float* stage_maskcol_[2] = {nullptr, nullptr};
   float* mask_raw_ = nullptr;          // [max_batch][3969][R][R] raw mask-head output of the host-buffer step (lazy)
-  void step_lane(Lane& ln, int slot0, int B, const StepIO& io, cudaStream_t st);
+  void step_lane(Lane& ln, int slot0, int B, const StepIO& io, cudaStream_t st, const int32_t* slots = nullptr);
   void release();
   cudaStream_t h2d_stream_ = nullptr, d2h_stream_ = nullptr;
   cudaEvent_t h2d_done_[2] = {nullptr, nullptr}, d2h_done_[2] = {nullptr, nullptr};
@@ -278,7 +282,7 @@ class Engine {
   bool use_graphs_ = false;
   std::map<std::vector<uint64_t>, GraphEntry> graphs_;
   void track_lane(Lane& ln, int slot0, int B, const float* x, float* cls, float* loc, float* mask, int flags,
-                  cudaStream_t st);
+                  cudaStream_t st, const int32_t* slots = nullptr);
   void refine_lane(Lane& ln, int B, const int32_t* pos, float* out, cudaStream_t st);
   // host-buffer path with two lanes: both lanes run on their own streams and are never joined into the caller's
   // stream — each only waits for its inputs, the D2H waits for both — so consecutive steps of the two lanes slide
@@ -620,6 +624,7 @@ void Engine::release() {
   }
   cudaFree(kcache_hi_);
   cudaFree(kcache_lo_);
+  cudaFree(kscatter_);
   for (int i = 0; i < 2; ++i) {
     cudaFree(stage_x_[i]); cudaFree(stage_cls_[i]); cudaFree(stage_loc_[i]); cudaFree(stage_mask_[i]); cudaFree(stage_pos_[i]);
     cudaFree(stage_tsz_[i]); cudaFree(stage_rec_[i]); cudaFree(stage_best_[i]); cudaFree(stage_maskcol_[i]);
@@ -652,7 +657,7 @@ void Engine::size_arenas() {
     probe.search.measure = probe.refine.measure = true;
     const int B = lanes_[l].cap_B;
     for (int flags = 0; flags <= max_flags; ++flags)
-      track_lane(probe, 0, B, nullptr, nullptr, nullptr, nullptr, flags, nullptr);
+      track_lane(probe, 0, B, nullptr, nullptr, nullptr, nullptr, flags, nullptr, nullptr);
     float out;                         // refine_lane's last layer writes the caller's buffer, not the arena
     if (cfg_.with_mask) refine_lane(probe, B, nullptr, &out, nullptr);
     lanes_[l].search.cap = align_up(probe.search.peak + (1u << 20));
@@ -1180,10 +1185,17 @@ Act Engine::backbone(const float* x, int B, int S, Arena& ar, std::map<std::stri
 static const char* kBranch[3] = {"rpn_model.cls.", "rpn_model.loc.", "mask_model.mask."};
 static const char* kCorrName[3] = {"corr_cls", "corr_loc", "corr_mask"};
 
-void Engine::do_template(int slot0, int B, const float* z, cudaStream_t st) {
+void Engine::do_template(int slot0, int B, const float* z, cudaStream_t st, const int32_t* slots) {
   SMK_CHECK(weights_ready_, "weights not loaded");
-  SMK_CHECK(B >= 1 && B <= cfg_.max_batch && slot0 >= 0 && slot0 + B <= cfg_.num_slots, "template batch/slot range");
+  SMK_CHECK(B >= 1 && B <= cfg_.max_batch && (slots != nullptr || (slot0 >= 0 && slot0 + B <= cfg_.num_slots)),
+            "template batch/slot range");
   join_lanes(st);
+  const size_t kslot = 25 * 256;               // halves of one slot's cached kernel, per plane
+  if (slots != nullptr && kscatter_ == nullptr) {
+    const size_t n = (size_t)n_branches_ * cfg_.max_batch * kslot;
+    SMK_CUDA(cudaMalloc(&kscatter_, 2 * n * sizeof(__half)));
+    total_bytes_ += 2 * n * sizeof(__half);
+  }
   templ_arena_.reset();
   Act zf = backbone(z, B, 127, templ_arena_, nullptr, st);
   SMK_CHECK(zf.H == 7 && zf.W == 7, "template feature must be 7x7");
@@ -1194,10 +1206,23 @@ void Engine::do_template(int slot0, int B, const float* z, cudaStream_t st) {
     Epilogue ep;
     ep.relu = 1;
     ep.out_mode = OUT_NHWC_SPLIT;
-    const size_t off = ((size_t)br * cfg_.num_slots + slot0) * 25 * 256;
-    ep.out_hi = kcache_hi_ + off;
-    ep.out_lo = exact_ ? kcache_lo_ + off : nullptr;
+    if (slots == nullptr) {
+      const size_t off = ((size_t)br * cfg_.num_slots + slot0) * kslot;
+      ep.out_hi = kcache_hi_ + off;
+      ep.out_lo = exact_ ? kcache_lo_ + off : nullptr;
+    } else {                                   // contiguous write, then a scatter through the table
+      const size_t n = (size_t)n_branches_ * cfg_.max_batch * kslot;
+      ep.out_hi = kscatter_ + (size_t)br * cfg_.max_batch * kslot;
+      ep.out_lo = exact_ ? ep.out_hi + n : nullptr;
+    }
     conv_into(zf, ck, ep, st);
+    if (slots != nullptr) {
+      const size_t cache_off = (size_t)br * cfg_.num_slots * kslot;
+      launch(st, 1, "scatter_slots", "misc", 0, 2.0 * 2 * B * kslot * (exact_ ? 2 : 1), [&] {
+        launch_scatter_slots(ep.out_hi, ep.out_lo, kcache_hi_ + cache_off, exact_ ? kcache_lo_ + cache_off : nullptr,
+                             slots, B, cfg_.num_slots, (int)kslot, ovf_flag_, st);
+      });
+    }
     if (calibrating_) {
       Act kc;
       kc.hi = ep.out_hi; kc.lo = ep.out_lo; kc.B = B; kc.H = 5; kc.W = 5; kc.C = 256;
@@ -1268,7 +1293,7 @@ void Engine::do_track(int slot0, int B, const float* x, float* cls, float* loc, 
 }
 
 void Engine::track_lane(Lane& ln, int slot0, int B, const float* x, float* cls, float* loc, float* mask, int flags,
-                        cudaStream_t st) {
+                        cudaStream_t st, const int32_t* slots) {
   const bool want_feats = (flags & SM_TRACK_MASK_FEATURES) != 0;
   const bool want_mask_head = (flags & SM_TRACK_MASK_HEAD) != 0;
   Arena& search_arena = ln.search;
@@ -1291,13 +1316,14 @@ void Engine::track_lane(Lane& ln, int slot0, int B, const float* x, float* cls, 
     const std::string P = kBranch[br];
     Act cs = use_cat ? cs_all : conv(xf, L(P + "conv_search.0"), true, nullptr, search_arena, bs);
     Act corr = alloc_act(search_arena, B, cs.H - 4, cs.W - 4, 256);
-    const size_t off = ((size_t)br * cfg_.num_slots + slot0) * 25 * 256;
+    // with a slot table the kernel indexes the branch's cache by slots[b]; without, stream b reads slot slot0 + b
+    const size_t off = ((size_t)br * cfg_.num_slots + (slots != nullptr ? 0 : slot0)) * 25 * 256;
     corr.sexp = tscale(kCorrName[br]);
     const int s_kc = L(P + "conv_kernel.0").s_out;
     launch(bs, 1, kCorrName[br], "xcorr", 2.0 * 25 * corr.numel(),
            4.0 * (2.0 * corr.numel() + (double)B * cs.H * cs.W * 256 + (double)B * 25 * 256), [&] {
       launch_xcorr_nhwc(cs, use_cat ? 256 * br : 0, kcache_hi_ + off, exact_ ? kcache_lo_ + off : nullptr, 5, 5, corr,
-                        std::ldexp(1.f, corr.sexp - cs.sexp - s_kc), ovf_flag_, bs);
+                        std::ldexp(1.f, corr.sexp - cs.sexp - s_kc), ovf_flag_, bs, slots, cfg_.num_slots);
       last_end_[corr.hi] = +1;
     });
     note_tensor(corr, kCorrName[br], bs);
@@ -1511,8 +1537,8 @@ Engine::StepIO slice_io(const Engine::StepIO& io, int b0, size_t S, size_t A, si
 }
 }  // namespace
 
-void Engine::step_lane(Lane& ln, int slot0, int B, const StepIO& io, cudaStream_t st) {
-  track_lane(ln, slot0, B, io.x, io.cls, io.loc, io.mask, io.flags, st);
+void Engine::step_lane(Lane& ln, int slot0, int B, const StepIO& io, cudaStream_t st, const int32_t* slots) {
+  track_lane(ln, slot0, B, io.x, io.cls, io.loc, io.mask, io.flags, st, slots);
   launch(st, 1, "select", "select", 0, 4.0 * B * 6.0 * cfg_.anchor_num * R_ * R_, [&] {
     launch_select(io.cls, io.loc, io.anchors, io.window, io.tsz, B, cfg_.anchor_num, R_, io.penalty_k,
                   io.window_influence, io.best, io.pos, io.rec, st);
@@ -1522,9 +1548,10 @@ void Engine::step_lane(Lane& ln, int slot0, int B, const StepIO& io, cudaStream_
     launch(st, 1, [&] { launch_gather_mask_col(io.mask, io.pos, B, 3969, R_, io.mask_col, st); });
 }
 
-void Engine::do_step(int slot0, int B, const StepIO& io, cudaStream_t st) {
+void Engine::do_step(int slot0, int B, const StepIO& io, cudaStream_t st, const int32_t* slots) {
   SMK_CHECK(weights_ready_, "weights not loaded");
-  SMK_CHECK(B >= 1 && B <= cfg_.max_batch && slot0 >= 0 && slot0 + B <= cfg_.num_slots, "step batch/slot range");
+  SMK_CHECK(B >= 1 && B <= cfg_.max_batch && (slots != nullptr || (slot0 >= 0 && slot0 + B <= cfg_.num_slots)),
+            "step batch/slot range");
   SMK_CHECK(io.x && io.tsz && io.anchors && io.window && io.cls && io.loc && io.best && io.pos && io.rec, "null argument");
   const bool want_feats = (io.flags & SM_TRACK_MASK_FEATURES) != 0, want_head = (io.flags & SM_TRACK_MASK_HEAD) != 0;
   SMK_CHECK(!(want_feats || want_head || io.refine) || cfg_.with_mask, "engine was built without the mask branch");
@@ -1535,12 +1562,12 @@ void Engine::do_step(int slot0, int B, const StepIO& io, cudaStream_t st) {
   const std::vector<uint64_t> key = {3, (uint64_t)slot0, (uint64_t)B, (uint64_t)io.x, (uint64_t)io.tsz, (uint64_t)io.cls,
                                      (uint64_t)io.loc, (uint64_t)io.mask, (uint64_t)io.flags, (uint64_t)io.pos,
                                      (uint64_t)io.rec, (uint64_t)io.refine, (uint64_t)io.mask_col, (uint64_t)st,
-                                     (uint64_t)io.anchors, (uint64_t)io.window};
+                                     (uint64_t)io.anchors, (uint64_t)io.window, (uint64_t)slots};
   const size_t S = cfg_.search_size, A = cfg_.anchor_num, RR = (size_t)R_ * R_;
   run_with_graph(key, st, [&] {
     split_batch(B);
     run_lanes(st, kJoined, [&](Lane& ln, int b0, int nbat, cudaStream_t ls) {
-      step_lane(ln, slot0 + b0, nbat, slice_io(io, b0, S, A, RR), ls);
+      step_lane(ln, slot0 + b0, nbat, slice_io(io, b0, S, A, RR), ls, slots != nullptr ? slots + b0 : nullptr);
     });
     state_.last_B = B;
     state_.have_mask_feats = want_feats || want_head;
@@ -1860,6 +1887,28 @@ int sm_step(sm_engine* e, int32_t slot0, int32_t B, const float* x, const double
   SM_API_END
 }
 
+int sm_template_slots(sm_engine* e, int32_t B, const int32_t* slots, const float* z, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(e && slots && z, "null argument");
+  e->impl->do_template(0, B, z, static_cast<cudaStream_t>(stream), slots);
+  SM_API_END
+}
+
+int sm_step_slots(sm_engine* e, int32_t B, const int32_t* slots, const float* x, const double* target_sz_in_crop,
+                  const float* anchors, const float* window, double penalty_k, double window_influence, int32_t flags,
+                  float* cls, float* loc, float* mask, int32_t* best_idx, int32_t* pos, float* records, float* refine_out,
+                  float* mask_col, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(e && slots, "null argument");
+  smk::Engine::StepIO io;
+  io.x = x; io.tsz = target_sz_in_crop; io.anchors = anchors; io.window = window;
+  io.penalty_k = penalty_k; io.window_influence = window_influence; io.flags = flags;
+  io.cls = cls; io.loc = loc; io.mask = mask; io.best = best_idx; io.pos = pos; io.rec = records;
+  io.refine = refine_out; io.mask_col = mask_col;
+  e->impl->do_step(0, B, io, static_cast<cudaStream_t>(stream), slots);
+  SM_API_END
+}
+
 int sm_step_host_async(sm_engine* e, int32_t slot0, int32_t B, const sm_step_io* io, void* stream, int32_t* ticket) {
   SM_API_BEGIN
   SMK_CHECK(e && io && ticket, "null argument");
@@ -1893,6 +1942,37 @@ int sm_crop_resize(const uint8_t* frames, size_t frame_stride, int32_t H, int32_
   SMK_CHECK(frames && boxes && out && B >= 1 && H > 0 && W > 0 && model_size > 0, "bad argument");
   require_device();
   smk::launch_crop_resize(frames, frame_stride, H, W, boxes, B, model_size, out, static_cast<cudaStream_t>(stream));
+  SM_API_END
+}
+
+int sm_crop_resize_indexed(const uint8_t* frames, size_t frame_stride, int32_t H, int32_t W, const int32_t* frame_idx,
+                           const int32_t* boxes, int32_t B, int32_t model_size, float* out, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(frames && frame_idx && boxes && out && B >= 1 && H > 0 && W > 0 && model_size > 0, "bad argument");
+  require_device();
+  smk::launch_crop_resize(frames, frame_stride, H, W, boxes, B, model_size, out, static_cast<cudaStream_t>(stream),
+                          frame_idx);
+  SM_API_END
+}
+
+int sm_paste_labels(const float* masks, int32_t side, const double* maps, const uint8_t* anno, const int32_t* obj_offsets,
+                    const int32_t* objects, int32_t G, int32_t H, int32_t W, double seg_thr, uint8_t* labels,
+                    void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(obj_offsets && objects && labels && G >= 1 && H > 0 && W > 0 && side > 0, "bad argument");
+  SMK_CHECK(seg_thr >= -1.0, "seg_thr must be >= -1 (objects that miss a pixel are skipped as value -1)");
+  require_device();
+  smk::launch_paste_labels(masks, side, maps, anno, obj_offsets, objects, G, H, W, seg_thr, labels,
+                           static_cast<cudaStream_t>(stream));
+  SM_API_END
+}
+
+int sm_label_boxes(const uint8_t* anno, int32_t G, int32_t H, int32_t W, const int32_t* queries, int32_t Q, int32_t* boxes,
+                   void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(anno && queries && boxes && G >= 1 && H > 0 && W > 0 && Q >= 1, "bad argument");
+  require_device();
+  smk::launch_label_boxes(anno, G, H, W, queries, Q, boxes, static_cast<cudaStream_t>(stream));
   SM_API_END
 }
 

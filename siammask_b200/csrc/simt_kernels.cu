@@ -2,8 +2,10 @@
 // large enough for the tensor pipe — the 3-channel 7x7 stem, max-pool, the bandwidth-bound depthwise
 // cross-correlation, the crops/gathers of the refine stage, its 1-32 channel 3x3 convs and the
 // 1x1 -> 15x15 transposed conv — plus a plain reference convolution used to bisect the tensor-core path.
+#include "../../include/siammask_b200.h"
 #include "common.cuh"
 
+#include <climits>
 #include <cmath>
 #include <type_traits>
 #include <cstdlib>
@@ -197,10 +199,19 @@ template <int KH, int KW, int NR, int SW, int NTHREADS>
 __global__ void __launch_bounds__(NTHREADS, 2) xcorr_nhwc_kernel(Act x, const __half* __restrict__ k_hi,
                                                                   const __half* __restrict__ k_lo, Act out,
                                                                   int band_rows, int c_off, float mul,
-                                                                  int* __restrict__ ovf) {
+                                                                  int* __restrict__ ovf,
+                                                                  const int32_t* __restrict__ slots, int num_slots) {
   constexpr int XC_CH = 32;
   extern __shared__ float xs[];                  // [(band rows + KH - 1) * W][32]
   const int b = blockIdx.y;
+  int kb = b;                                    // which cached template kernel this stream correlates with
+  if (slots != nullptr) {
+    kb = slots[b];
+    if (kb < 0 || kb >= num_slots) {             // block-uniform: the whole stream is skipped
+      if (threadIdx.x == 0 && blockIdx.x == 0 && blockIdx.z == 0 && ovf != nullptr) atomicOr(ovf, kStatusBadSlot);
+      return;
+    }
+  }
   const int c0 = blockIdx.x * XC_CH;
   const int y0 = blockIdx.z * band_rows;                             // first output row of this block's band
   const int Hob = min(band_rows, out.H - y0);                        // output rows of the band
@@ -253,7 +264,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) xcorr_nhwc_kernel(Act x, const __
 #pragma unroll
   for (int u = 0; u < KH; ++u)
 #pragma unroll
-    for (int v = 0; v < KW; ++v) kk[u][v] = split_load(k_hi, k_lo, (((size_t)b * KH + u) * KW + v) * out.C + c);
+    for (int v = 0; v < KW; ++v) kk[u][v] = split_load(k_hi, k_lo, (((size_t)kb * KH + u) * KW + v) * out.C + c);
   __syncthreads();
   const int Ho = Hob, Wo = out.W, W = x.W;
   // balanced task grid: row blocks of NR or NR-1 rows (25 -> 7,6,6,6), strips of SW or SW-1 columns; tasks are
@@ -817,15 +828,17 @@ __device__ __forceinline__ void cv_coeff(int d, double scale, int src_n, bool cl
   a1 = __float2int_rn(f * 2048.f);
 }
 
+// frame_idx (optional, sm_crop_resize_indexed): stream b crops frame frame_idx[b] instead of frame b.
 __global__ void crop_resize_kernel(const uint8_t* __restrict__ frames, size_t frame_stride, int H, int W,
-                                   const int32_t* __restrict__ box, int model, float* __restrict__ out) {
+                                   const int32_t* __restrict__ box, int model, float* __restrict__ out,
+                                   const int32_t* __restrict__ frame_idx) {
   const int b = blockIdx.z;
   const int dx = blockIdx.x * blockDim.x + threadIdx.x;
   const int dy = blockIdx.y * blockDim.y + threadIdx.y;
   if (dx >= model || dy >= model) return;
   const int32_t* bx = box + 8 * b;
   const int xmin = bx[0], ymin = bx[1], sz = bx[2];
-  const uint8_t* fr = frames + (size_t)b * frame_stride;
+  const uint8_t* fr = frames + (size_t)(frame_idx != nullptr ? frame_idx[b] : b) * frame_stride;
   auto px = [&](int y, int x, int c) -> int {      // pixel of the (virtual, padded) patch
     const int fy = y + ymin, fx = x + xmin;
     if (fy < 0 || fy >= H || fx < 0 || fx >= W) return bx[3 + c];
@@ -858,39 +871,192 @@ __global__ void crop_resize_kernel(const uint8_t* __restrict__ frames, size_t fr
 // inverted in double; source coordinates are generated in fixed point (AB_BITS = 10, 1/32-pixel sub-positions,
 // round_delta = 16); the four bilinear weights are float products of the 1-D (1 - f, f) tables; out-of-image taps
 // take the border value.  One thread per destination pixel; maps: double [B][6] on the device.
-__global__ void warp_affine_kernel(const float* __restrict__ src, int sh, int sw, const double* __restrict__ maps,
-                                   float* __restrict__ dst, int dh, int dw, float border) {
-  const int b = blockIdx.z;
-  const int x = blockIdx.x * blockDim.x + threadIdx.x;
-  const int y = blockIdx.y * blockDim.y + threadIdx.y;
-  if (x >= dw || y >= dh) return;
-  const double* m = maps + 6 * b;
+// The map inversion and the per-pixel body are shared with paste_labels_kernel (sm_paste_labels), which must produce
+// the same values bit for bit.
+__device__ __forceinline__ void warp_invert_map(const double* __restrict__ m, double inv[6]) {
   double M0 = m[0], M1 = m[1], M2 = m[2], M3 = m[3], M4 = m[4], M5 = m[5];
   double D = M0 * M4 - M1 * M3;
   D = D != 0.0 ? 1.0 / D : 0.0;
   const double A11 = M4 * D, A22 = M0 * D;
   M0 = A11; M1 *= -D; M3 *= -D; M4 = A22;
   const double b1 = -M0 * M2 - M1 * M5, b2 = -M3 * M2 - M4 * M5;
-  M2 = b1; M5 = b2;
-  const long long adelta = llrint(M0 * x * 1024.0), bdelta = llrint(M3 * x * 1024.0);
-  const long long X0 = llrint((M1 * y + M2) * 1024.0) + 16, Y0 = llrint((M4 * y + M5) * 1024.0) + 16;
+  inv[0] = M0; inv[1] = M1; inv[2] = b1; inv[3] = M3; inv[4] = M4; inv[5] = b2;
+}
+
+// Fixed-point source position of destination pixel (x, y): top-left tap (sx, sy) and the 1/32 fractions (X & 31, Y & 31).
+struct WarpTap {
+  long long sx, sy;
+  int fx, fy;
+  // false: all four taps lie outside a sh x sw source, so the pixel's value is exactly the border value when that is -1
+  // (the bilinear weights are multiples of 1/1024 that sum to 1)
+  __device__ __forceinline__ bool touches(int sh, int sw) const { return sx >= -1 && sx < sw && sy >= -1 && sy < sh; }
+};
+
+__device__ __forceinline__ WarpTap warp_tap(const double inv[6], int x, int y) {
+  const long long adelta = llrint(inv[0] * x * 1024.0), bdelta = llrint(inv[3] * x * 1024.0);
+  const long long X0 = llrint((inv[1] * y + inv[2]) * 1024.0) + 16, Y0 = llrint((inv[4] * y + inv[5]) * 1024.0) + 16;
   const long long X = (X0 + adelta) >> 5, Y = (Y0 + bdelta) >> 5;
   long long sx = X >> 5, sy = Y >> 5;
   sx = sx < -32768 ? -32768 : (sx > 32767 ? 32767 : sx);     // saturate_cast<short>
   sy = sy < -32768 ? -32768 : (sy > 32767 ? 32767 : sy);
-  const float fx = (float)(X & 31) / 32.f, fy = (float)(Y & 31) / 32.f;
+  return WarpTap{sx, sy, (int)(X & 31), (int)(Y & 31)};
+}
+
+__device__ __forceinline__ float warp_sample(const float* __restrict__ s, int sh, int sw, const WarpTap& t, float border) {
+  const float fx = (float)t.fx / 32.f, fy = (float)t.fy / 32.f;
   const float wx0 = 1.f - fx, wy0 = 1.f - fy;
   const float w00 = wy0 * wx0, w01 = wy0 * fx, w10 = fy * wx0, w11 = fy * fx;
-  const float* s = src + (size_t)b * sh * sw;
   auto px = [&](long long yy, long long xx) -> float {
     return (yy >= 0 && yy < sh && xx >= 0 && xx < sw) ? s[yy * sw + xx] : border;
   };
   // same evaluation order as remapBilinear (no fused multiply-add)
-  float v = __fmul_rn(px(sy, sx), w00);
-  v = __fadd_rn(v, __fmul_rn(px(sy, sx + 1), w01));
-  v = __fadd_rn(v, __fmul_rn(px(sy + 1, sx), w10));
-  v = __fadd_rn(v, __fmul_rn(px(sy + 1, sx + 1), w11));
-  dst[((size_t)b * dh + y) * dw + x] = v;
+  float v = __fmul_rn(px(t.sy, t.sx), w00);
+  v = __fadd_rn(v, __fmul_rn(px(t.sy, t.sx + 1), w01));
+  v = __fadd_rn(v, __fmul_rn(px(t.sy + 1, t.sx), w10));
+  v = __fadd_rn(v, __fmul_rn(px(t.sy + 1, t.sx + 1), w11));
+  return v;
+}
+
+__global__ void warp_affine_kernel(const float* __restrict__ src, int sh, int sw, const double* __restrict__ maps,
+                                   float* __restrict__ dst, int dh, int dw, float border) {
+  const int b = blockIdx.z;
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  const int y = blockIdx.y * blockDim.y + threadIdx.y;
+  if (x >= dw || y >= dh) return;
+  double inv[6];
+  warp_invert_map(maps + 6 * b, inv);
+  dst[((size_t)b * dh + y) * dw + x] = warp_sample(src + (size_t)b * sh * sw, sh, sw, warp_tap(inv, x, y), border);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Fused paste-back + label map of track_vos (tools/test.py:480-523): for every pixel of video g, the value of each of
+// the video's objects — the cv2.warpAffine(mask, map, INTER_LINEAR, BORDER_CONSTANT, -1) value of a tracked object
+// (warp_sample above, bit for bit), anno == id ? 1 : 0 for an object initialised this frame, -1 for an idle one — and
+// label = (first argmax + 1) * (max > seg_thr), compared in double as numpy compares the float64 pred_masks.  Objects
+// whose value at a pixel is -1 can never win for seg_thr >= -1 and are skipped: idle objects, and tracked objects none
+// of whose four taps falls inside the mask (per block first, conservatively, then exactly per pixel).  A NaN value makes
+// np.max NaN, hence label 0.  Block = 32 x 8 pixels of one video; objects are staged in shared memory in chunks, each
+// map inverted once per block.
+constexpr int PL_CHUNK = 64;
+
+__global__ void __launch_bounds__(256) paste_labels_kernel(const float* __restrict__ masks, int side,
+                                                           const double* __restrict__ maps, const uint8_t* __restrict__ anno,
+                                                           const int32_t* __restrict__ obj_off,
+                                                           const int32_t* __restrict__ objects, int H, int W,
+                                                           double seg_thr, uint8_t* __restrict__ labels) {
+  __shared__ double s_inv[PL_CHUNK][6];
+  __shared__ int s_kind[PL_CHUNK], s_arg[PL_CHUNK];
+  const int g = blockIdx.z;
+  const int tid = threadIdx.y * 32 + threadIdx.x;
+  const int bx0 = blockIdx.x * 32, by0 = blockIdx.y * 8;
+  const int x = bx0 + threadIdx.x, y = by0 + threadIdx.y;
+  const bool inside = x < W && y < H;
+  const int o0 = obj_off[g];
+  // labels are uint8: a video with more than 255 objects (a violated precondition) gets no objects, i.e. label 0,
+  // rather than wrapped labels
+  const int o1 = obj_off[g + 1] - o0 > 255 ? o0 : obj_off[g + 1];
+  double best = 0.0;
+  int best_k = -1;
+  bool nan = false;
+  const size_t pix = ((size_t)g * H + y) * W + x;
+  for (int c0 = o0; c0 < o1; c0 += PL_CHUNK) {
+    const int n = min(PL_CHUNK, o1 - c0);
+    __syncthreads();                                   // the previous chunk is no longer read
+    if (tid < n) {
+      int kind = objects[2 * (c0 + tid)], arg = objects[2 * (c0 + tid) + 1];
+      if (kind == SM_OBJ_TRACKED) {
+        double* inv = s_inv[tid];
+        warp_invert_map(maps + 6 * (size_t)arg, inv);
+        // block cull: the source positions of the block's pixels lie in the hull of its corners' (exact) positions;
+        // the fixed-point rounding moves a position by far less than the 2-pixel margin
+        const int xe = min(bx0 + 31, W - 1), ye = min(by0 + 7, H - 1);
+        double xmn = 1e300, xmx = -1e300, ymn = 1e300, ymx = -1e300;
+        for (int cy = 0; cy < 2; ++cy)
+          for (int cx = 0; cx < 2; ++cx) {
+            const double px = cx ? xe : bx0, py = cy ? ye : by0;
+            const double u = inv[0] * px + inv[1] * py + inv[2], v = inv[3] * px + inv[4] * py + inv[5];
+            xmn = fmin(xmn, u); xmx = fmax(xmx, u); ymn = fmin(ymn, v); ymx = fmax(ymx, v);
+          }
+        if (!(xmx >= -2.0 && xmn <= side + 1.0 && ymx >= -2.0 && ymn <= side + 1.0)) kind = SM_OBJ_IDLE;
+      }
+      s_kind[tid] = kind;
+      s_arg[tid] = arg;
+    }
+    __syncthreads();
+    if (!inside) continue;
+    for (int k = 0; k < n; ++k) {
+      const int kind = s_kind[k];
+      double v;
+      if (kind == SM_OBJ_TRACKED) {
+        const WarpTap t = warp_tap(s_inv[k], x, y);
+        if (!t.touches(side, side)) continue;
+        v = (double)warp_sample(masks + (size_t)s_arg[k] * side * side, side, side, t, -1.f);
+      } else if (kind == SM_OBJ_INIT) {
+        v = anno[pix] == s_arg[k] ? 1.0 : 0.0;
+      } else {
+        continue;
+      }
+      if (v != v) nan = true;
+      if (best_k < 0 || v > best) { best = v; best_k = c0 - o0 + k; }
+    }
+  }
+  if (inside) labels[pix] = (!nan && best_k >= 0 && best > seg_thr) ? (uint8_t)(best_k + 1) : (uint8_t)0;
+}
+
+// cv2.boundingRect(anno[g] == id) for one (g, id) query per block: min / max of the matching pixels' x and y.
+constexpr int LB_THREADS = 512;
+
+__global__ void __launch_bounds__(LB_THREADS) label_boxes_kernel(const uint8_t* __restrict__ anno, int G, int H, int W,
+                                                                 const int32_t* __restrict__ queries,
+                                                                 int32_t* __restrict__ boxes) {
+  __shared__ int red[4][LB_THREADS / 32];
+  const int q = blockIdx.x;
+  const int g = queries[2 * q], id = queries[2 * q + 1];
+  int xmn = INT_MAX, ymn = INT_MAX, xmx = -1, ymx = -1;
+  if (g >= 0 && g < G) {
+    const uint8_t* a = anno + (size_t)g * H * W;
+    for (int y = 0; y < H; ++y)
+      for (int x = threadIdx.x; x < W; x += LB_THREADS)
+        if (a[(size_t)y * W + x] == id) {
+          xmn = min(xmn, x); xmx = max(xmx, x);
+          ymn = min(ymn, y); ymx = max(ymx, y);
+        }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    xmn = min(xmn, __shfl_xor_sync(0xffffffffu, xmn, o));
+    ymn = min(ymn, __shfl_xor_sync(0xffffffffu, ymn, o));
+    xmx = max(xmx, __shfl_xor_sync(0xffffffffu, xmx, o));
+    ymx = max(ymx, __shfl_xor_sync(0xffffffffu, ymx, o));
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) { red[0][warp] = xmn; red[1][warp] = ymn; red[2][warp] = xmx; red[3][warp] = ymx; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < LB_THREADS / 32; ++w) {
+      xmn = min(xmn, red[0][w]); ymn = min(ymn, red[1][w]); xmx = max(xmx, red[2][w]); ymx = max(ymx, red[3][w]);
+    }
+    int32_t* o = boxes + 4 * q;
+    if (xmx < 0) { o[0] = 0; o[1] = 0; o[2] = 0; o[3] = 0; }           // no pixel: cv2 returns (0, 0, 0, 0)
+    else { o[0] = xmn; o[1] = ymn; o[2] = xmx - xmn + 1; o[3] = ymx - ymn + 1; }
+  }
+}
+
+// sm_template_slots: one slot's worth of cached kernel (n8 x 16 bytes per plane) per (block.y = stream)
+__global__ void scatter_slots_kernel(const __half* __restrict__ src_hi, const __half* __restrict__ src_lo,
+                                     __half* __restrict__ dst_hi, __half* __restrict__ dst_lo,
+                                     const int32_t* __restrict__ slots, int num_slots, int n8, int* __restrict__ status) {
+  const int b = blockIdx.y;
+  const int s = slots[b];
+  if (s < 0 || s >= num_slots) {
+    if (blockIdx.x == 0 && threadIdx.x == 0 && status != nullptr) atomicOr(status, kStatusBadSlot);
+    return;
+  }
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n8) return;
+  const size_t so = (size_t)b * n8 + i, d = (size_t)s * n8 + i;
+  reinterpret_cast<uint4*>(dst_hi)[d] = reinterpret_cast<const uint4*>(src_hi)[so];
+  if (dst_lo != nullptr) reinterpret_cast<uint4*>(dst_lo)[d] = reinterpret_cast<const uint4*>(src_lo)[so];
 }
 
 
@@ -1115,7 +1281,7 @@ void launch_maxpool3s2(const Act& in, Act out, cudaStream_t st) {
 }
 
 void launch_xcorr_nhwc(const Act& x, int c_off, const __half* k_hi, const __half* k_lo, int kh, int kw, Act out, float mul,
-                       int* ovf, cudaStream_t st) {
+                       int* ovf, cudaStream_t st, const int32_t* slots, int num_slots) {
   SMK_CHECK(kh == 5 && kw == 5, "engine xcorr is specialised for the 5x5 template kernel");
   SMK_CHECK(out.H == x.H - kh + 1 && out.W == x.W - kw + 1 && c_off % 8 == 0 && c_off + out.C <= x.C && out.C % 32 == 0,
             "xcorr shapes");
@@ -1129,7 +1295,16 @@ void launch_xcorr_nhwc(const Act& x, int c_off, const __half* k_hi, const __half
   auto kern = xcorr_nhwc_kernel<5, 5, 7, 5, 320>;
   static unsigned long long attr = 0;
   ensure_dynamic_smem(kern, 160 * 1024, attr);
-  kern<<<dim3(out.C / 32, x.B, bands), 320, smem, st>>>(x, k_hi, k_lo, out, band_rows, c_off, mul, ovf);
+  kern<<<dim3(out.C / 32, x.B, bands), 320, smem, st>>>(x, k_hi, k_lo, out, band_rows, c_off, mul, ovf, slots,
+                                                        num_slots);
+  SMK_CUDA(cudaGetLastError());
+}
+
+void launch_scatter_slots(const __half* src_hi, const __half* src_lo, __half* dst_hi, __half* dst_lo,
+                          const int32_t* slots, int B, int num_slots, int n, int* status, cudaStream_t st) {
+  SMK_CHECK(n % 8 == 0, "scatter_slots: slot size must be a multiple of 8 halves");
+  scatter_slots_kernel<<<dim3((n / 8 + 255) / 256, B), 256, 0, st>>>(src_hi, src_lo, dst_hi, dst_lo, slots, num_slots,
+                                                                      n / 8, status);
   SMK_CUDA(cudaGetLastError());
 }
 
@@ -1230,9 +1405,22 @@ void launch_tracker_update(int B, double* state, const float* rec, const double*
 }
 
 void launch_crop_resize(const uint8_t* frames, size_t frame_stride, int H, int W, const int32_t* box, int B, int model,
-                        float* out, cudaStream_t st) {
+                        float* out, cudaStream_t st, const int32_t* frame_idx) {
   dim3 block(32, 8), grid((model + 31) / 32, (model + 7) / 8, B);
-  crop_resize_kernel<<<grid, block, 0, st>>>(frames, frame_stride, H, W, box, model, out);
+  crop_resize_kernel<<<grid, block, 0, st>>>(frames, frame_stride, H, W, box, model, out, frame_idx);
+  SMK_CUDA(cudaGetLastError());
+}
+
+void launch_paste_labels(const float* masks, int side, const double* maps, const uint8_t* anno, const int32_t* obj_off,
+                         const int32_t* objects, int G, int H, int W, double seg_thr, uint8_t* labels, cudaStream_t st) {
+  dim3 block(32, 8), grid((W + 31) / 32, (H + 7) / 8, G);
+  paste_labels_kernel<<<grid, block, 0, st>>>(masks, side, maps, anno, obj_off, objects, H, W, seg_thr, labels);
+  SMK_CUDA(cudaGetLastError());
+}
+
+void launch_label_boxes(const uint8_t* anno, int G, int H, int W, const int32_t* queries, int Q, int32_t* boxes,
+                        cudaStream_t st) {
+  label_boxes_kernel<<<Q, LB_THREADS, 0, st>>>(anno, G, H, W, queries, boxes);
   SMK_CUDA(cudaGetLastError());
 }
 

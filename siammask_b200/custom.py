@@ -241,13 +241,49 @@ class Custom:
         if self.graphs:
             torch.cuda.current_stream(self._device).wait_stream(self._gstream)
 
+    def _check_slots(self, slots, B: int, distinct: bool) -> torch.Tensor:
+        """A slot table: int32 CUDA tensor [B] with entries in [0, num_slots) (distinct for template).  The check reads
+        the table back to the host, so it runs before anything is enqueued."""
+        if not (isinstance(slots, torch.Tensor) and slots.is_cuda and slots.dtype == torch.int32):
+            raise ValueError("slots must be an int32 CUDA tensor")
+        if slots.device != self._device:
+            raise ValueError(f"slots live on {slots.device}, the engine on {self._device}")
+        if slots.dim() != 1 or slots.numel() != B:
+            raise ValueError(f"slots must have shape [{B}], got {tuple(slots.shape)}")
+        host = slots.cpu().numpy()
+        if ((host < 0) | (host >= self.num_slots)).any():
+            raise ValueError(f"slot table entries must lie in [0, {self.num_slots})")
+        if distinct and np.unique(host).size != B:
+            raise ValueError("slot table entries must be distinct")
+        return slots.contiguous()
+
+    def _stage_slots(self, slots: torch.Tensor) -> torch.Tensor:
+        """Graph replay reads the table at a stable address: copy it there on the caller's stream.  Call before
+        `_fence_in`, so that the engine's stream is ordered after the copy."""
+        if self.graphs:
+            buf = self._buf(("slots", slots.numel()), (slots.numel(),), torch.int32)
+            buf.copy_(slots)
+            return buf
+        return slots
+
     @torch.no_grad()
-    def template(self, z, slot0: int = 0):
+    def template(self, z, slot0: int = 0, slots=None):
+        """slots (optional): int32 CUDA tensor [B] of distinct engine slots; stream b's template is cached in slots[b]
+        instead of slot0 + b."""
+        if slots is not None:
+            slots = self._check_slots(slots, z.shape[0], distinct=True)
         z = self._prep(z, 127)
         with torch.cuda.device(self._device):
+            if slots is not None:
+                slots = self._stage_slots(slots)
             self._fence_in()
-            _lib.check(self._lib.sm_template(self._engine, slot0, z.shape[0], z.data_ptr(), self._stream()))
+            if slots is None:
+                _lib.check(self._lib.sm_template(self._engine, slot0, z.shape[0], z.data_ptr(), self._stream()))
+            else:
+                _lib.check(self._lib.sm_template_slots(self._engine, z.shape[0], slots.data_ptr(), z.data_ptr(),
+                                                       self._stream()))
             self._fence_out()
+        self._keep_slots = slots
 
     def _track(self, x, slot0, flags):
         x = self._prep(x, self.search_size)
@@ -330,10 +366,19 @@ class Custom:
 
     @torch.no_grad()
     def step(self, x, anchors, window, target_sz_in_crop, penalty_k: float, window_influence: float, slot0: int = 0,
-             refine: bool = True, mask_head: bool = False, mask_col: bool = False):
+             refine: bool = True, mask_head: bool = False, mask_col: bool = False, slots=None):
         """One whole frame of siamese_track (tools/test.py:201-261) in ONE engine call (C ABI `sm_step`):
         track(_mask) -> on-device selection -> track_refine at the selected position.  Returns a dict with cls, loc,
-        mask (raw head or None), best, pos, records, refine (or None), mask_col (or None)."""
+        mask (raw head or None), best, pos, records, refine (or None), mask_col (or None).  slots (optional): int32
+        CUDA tensor [B]; stream b then uses the template cached in slots[b] (`sm_step_slots`) instead of slot0 + b."""
+        if slots is not None:
+            slots = self._check_slots(slots, x.shape[0], distinct=False)
+        return self._step(x, anchors, window, target_sz_in_crop, penalty_k, window_influence, slot0, refine, mask_head,
+                          mask_col, slots)
+
+    def _step(self, x, anchors, window, target_sz_in_crop, penalty_k, window_influence, slot0=0, refine=True,
+              mask_head=False, mask_col=False, slots=None):
+        """`step` without the host-side check of `slots` (callers that own a table they have validated)."""
         x = self._prep(x, self.search_size)
         dev = self._device
         B, A, R = x.shape[0], self.anchor_num, self.score_size
@@ -358,16 +403,22 @@ class Custom:
 
         def ptr(t):
             return t.data_ptr() if t is not None else None
+        outs = (ptr(out["cls"]), ptr(out["loc"]), ptr(out["mask"]), ptr(out["best"]), ptr(out["pos"]),
+                ptr(out["records"]), ptr(out["refine"]), ptr(out["mask_col"]), self._stream())
         with torch.cuda.device(dev):
+            if slots is not None:
+                slots = self._stage_slots(slots)
             self._fence_in()
-            _lib.check(self._lib.sm_step(self._engine, slot0, B, x.data_ptr(), tsz.data_ptr(), anchors.data_ptr(),
-                                         window.data_ptr(), float(penalty_k), float(window_influence), flags,
-                                         ptr(out["cls"]), ptr(out["loc"]), ptr(out["mask"]), ptr(out["best"]),
-                                         ptr(out["pos"]), ptr(out["records"]), ptr(out["refine"]), ptr(out["mask_col"]),
-                                         self._stream()))
+            if slots is None:
+                _lib.check(self._lib.sm_step(self._engine, slot0, B, x.data_ptr(), tsz.data_ptr(), anchors.data_ptr(),
+                                             window.data_ptr(), float(penalty_k), float(window_influence), flags, *outs))
+            else:
+                _lib.check(self._lib.sm_step_slots(self._engine, B, slots.data_ptr(), x.data_ptr(), tsz.data_ptr(),
+                                                   anchors.data_ptr(), window.data_ptr(), float(penalty_k),
+                                                   float(window_influence), flags, *outs))
             self._fence_out()
         self._last_B = B
-        self._keep = (anchors, window, tsz)       # alive until the next call (the work is asynchronous)
+        self._keep = (anchors, window, tsz, slots)       # alive until the next call (the work is asynchronous)
         return out
 
     # ------------------------------------------------------------------ introspection used by tests / bench

@@ -5,6 +5,7 @@ from __future__ import annotations
 
 import ctypes as C
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -109,3 +110,76 @@ def warp_affine(src: torch.Tensor, maps, dsize, border_value: float = -1.0) -> t
         _lib.check(lib.sm_warp_affine(s3.data_ptr(), sh, sw, m.data_ptr(), out.data_ptr(), dh, dw, float(border_value), B,
                                       _stream(dev)))
     return out[0] if squeeze else out
+
+
+OBJ_IDLE, OBJ_TRACKED, OBJ_INIT = 0, 1, 2          # SM_OBJ_* of include/siammask_b200.h
+
+
+def paste_labels(masks, maps, anno, obj_offsets, objects, size, seg_thr: float) -> torch.Tensor:
+    """Fused paste-back + multi-object label map of track_vos (tools/test.py:480-523, C ABI `sm_paste_labels`).
+    masks f32 CUDA [rows,side,side] (sigmoid masks) and maps f64 [rows,6] (forward paste-back maps) of the tracked
+    objects, or None when no object is tracked; anno uint8 CUDA [G,H,W] (or None when no object is initialised);
+    obj_offsets int32 [G+1]: the objects of video g are entries obj_offsets[g]..obj_offsets[g+1]-1 of objects int32
+    [n,2] = (kind, arg) with kind OBJ_TRACKED (arg = row), OBJ_INIT (arg = label id) or OBJ_IDLE; size = (H, W).
+    Returns labels uint8 [G,H,W] = (first argmax over the video's objects + 1) * (max > seg_thr) in float64.
+    The offsets are checked on the host (one D2H copy if they live on the device): non-decreasing, covering `objects`,
+    at most 255 objects per video (labels are uint8)."""
+    off = np.asarray(obj_offsets.cpu() if torch.is_tensor(obj_offsets) else obj_offsets, dtype=np.int64).reshape(-1)
+    n = int(np.prod(objects.shape[:-1])) if torch.is_tensor(objects) else len(np.asarray(objects).reshape(-1, 2))
+    if off.size < 2 or off[0] != 0 or off[-1] != n or (np.diff(off) < 0).any():
+        raise ValueError(f"obj_offsets must rise from 0 to the number of objects ({n})")
+    if (np.diff(off) > 255).any():
+        raise ValueError("at most 255 objects per video (labels are uint8)")
+    return _paste_labels(masks, maps, anno, obj_offsets, objects, size, seg_thr)
+
+
+def _paste_labels(masks, maps, anno, obj_offsets, objects, size, seg_thr: float) -> torch.Tensor:
+    """`paste_labels` without the host-side check of the offsets (callers that validated their tables once)."""
+    off = torch.as_tensor(obj_offsets, dtype=torch.int32).reshape(-1)
+    G = off.numel() - 1
+    H, W = int(size[0]), int(size[1])
+    ref = masks if masks is not None else anno
+    dev = ref.device if ref is not None else torch.device("cuda", torch.cuda.current_device())
+    if dev.type != "cuda":
+        raise RuntimeError("paste_labels expects CUDA tensors; there is no CPU path")
+    lib = _lib.load()
+    off = off.to(dev).contiguous()
+    obj = torch.as_tensor(objects, dtype=torch.int32).reshape(-1, 2)
+    obj = (obj if obj.numel() else torch.zeros(1, 2, dtype=torch.int32)).to(dev).contiguous()
+    side = 1
+    if masks is not None:
+        masks = masks.to(dev, torch.float32).contiguous()
+        side = int(masks.shape[-1])
+        maps = torch.as_tensor(maps, dtype=torch.float64).reshape(-1, 6).to(dev).contiguous()
+    if anno is not None:
+        anno = anno.to(dev).contiguous()
+        if anno.dtype != torch.uint8 or tuple(anno.shape) != (G, H, W):
+            raise ValueError(f"anno must be uint8 [{G},{H},{W}]")
+    out = torch.empty(G, H, W, dtype=torch.uint8, device=dev)
+
+    def ptr(t):
+        return t.data_ptr() if t is not None else None
+    with torch.cuda.device(dev):
+        _lib.check(lib.sm_paste_labels(ptr(masks), side, ptr(maps) if masks is not None else None, ptr(anno),
+                                       off.data_ptr(), obj.data_ptr(), G, H, W, float(seg_thr), out.data_ptr(),
+                                       _stream(dev)))
+    return out
+
+
+def label_boxes(anno: torch.Tensor, queries) -> torch.Tensor:
+    """cv2.boundingRect(anno[g] == id) for every query (g, id) on the device (init boxes of track_vos,
+    tools/test.py:483-496, C ABI `sm_label_boxes`).  anno uint8 CUDA [G,H,W]; queries int [Q,2].  Returns int32 [Q,4]
+    x, y, w, h ((0, 0, 0, 0) where no pixel carries the id)."""
+    if not anno.is_cuda or anno.dtype != torch.uint8 or anno.dim() != 3:
+        raise RuntimeError("label_boxes expects a uint8 CUDA tensor [G,H,W]; there is no CPU path")
+    lib = _lib.load()
+    dev = anno.device
+    anno = anno.contiguous()
+    q = torch.as_tensor(queries, dtype=torch.int32).reshape(-1, 2).to(dev).contiguous()
+    out = torch.zeros(q.shape[0], 4, dtype=torch.int32, device=dev)
+    if q.shape[0] == 0:
+        return out
+    G, H, W = anno.shape
+    with torch.cuda.device(dev):
+        _lib.check(lib.sm_label_boxes(anno.data_ptr(), G, H, W, q.data_ptr(), q.shape[0], out.data_ptr(), _stream(dev)))
+    return out

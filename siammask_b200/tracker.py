@@ -5,14 +5,21 @@ What the reference does per frame on the host in numpy, for ONE stream (tools/te
 arithmetic, crop + resize, score/box post-processing + argmax, learning-rate update and clamping of the target state,
 mask paste-back — runs here as a fixed sequence of kernels over all streams (C ABI in include/siammask_b200.h):
 
-    sm_tracker_prepare   state -> crop boxes, target size in the crop, scale          (tools/test.py:180-198, 71-76)
-    sm_crop_resize       uint8 frames -> f32 [N,3,S,S] search crops (cv2-exact)        (:67-110)
-    sm_step              track_mask -> select -> track_refine                          (:201-261)
-    sm_tracker_update    winner box + score -> new state (lr, clamps), paste-back map  (:239-249, 263-282, 305-315)
-    sm_warp_affine       127x127 sigmoid mask -> frame, threshold                      (:263-284)
+    sm_tracker_prepare      state -> crop boxes, target size in the crop, scale          (tools/test.py:180-198, 71-76)
+    sm_crop_resize_indexed  uint8 frames -> f32 [N,3,S,S] search crops (cv2-exact)        (:67-110)
+    sm_step_slots           track_mask -> select -> track_refine                          (:201-261)
+    sm_tracker_update       winner box + score -> new state (lr, clamps), paste-back map  (:239-249, 263-282, 305-315)
+    sm_warp_affine          127x127 sigmoid mask -> frame, threshold                      (:263-284)
 
 The state (target_pos, target_sz, float64) lives on the device; a frame costs one small D2H copy only if the caller
 asks for the numbers (`TrackResult.cpu()`).  Contour extraction / minAreaRect (:285-303) is not part of this module.
+
+Streams join and leave a running tracker: `add` templates new streams into free engine slots, `remove` frees them.  The
+active streams are kept as compact rows (state, slot, frame index), and every frame runs exactly those rows as one
+batch through the slot table (`sm_step_slots`) and the frame-index table (`sm_crop_resize_indexed`); both tables are
+uploaded only when the set changes.  Each stream reads one frame of the tensor passed to `track`: its frame index, set
+by `add` (for `init`, stream i reads frame i; a single [H,W,3] frame is shared by all streams).
+
 The arithmetic is pinned by `tests/test_batch_tracker.py` to the reference loop's golden trajectory and to
 single-stream runs of the host restatement in `oracle/ref_loop.py`.
 """
@@ -55,8 +62,10 @@ class TrackerParams:
 
 @dataclass
 class TrackResult:
-    """Per-frame outputs, all on the device.  state f64 [N,8] = x, y, w, h (new target_pos / target_sz), score,
-    penalty, lr, best index; mask: bool [N,H,W] frame-sized masks (or None)."""
+    """Per-frame outputs, all on the device, one row per active stream in the order of `BatchTracker.ids`.  state f64
+    [N,8] = x, y, w, h (new target_pos / target_sz), score, penalty, lr, best index; mask: bool [N,H,W] frame-sized masks
+    (or None).  With mask=True, extras also holds "mask_prob" f32 [N,side,side] (sigmoid masks) and "maps" f64 [N,6]
+    (their paste-back maps, overwritten by the next frame)."""
     state: torch.Tensor
     mask: torch.Tensor | None = None
     extras: dict = field(default_factory=dict)
@@ -68,8 +77,8 @@ class TrackResult:
 
 
 class BatchTracker:
-    """N tracker streams on one engine.  `net` is a `siammask_b200.Custom` on a CUDA device with
-    max_batch >= N and num_slots >= slot0 + N."""
+    """Tracker streams on one engine.  `net` is a `siammask_b200.Custom` on a CUDA device; at most max_batch streams are
+    active at once, in engine slots slot0 .. num_slots-1."""
 
     def __init__(self, net, params: TrackerParams | None = None, slot0: int = 0):
         self.net = net
@@ -83,96 +92,195 @@ class BatchTracker:
         self.anchors = torch.from_numpy(generate_anchor(net.anchors, R)).to(self.dev)
         self.window = torch.from_numpy(cosine_window(R, A, self.p.windowing).astype(np.float32)).to(self.dev)
         self.hp = self.p.c_struct()
+        self._next_id = 0
+        self._clear()
+
+    def _clear(self):
         self.N = 0
+        self._ids: list[int] = []
+        self._slots: list[int] = []
+        self._fidx: list[int] = []
+        self.im_w = self.im_h = None
+        dev = self.dev
+        self.state = torch.zeros(0, 4, dtype=torch.float64, device=dev)
+        self.avg = torch.zeros(0, 3, dtype=torch.int32, device=dev)
+        self.imsize = torch.zeros(0, 2, dtype=torch.int32, device=dev)
+
+    @property
+    def ids(self) -> list[int]:
+        """Ids of the active streams, in the row order of every per-frame output."""
+        return list(self._ids)
+
+    @property
+    def slots(self) -> list[int]:
+        return list(self._slots)
 
     # ------------------------------------------------------------------ helpers
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
 
     def _frames(self, frames) -> torch.Tensor:
-        """uint8 [N,H,W,3] on the device (a single [H,W,3] frame is shared by all streams)."""
+        """uint8 [F,H,W,3] on the device (a single [H,W,3] frame is shared by all streams)."""
         if isinstance(frames, (list, tuple)):
             frames = np.stack([np.asarray(f) for f in frames], 0)
         t = torch.as_tensor(frames)
         if t.dtype != torch.uint8:
             raise ValueError("frames must be uint8 HWC (BGR as cv2.imread returns them)")
+        if t.dim() not in (3, 4) or t.shape[-1] != 3:
+            raise ValueError(f"frames must be [H,W,3] or [F,H,W,3], got {tuple(t.shape)}")
         return t.to(self.dev).contiguous()
 
-    def _crop(self, frames: torch.Tensor, boxes: torch.Tensor, size: int) -> torch.Tensor:
+    @staticmethod
+    def _hw(fr: torch.Tensor):
+        return (int(fr.shape[0]), int(fr.shape[1])) if fr.dim() == 3 else (int(fr.shape[1]), int(fr.shape[2]))
+
+    def _crop(self, frames: torch.Tensor, frame_idx: torch.Tensor, boxes: torch.Tensor, size: int) -> torch.Tensor:
         N = boxes.shape[0]
-        if frames.dim() == 3:
-            H, W, stride = frames.shape[0], frames.shape[1], 0
-        else:
-            if frames.shape[0] != N:
-                raise ValueError("one frame per stream expected")
-            H, W, stride = frames.shape[1], frames.shape[2], frames.shape[1] * frames.shape[2] * 3
+        H, W = self._hw(frames)
+        stride = 0 if frames.dim() == 3 else H * W * 3
         out = torch.empty(N, 3, size, size, device=self.dev, dtype=torch.float32)
-        _lib.check(self.lib.sm_crop_resize(frames.data_ptr(), stride, H, W, boxes.data_ptr(), N, size, out.data_ptr(),
-                                           self._stream()))
+        _lib.check(self.lib.sm_crop_resize_indexed(frames.data_ptr(), stride, H, W, frame_idx.data_ptr(),
+                                                   boxes.data_ptr(), N, size, out.data_ptr(), self._stream()))
         return out
 
-    # ------------------------------------------------------------------ siamese_init (tools/test.py:132-169)
+    def _upload_tables(self):
+        """Device copies of the active set (slot table, frame-index table) and per-frame work buffers; runs only when the
+        set changes."""
+        N, dev = self.N, self.dev
+        self._slots_dev = torch.tensor(self._slots, dtype=torch.int32, device=dev)
+        self._fidx_dev = torch.tensor(self._fidx, dtype=torch.int32, device=dev)
+        self._max_fidx = max(self._fidx) if self._fidx else -1
+        self.boxes = torch.zeros(N, 8, dtype=torch.int32, device=dev)
+        self.tsz = torch.zeros(N, 2, dtype=torch.float64, device=dev)
+        self.aux = torch.zeros(N, 4, dtype=torch.float64, device=dev)
+        self.maps = torch.zeros(N, 6, dtype=torch.float64, device=dev)
+
+    # ------------------------------------------------------------------ stream lifecycle
     @torch.no_grad()
-    def init(self, frames, boxes_xywh):
-        """frames: uint8 [N,H,W,3] (or one shared [H,W,3]); boxes_xywh: [N,4] top-left x, y, w, h of the targets."""
+    def add(self, frames, boxes_xywh, frame_index=None) -> list[int]:
+        """siamese_init (tools/test.py:132-169) for new streams, which join the running batch in free engine slots.
+        frames: uint8 [F,H,W,3] (or one shared [H,W,3]); boxes_xywh: [n,4] top-left x, y, w, h of the targets;
+        frame_index: [n] frame of `frames` each new stream reads, now and in every later `track` (default: stream i reads
+        frame i).  Returns the new streams' ids."""
         with torch.cuda.device(self.dev):
             fr = self._frames(frames)
             bx = torch.as_tensor(np.asarray(boxes_xywh, dtype=np.float64)).reshape(-1, 4).to(self.dev)
-            N = bx.shape[0]
-            if N > self.net.max_batch or self.slot0 + N > self.net.num_slots:
+            n = bx.shape[0]
+            H, W = self._hw(fr)
+            if self.N and (H, W) != (self.im_h, self.im_w):
+                raise ValueError(f"all streams of a tracker share one frame size ({self.im_h}x{self.im_w})")
+            idx = list(range(n)) if frame_index is None else [int(i) for i in np.asarray(frame_index).reshape(-1)]
+            if len(idx) != n:
+                raise ValueError("one frame index per new stream expected")
+            F = 1 if fr.dim() == 3 else int(fr.shape[0])
+            if fr.dim() == 4 and any(i < 0 or i >= F for i in idx):
+                raise ValueError(f"frame index out of range [0, {F})")
+            if any(i < 0 for i in idx):
+                raise ValueError("frame indices must be >= 0")
+            used = set(self._slots)
+            free = [s for s in range(self.slot0, self.net.num_slots) if s not in used][:n]
+            if n == 0:
+                return []
+            if self.N + n > self.net.max_batch or len(free) < n:
                 raise ValueError("more streams than the engine was built for")
-            self.N = N
-            H, W = (fr.shape[0], fr.shape[1]) if fr.dim() == 3 else (fr.shape[1], fr.shape[2])
-            self.im_w, self.im_h = int(W), int(H)
-            self.imsize = torch.tensor([[W, H]] * N, dtype=torch.int32, device=self.dev)
+            src = idx if fr.dim() == 4 else [0] * n          # frame each new stream reads in this call
+            src_dev = torch.tensor(src, dtype=torch.int32, device=self.dev)
             # target_pos = box centre, target_sz = (w, h)  (tools/test.py:338-339 / demo.py)
-            self.state = torch.stack([bx[:, 0] + bx[:, 2] / 2, bx[:, 1] + bx[:, 3] / 2, bx[:, 2], bx[:, 3]], 1).contiguous()
+            state = torch.stack([bx[:, 0] + bx[:, 2] / 2, bx[:, 1] + bx[:, 3] / 2, bx[:, 2], bx[:, 3]], 1).contiguous()
             # avg_chans = np.mean(im, axis=(0, 1)); written into a uint8 image it truncates (:146, :89-100).
             # Sums of < 2^53 integers are exact in float64, so sum / n equals numpy's mean bit for bit.
-            f4 = fr if fr.dim() == 4 else fr.unsqueeze(0).expand(N, -1, -1, -1)
-            mean = f4.to(torch.float64).sum(dim=(1, 2)) / float(H * W)
-            self.avg = mean.to(torch.uint8).to(torch.int32).contiguous()
+            f4 = fr if fr.dim() == 4 else fr.unsqueeze(0)
+            uniq = sorted(set(src))
+            mean = f4[uniq].to(torch.float64).sum(dim=(1, 2)) / float(H * W)
+            where = torch.tensor([uniq.index(i) for i in src], device=self.dev)
+            avg = mean[where].to(torch.uint8).to(torch.int32).contiguous()
             # template window (:149-155): s_z = round(sqrt(wc_z * hc_z)), crop around target_pos, resize to 127
-            sw, sh = self.state[:, 2], self.state[:, 3]
+            sw, sh = state[:, 2], state[:, 3]
             wc_z = sw + self.p.context_amount * (sw + sh)
             hc_z = sh + self.p.context_amount * (sw + sh)
             s_z = torch.round(torch.sqrt(wc_z * hc_z))                  # half-to-even, like Python's round()
             c = (s_z + 1) / 2
-            zb = torch.zeros(N, 8, dtype=torch.int32, device=self.dev)
-            zb[:, 0] = torch.round(self.state[:, 0] - c).to(torch.int32)
-            zb[:, 1] = torch.round(self.state[:, 1] - c).to(torch.int32)
+            zb = torch.zeros(n, 8, dtype=torch.int32, device=self.dev)
+            zb[:, 0] = torch.round(state[:, 0] - c).to(torch.int32)
+            zb[:, 1] = torch.round(state[:, 1] - c).to(torch.int32)
             zb[:, 2] = s_z.to(torch.int32)
-            zb[:, 3:6] = self.avg
-            z = self._crop(fr, zb, self.p.exemplar_size)
-            self.net.template(z, slot0=self.slot0)
-            self.boxes = torch.zeros(N, 8, dtype=torch.int32, device=self.dev)
-            self.tsz = torch.zeros(N, 2, dtype=torch.float64, device=self.dev)
-            self.aux = torch.zeros(N, 4, dtype=torch.float64, device=self.dev)
-            self.maps = torch.zeros(N, 6, dtype=torch.float64, device=self.dev)
+            zb[:, 3:6] = avg
+            z = self._crop(fr, src_dev, zb, self.p.exemplar_size)
+            self.net.template(z, slots=torch.tensor(free, dtype=torch.int32, device=self.dev))
+            ids = list(range(self._next_id, self._next_id + n))
+            self._next_id += n
+            self.im_w, self.im_h = W, H
+            self.state = torch.cat([self.state, state], 0).contiguous()
+            self.avg = torch.cat([self.avg, avg], 0).contiguous()
+            self.imsize = torch.tensor([[W, H]] * (self.N + n), dtype=torch.int32, device=self.dev)
+            self._ids += ids
+            self._slots += free
+            self._fidx += idx
+            self.N += n
+            self._upload_tables()
+        return ids
+
+    @torch.no_grad()
+    def remove(self, ids) -> None:
+        """Stop tracking the given streams and free their engine slots (a later `add` may reuse them)."""
+        drop = {int(i) for i in np.asarray(ids).reshape(-1)}
+        unknown = drop - set(self._ids)
+        if unknown:
+            raise ValueError(f"unknown stream ids {sorted(unknown)}")
+        if not drop:
+            return
+        keep = [r for r, i in enumerate(self._ids) if i not in drop]
+        with torch.cuda.device(self.dev):
+            rows = torch.tensor(keep, dtype=torch.long, device=self.dev)
+            self.state = self.state.index_select(0, rows).contiguous()
+            self.avg = self.avg.index_select(0, rows).contiguous()
+            self.imsize = self.imsize.index_select(0, rows).contiguous()
+            self._ids = [self._ids[r] for r in keep]
+            self._slots = [self._slots[r] for r in keep]
+            self._fidx = [self._fidx[r] for r in keep]
+            self.N = len(keep)
+            self._upload_tables()
+
+    # ------------------------------------------------------------------ siamese_init (tools/test.py:132-169)
+    @torch.no_grad()
+    def init(self, frames, boxes_xywh):
+        """Start over with N streams in slots slot0 .. slot0+N-1.  frames: uint8 [N,H,W,3] (or one shared [H,W,3]);
+        boxes_xywh: [N,4] top-left x, y, w, h of the targets.  Stream i reads frame i of later per-stream frame tensors."""
+        n = np.asarray(boxes_xywh).reshape(-1, 4).shape[0]
+        if n > self.net.max_batch or self.slot0 + n > self.net.num_slots:
+            raise ValueError("more streams than the engine was built for")
+        self._clear()
+        self.add(frames, boxes_xywh, frame_index=range(n))
         return self
 
     # ------------------------------------------------------------------ siamese_track (tools/test.py:172-315)
     @torch.no_grad()
-    def track(self, frames, mask: bool = True, refine: bool = True) -> TrackResult:
-        """Advance all N streams by one frame.  mask=True pastes the (refined) mask back into the frame and thresholds it
-        at seg_thr; refine=False uses the 63x63 mask head column instead of the refine module (tools/test.py:256-260)."""
+    def track(self, frames, mask: bool = True, refine: bool = True, paste: bool = True) -> TrackResult:
+        """Advance all active streams by one frame.  mask=True computes the (refined) mask; with paste=True it is pasted
+        back into the frame and thresholded at seg_thr.  refine=False uses the 63x63 mask head column instead of the
+        refine module (tools/test.py:256-260)."""
         if self.N == 0:
-            raise RuntimeError("call init() first")
+            raise RuntimeError("no active streams: call init() or add() first")
         p, N = self.p, self.N
         with torch.cuda.device(self.dev):
             fr = self._frames(frames)
+            if self._hw(fr) != (self.im_h, self.im_w):
+                raise ValueError(f"frames must be {self.im_h}x{self.im_w}")
+            if fr.dim() == 4 and self._max_fidx >= fr.shape[0]:
+                raise ValueError(f"a stream reads frame {self._max_fidx}, but only {fr.shape[0]} frames were given")
             st = self._stream()
             _lib.check(self.lib.sm_tracker_prepare(N, self.state.data_ptr(), self.avg.data_ptr(), C.byref(self.hp),
                                                    self.boxes.data_ptr(), self.tsz.data_ptr(), self.aux.data_ptr(), st))
-            x = self._crop(fr, self.boxes, p.instance_size)
+            x = self._crop(fr, self._fidx_dev, self.boxes, p.instance_size)
             use_refine = mask and refine
             use_head = mask and not refine
-            out = self.net.step(x, self.anchors, self.window, self.tsz, p.penalty_k, p.window_influence, slot0=self.slot0,
-                                refine=use_refine, mask_head=use_head, mask_col=use_head)
+            out = self.net._step(x, self.anchors, self.window, self.tsz, p.penalty_k, p.window_influence,
+                                 refine=use_refine, mask_head=use_head, mask_col=use_head, slots=self._slots_dev)
             res = torch.empty(N, 8, dtype=torch.float64, device=self.dev)
             _lib.check(self.lib.sm_tracker_update(N, self.state.data_ptr(), out["records"].data_ptr(), self.aux.data_ptr(),
                                                   self.imsize.data_ptr(), C.byref(self.hp), self.net.anchor_num,
                                                   p.score_size, self.maps.data_ptr() if mask else None, res.data_ptr(), st))
+            extras = {"records": out["records"], "pos": out["pos"], "x_crop": x, "ids": list(self._ids)}
             mask_out = None
             if mask:
                 logits = out["refine"] if use_refine else out["mask_col"]
@@ -180,9 +288,11 @@ class BatchTracker:
                 if side != p.out_size:
                     raise ValueError(f"out_size {p.out_size} does not match the mask source ({side})")
                 m = logits.sigmoid().view(N, side, side).contiguous()
-                W, H = self.im_w, self.im_h
-                pasted = torch.empty(N, H, W, device=self.dev, dtype=torch.float32)
-                _lib.check(self.lib.sm_warp_affine(m.data_ptr(), side, side, self.maps.data_ptr(), pasted.data_ptr(), H, W,
-                                                   C.c_float(-1.0), N, st))
-                mask_out = pasted > p.seg_thr
-            return TrackResult(state=res, mask=mask_out, extras={"records": out["records"], "pos": out["pos"], "x_crop": x})
+                extras["mask_prob"], extras["maps"] = m, self.maps
+                if paste:
+                    W, H = self.im_w, self.im_h
+                    pasted = torch.empty(N, H, W, device=self.dev, dtype=torch.float32)
+                    _lib.check(self.lib.sm_warp_affine(m.data_ptr(), side, side, self.maps.data_ptr(), pasted.data_ptr(),
+                                                       H, W, C.c_float(-1.0), N, st))
+                    mask_out = pasted > p.seg_thr
+            return TrackResult(state=res, mask=mask_out, extras=extras)
