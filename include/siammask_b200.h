@@ -138,6 +138,20 @@ int sm_paste_labels(const float* masks, int32_t side, const double* maps, const 
                     const int32_t* objects, int32_t G, int32_t H, int32_t W, double seg_thr, uint8_t* labels,
                     void* stream);
 
+/* Fused paste-back + IoU counts of IouMeter.add (utils/average_meter_helper.py:71-113), the per-frame score of
+ * tools/tune_vos.py, for B streams of one frame size H x W.  Stream b's value v at a pixel is
+ * cv2.warpAffine(masks[b], maps[b], (W, H), INTER_LINEAR, BORDER_CONSTANT, -1), bit for bit with sm_warp_affine
+ * (masks f32 [B][side][side] sigmoid masks, maps f64 [B][6] forward maps of sm_tracker_update*), and the annotation is
+ * anno[video[b]] (anno uint8 [G][H][W], video int32 [B] in [0, G), not checked here).  For each of the T <= 32
+ * thresholds thrs (f64 [T]), counts int32 [B][T][2] = (intersection, union) of pred = v > thrs[t] and target = anno > 0.
+ * The comparison is made in double, (double)v > thr, as NumPy 2 evaluates float32_array > np.float64; NumPy 1.x
+ * compared in float32, which differs only where v == (float)thr and (float)thr rounded up.
+ * Precondition: thrs[t] >= -1.  It makes pixels whose four taps all miss the mask exact without visiting them (their
+ * value is -1); a threshold below -1 yields counts (-1, -1) instead.  Frame-sized per-stream masks are never
+ * materialised; all pointers are device pointers. */
+int sm_mask_iou(const float* masks, int32_t side, const double* maps, const uint8_t* anno, const int32_t* video,
+                int32_t B, int32_t H, int32_t W, const double* thrs, int32_t T, int32_t* counts, void* stream);
+
 /* Init boxes of track_vos (tools/test.py:483-496): for each query q = (video g, label id) of queries (device int32
  * [Q][2]), boxes[q] (device int32 [Q][4]) = x, y, w, h = cv2.boundingRect(anno[g] == id); (0, 0, 0, 0) when no pixel
  * carries the id. */
@@ -174,6 +188,12 @@ int sm_tracker_prepare(int32_t B, const double* state, const int32_t* avg_chans,
 int sm_tracker_update(int32_t B, double* state, const float* records, const double* aux, const int32_t* im_wh,
                       const sm_tracker_hp* hp, int32_t anchor_num, int32_t score_size, double* maps, double* out,
                       void* stream);
+/* sm_tracker_update with per-stream hyper-parameters: hp_table (device f64 [B][3] = penalty_k, window_influence, lr)
+ * supplies stream b's penalty_k and lr; context_amount, sizes and strides stay those of *hp.  With every row equal to
+ * the struct's values it computes what sm_tracker_update computes, bit for bit. */
+int sm_tracker_update_hp(int32_t B, double* state, const float* records, const double* aux, const int32_t* im_wh,
+                         const sm_tracker_hp* hp, const double* hp_table, int32_t anchor_num, int32_t score_size,
+                         double* maps, double* out, void* stream);
 
 /* One whole frame of siamese_track (tools/test.py:201-261) on the device, all pointers device pointers:
  * sm_track(flags) -> sm_select -> sm_refine at the position sm_select chose (refine_out != NULL needs
@@ -192,6 +212,15 @@ int sm_step_slots(sm_engine* e, int32_t B, const int32_t* slots, const float* x_
                   const float* anchors, const float* window, double penalty_k, double window_influence, int32_t flags,
                   float* cls, float* loc, float* mask, int32_t* best_idx, int32_t* pos, float* records, float* refine_out,
                   float* mask_col, void* stream);
+
+/* sm_step_slots with per-stream hyper-parameters instead of the two scalars: hp is a device f64 [B][3] table of
+ * (penalty_k, window_influence, lr) rows (lr is read by sm_tracker_update_hp, not here), so that one batch can run
+ * different tracker settings, e.g. a grid search over them.  Stream b's selection, including records[b][5] (its
+ * penalty), uses row b.  Like the slot table, the hp table's contents are read at run time under graph replay. */
+int sm_step_slots_hp(sm_engine* e, int32_t B, const int32_t* slots, const double* hp, const float* x_nchw,
+                     const double* target_sz_in_crop, const float* anchors, const float* window, int32_t flags,
+                     float* cls, float* loc, float* mask, int32_t* best_idx, int32_t* pos, float* records,
+                     float* refine_out, float* mask_col, void* stream);
 
 /* The same frame through HOST buffers: H2D of x and target_sz_in_crop, sm_step on staging buffers, D2H of the
  * records (always) and of whichever of refine / mask_col / cls / loc are non-NULL.  anchors / window stay device

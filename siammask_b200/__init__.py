@@ -4,11 +4,15 @@ Public surface mirrors the reference's model object for that path:
     Custom.template / track / track_mask / track_refine   (experiments/siammask_sharp/custom.py:173-190)
     conv2d_dw_group                                       (models/rpn.py:32-38)
     VideoSegmenter (multi-object track_vos on the device)  (tools/test.py:459-542)
+    ParamSweep (tune_vos's hyper-parameter grid search)    (tools/tune_vos.py)
 All compute lives in libsiammask_b200.so (C ABI: include/siammask_b200.h)."""
 from .custom import Custom, DEFAULT_ANCHORS
-from .ops import conv2d_dw_group, xcorr_depthwise, conv2d, crop_resize, warp_affine, paste_labels, label_boxes
+from .ops import conv2d_dw_group, xcorr_depthwise, conv2d, crop_resize, warp_affine, paste_labels, label_boxes, \
+    mask_iou
 from .checkpoint import synthetic_state_dict, load_checkpoint, expected_keys
 from .vos import VideoSegmenter
+from .tune import ParamSweep
 
 __all__ = ["Custom", "DEFAULT_ANCHORS", "conv2d_dw_group", "xcorr_depthwise", "conv2d", "crop_resize", "warp_affine",
-           "paste_labels", "label_boxes", "VideoSegmenter", "synthetic_state_dict", "load_checkpoint", "expected_keys"]
+           "paste_labels", "label_boxes", "mask_iou", "VideoSegmenter", "ParamSweep", "synthetic_state_dict",
+           "load_checkpoint", "expected_keys"]

@@ -70,6 +70,12 @@ SIGNATURES = {
     "sm_template_slots": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sm_step_slots": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 5 + [C.c_double, C.c_double, C.c_int32] +
                       [C.c_void_p] * 9),
+    "sm_step_slots_hp": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 6 + [C.c_int32] + [C.c_void_p] * 9),
+    "sm_tracker_update_hp": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.POINTER(SmTrackerHp), C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]),
+    "sm_mask_iou": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 3 + [C.c_int32] * 3 +
+                    [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "sm_crop_resize_indexed": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                          C.c_int32, C.c_void_p, C.c_void_p]),
     "sm_paste_labels": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 4 + [C.c_int32] * 3 +

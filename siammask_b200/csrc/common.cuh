@@ -175,14 +175,20 @@ void launch_warp_affine(const float* src, int sh, int sw, const double* maps, fl
                         int B, cudaStream_t st);
 void launch_tracker_prepare(int B, const double* state, const int32_t* avg, const TrackerHp& hp, int32_t* boxes,
                             double* tsz, double* aux, cudaStream_t st);
+// hp_table (optional): device f64 [B][3] = (penalty_k, window_influence, lr) per stream, replacing hp.penalty_k / hp.lr
 void launch_tracker_update(int B, double* state, const float* rec, const double* aux, const int32_t* imsize,
-                           const TrackerHp& hp, int A, int R, double* maps, double* out, cudaStream_t st);
+                           const TrackerHp& hp, int A, int R, double* maps, double* out, cudaStream_t st,
+                           const double* hp_table = nullptr);
 // frame_idx == nullptr: stream b crops frames + b * frame_stride; else frames + frame_idx[b] * frame_stride
 void launch_crop_resize(const uint8_t* frames, size_t frame_stride, int H, int W, const int32_t* box, int B, int model,
                         float* out, cudaStream_t st, const int32_t* frame_idx = nullptr);
+// hp (optional): device f64 [B][3] per-stream table; stream b then uses hp[b][0] / hp[b][1] instead of the scalars
 void launch_select(const float* cls, const float* loc, const float* anchors, const float* window, const double* tsz,
                    int B, int A, int R, double penalty_k, double window_influence, int32_t* best_idx, int32_t* pos,
-                   float* rec, cudaStream_t st);
+                   float* rec, cudaStream_t st, const double* hp = nullptr);
+// sm_mask_iou (include/siammask_b200.h): fused paste-back + IouMeter counts; counts must hold B*T*2 int32
+void launch_mask_iou(const float* masks, int side, const double* maps, const uint8_t* anno, const int32_t* video, int B,
+                     int H, int W, const double* thrs, int T, int32_t* counts, cudaStream_t st);
 // small-channel fp32 NHWC 3x3 pad-1 conv: in = up(a (+ b)); ymap/xmap: device nearest-upsample source indices
 void launch_small_conv3x3_maps(const float* a, const float* b, int B, int Hi, int Wi, int Ho, int Wo, int Cin, int Cout,
                                const int* ymap, const int* xmap, const float* w, const float* bias, int relu,

@@ -128,6 +128,7 @@ class Engine {
     const float* anchors = nullptr;      // device [A*R*R][4]
     const float* window = nullptr;       // device [A*R*R]
     double penalty_k = 0, window_influence = 0;
+    const double* hp = nullptr;          // device [B][3] per-stream (penalty_k, window_influence, lr) or null: scalars
     int flags = 0;
     float* cls = nullptr; float* loc = nullptr; float* mask = nullptr;   // device outputs (mask: raw 3969-ch head)
     int32_t* best = nullptr; int32_t* pos = nullptr; float* rec = nullptr;
@@ -1525,6 +1526,7 @@ Engine::StepIO slice_io(const Engine::StepIO& io, int b0, size_t S, size_t A, si
   Engine::StepIO o = io;
   o.x = io.x + (size_t)b0 * 3 * S * S;
   o.tsz = io.tsz + 2 * (size_t)b0;
+  if (io.hp) o.hp = io.hp + 3 * (size_t)b0;
   o.cls = io.cls + (size_t)b0 * 2 * A * RR;
   o.loc = io.loc + (size_t)b0 * 4 * A * RR;
   if (io.mask) o.mask = io.mask + (size_t)b0 * 3969 * RR;
@@ -1541,7 +1543,7 @@ void Engine::step_lane(Lane& ln, int slot0, int B, const StepIO& io, cudaStream_
   track_lane(ln, slot0, B, io.x, io.cls, io.loc, io.mask, io.flags, st, slots);
   launch(st, 1, "select", "select", 0, 4.0 * B * 6.0 * cfg_.anchor_num * R_ * R_, [&] {
     launch_select(io.cls, io.loc, io.anchors, io.window, io.tsz, B, cfg_.anchor_num, R_, io.penalty_k,
-                  io.window_influence, io.best, io.pos, io.rec, st);
+                  io.window_influence, io.best, io.pos, io.rec, st, io.hp);
   });
   if (io.refine != nullptr) refine_lane(ln, B, io.pos, io.refine, st);
   if (io.mask_col != nullptr)
@@ -1559,10 +1561,16 @@ void Engine::do_step(int slot0, int B, const StepIO& io, cudaStream_t st, const 
   SMK_CHECK(!want_head || io.mask != nullptr, "mask output buffer required");
   SMK_CHECK(io.mask_col == nullptr || want_head, "mask column needs SM_TRACK_MASK_HEAD");
   join_lanes(st);
+  // the scalars are kernel arguments baked into a captured graph, so their bit patterns are part of the key; a table
+  // (slots, hp) is read at run time and only its address is
+  uint64_t pk_bits, wi_bits;
+  std::memcpy(&pk_bits, &io.penalty_k, sizeof(pk_bits));
+  std::memcpy(&wi_bits, &io.window_influence, sizeof(wi_bits));
   const std::vector<uint64_t> key = {3, (uint64_t)slot0, (uint64_t)B, (uint64_t)io.x, (uint64_t)io.tsz, (uint64_t)io.cls,
                                      (uint64_t)io.loc, (uint64_t)io.mask, (uint64_t)io.flags, (uint64_t)io.pos,
                                      (uint64_t)io.rec, (uint64_t)io.refine, (uint64_t)io.mask_col, (uint64_t)st,
-                                     (uint64_t)io.anchors, (uint64_t)io.window, (uint64_t)slots};
+                                     (uint64_t)io.anchors, (uint64_t)io.window, (uint64_t)slots, pk_bits, wi_bits,
+                                     (uint64_t)io.hp};
   const size_t S = cfg_.search_size, A = cfg_.anchor_num, RR = (size_t)R_ * R_;
   run_with_graph(key, st, [&] {
     split_batch(B);
@@ -1909,6 +1917,20 @@ int sm_step_slots(sm_engine* e, int32_t B, const int32_t* slots, const float* x,
   SM_API_END
 }
 
+int sm_step_slots_hp(sm_engine* e, int32_t B, const int32_t* slots, const double* hp, const float* x,
+                     const double* target_sz_in_crop, const float* anchors, const float* window, int32_t flags, float* cls,
+                     float* loc, float* mask, int32_t* best_idx, int32_t* pos, float* records, float* refine_out,
+                     float* mask_col, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(e && slots && hp, "null argument");
+  smk::Engine::StepIO io;
+  io.x = x; io.tsz = target_sz_in_crop; io.anchors = anchors; io.window = window; io.hp = hp; io.flags = flags;
+  io.cls = cls; io.loc = loc; io.mask = mask; io.best = best_idx; io.pos = pos; io.rec = records;
+  io.refine = refine_out; io.mask_col = mask_col;
+  e->impl->do_step(0, B, io, static_cast<cudaStream_t>(stream), slots);
+  SM_API_END
+}
+
 int sm_step_host_async(sm_engine* e, int32_t slot0, int32_t B, const sm_step_io* io, void* stream, int32_t* ticket) {
   SM_API_BEGIN
   SMK_CHECK(e && io && ticket, "null argument");
@@ -1967,6 +1989,17 @@ int sm_paste_labels(const float* masks, int32_t side, const double* maps, const 
   SM_API_END
 }
 
+int sm_mask_iou(const float* masks, int32_t side, const double* maps, const uint8_t* anno, const int32_t* video,
+                int32_t B, int32_t H, int32_t W, const double* thrs, int32_t T, int32_t* counts, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(masks && maps && anno && video && thrs && counts && B >= 1 && H > 0 && W > 0 && side > 0, "bad argument");
+  SMK_CHECK((int64_t)H * W <= INT32_MAX, "frame too large for int32 counts");
+  SMK_CHECK(T >= 1 && T <= 32, "1 <= T <= 32 thresholds");
+  require_device();
+  smk::launch_mask_iou(masks, side, maps, anno, video, B, H, W, thrs, T, counts, static_cast<cudaStream_t>(stream));
+  SM_API_END
+}
+
 int sm_label_boxes(const uint8_t* anno, int32_t G, int32_t H, int32_t W, const int32_t* queries, int32_t Q, int32_t* boxes,
                    void* stream) {
   SM_API_BEGIN
@@ -2010,6 +2043,17 @@ int sm_tracker_update(int32_t B, double* state, const float* records, const doub
   require_device();
   smk::launch_tracker_update(B, state, records, aux, im_wh, to_hp(hp), anchor_num, score_size, maps, out,
                              static_cast<cudaStream_t>(stream));
+  SM_API_END
+}
+
+int sm_tracker_update_hp(int32_t B, double* state, const float* records, const double* aux, const int32_t* im_wh,
+                         const sm_tracker_hp* hp, const double* hp_table, int32_t anchor_num, int32_t score_size,
+                         double* maps, double* out, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(state && records && aux && im_wh && hp && hp_table && B >= 1 && score_size >= 1, "bad argument");
+  require_device();
+  smk::launch_tracker_update(B, state, records, aux, im_wh, to_hp(hp), anchor_num, score_size, maps, out,
+                             static_cast<cudaStream_t>(stream), hp_table);
   SM_API_END
 }
 

@@ -5,6 +5,7 @@
 #include "../../include/siammask_b200.h"
 #include "common.cuh"
 
+#include <algorithm>
 #include <climits>
 #include <cmath>
 #include <type_traits>
@@ -722,8 +723,11 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(const float* __rest
                                                      const float* __restrict__ window,
                                                      const double* __restrict__ tsz, int A, int R, double penalty_k,
                                                      double window_influence, int32_t* __restrict__ best_idx,
-                                                     int32_t* __restrict__ pos, float* __restrict__ rec) {
+                                                     int32_t* __restrict__ pos, float* __restrict__ rec,
+                                                     const double* __restrict__ hp) {
   const int b = blockIdx.x;
+  // hp: per-stream table [B][3] = (penalty_k, window_influence, lr) that replaces the scalars.  Its entries are read
+  // where they are used rather than once into registers: kept live across the exp calls they cost a spill.
   const int RR = R * R, n = A * RR;
   const float* c = cls + (size_t)b * 2 * A * RR;
   const float* l = loc + (size_t)b * 4 * A * RR;
@@ -755,8 +759,9 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(const float* __rest
     sc = fmax(sc, 1.0 / sc);
     double rc = tratio / (double)(w / h);
     rc = fmax(rc, 1.0 / rc);
-    const double penalty = exp(-(rc * sc - 1.0) * penalty_k);
-    const double ps = penalty * (double)score * (1.0 - window_influence) + (double)window[idx] * window_influence;
+    const double pk = hp != nullptr ? hp[3 * b] : penalty_k, wi = hp != nullptr ? hp[3 * b + 1] : window_influence;
+    const double penalty = exp(-(rc * sc - 1.0) * pk);
+    const double ps = penalty * (double)score * (1.0 - wi) + (double)window[idx] * wi;
     const int isn = ps != ps ? 1 : 0;
     if (better(isn, ps, idx, bestnan, best, besti)) { best = ps; besti = idx; bestnan = isn; }
   }
@@ -802,7 +807,7 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(const float* __rest
     o[2] = w;
     o[3] = h;
     o[4] = score;
-    o[5] = (float)exp(-(rc * sc - 1.0) * penalty_k);
+    o[5] = (float)exp(-(rc * sc - 1.0) * (hp != nullptr ? hp[3 * b] : penalty_k));
     o[6] = (float)sv[0];
     o[7] = (float)idx;
   }
@@ -1003,6 +1008,141 @@ __global__ void __launch_bounds__(256) paste_labels_kernel(const float* __restri
   if (inside) labels[pix] = (!nan && best_k >= 0 && best > seg_thr) ? (uint8_t)(best_k + 1) : (uint8_t)0;
 }
 
+// Fused paste-back + IouMeter.add counts (utils/average_meter_helper.py:71-113, as tools/tune_vos.py scores a frame)
+// for B streams.  Stream b's value v at a pixel of video video[b] is the cv2.warpAffine value of its mask (warp_sample
+// above, border -1, bit for bit with sm_warp_affine); pred = (double)v > thrs[t], target = anno > 0, and
+// counts[b][t] = (#(pred && target), #(pred || target)).  A pixel none of whose four taps falls inside the mask has
+// v == -1, which no threshold >= -1 passes, so:
+//   mask_iou_rect_kernel visits only the frame-space image of the source square [-2, side+1]^2 (the whole frame when
+//     the map is singular or not finite) and adds pred && target to the intersection and pred && !target to the union;
+//   mask_iou_target_kernel adds the rest of the union, the video's target pixel count, counted once per video (by the
+//     blocks of the first stream that reads it) and added to every stream of that video.
+// counts is zeroed first; both kernels only add.  The skip is exact only for thresholds >= -1 (a NaN threshold passes
+// nothing, which is exact too): a threshold below -1 gets no counts but the marker (-1, -1), stored by block 0 of the
+// rectangle kernel.  Inside the rectangle one warp covers 32 consecutive pixels and counts
+// every threshold with two ballots; lane t keeps threshold t's counts, so T <= 32.
+constexpr int MI_THREADS = 256;
+constexpr int MI_MAX_T = 32;
+constexpr int MI_TARGET_BYTES = 16384;      // annotation bytes per block of mask_iou_target_kernel
+
+__global__ void __launch_bounds__(MI_THREADS) mask_iou_target_kernel(const uint8_t* __restrict__ anno,
+                                                                     const int32_t* __restrict__ video, int B,
+                                                                     size_t HW, const double* __restrict__ thrs, int T,
+                                                                     int32_t* __restrict__ counts) {
+  __shared__ int s_red[MI_THREADS / 32];
+  const int b = blockIdx.y;
+  const int g = video[b];
+  int dup = 0;
+  for (int j = threadIdx.x; j < b; j += MI_THREADS) dup |= video[j] == g;
+  if (__syncthreads_or(dup)) return;                   // an earlier stream reads the same video and counts it
+  const uint8_t* a = anno + (size_t)g * HW;
+  const size_t c0 = (size_t)blockIdx.x * MI_TARGET_BYTES, c1 = min(c0 + (size_t)MI_TARGET_BYTES, HW);
+  int cnt = 0;
+  if (((HW | reinterpret_cast<uintptr_t>(anno)) & 3) == 0) {
+    const uint32_t* w = reinterpret_cast<const uint32_t*>(a);
+    for (size_t i = c0 / 4 + threadIdx.x; i < c1 / 4; i += MI_THREADS) cnt += __popc(__vcmpne4(w[i], 0u)) >> 3;
+  } else {
+    for (size_t i = c0 + threadIdx.x; i < c1; i += MI_THREADS) cnt += a[i] != 0;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = cnt;
+  __syncthreads();
+  int total = 0;
+#pragma unroll
+  for (int w = 0; w < MI_THREADS / 32; ++w) total += s_red[w];
+  if (total == 0) return;
+  for (int j = threadIdx.x; j < B * T; j += MI_THREADS)
+    if (video[j / T] == g && !(thrs[j % T] < -1.0)) atomicAdd(&counts[2 * (size_t)j + 1], total);
+}
+
+__global__ void __launch_bounds__(MI_THREADS) mask_iou_rect_kernel(const float* __restrict__ masks, int side,
+                                                                   const double* __restrict__ maps,
+                                                                   const uint8_t* __restrict__ anno,
+                                                                   const int32_t* __restrict__ video, int H, int W,
+                                                                   const double* __restrict__ thrs, int T,
+                                                                   int32_t* __restrict__ counts) {
+  __shared__ double s_inv[6];
+  __shared__ double s_thr[MI_MAX_T];
+  __shared__ int s_rect[4];
+  __shared__ int s_cnt[MI_MAX_T][2];
+  const int b = blockIdx.y;
+  if (threadIdx.x < T) {
+    s_thr[threadIdx.x] = thrs[threadIdx.x];
+    s_cnt[threadIdx.x][0] = 0;
+    s_cnt[threadIdx.x][1] = 0;
+  }
+  if (threadIdx.x == 0) {
+    const double* m = maps + 6 * (size_t)b;
+    double inv[6];
+    warp_invert_map(m, inv);
+    double xmn = INFINITY, xmx = -INFINITY, ymn = INFINITY, ymx = -INFINITY;
+    for (int c = 0; c < 4; ++c) {
+      const double u = (c & 1) ? side + 1.0 : -2.0, v = (c & 2) ? side + 1.0 : -2.0;
+      const double X = m[0] * u + m[1] * v + m[2], Y = m[3] * u + m[4] * v + m[5];
+      xmn = fmin(xmn, X); xmx = fmax(xmx, X); ymn = fmin(ymn, Y); ymx = fmax(ymx, Y);
+    }
+    bool ok = isfinite(xmn) && isfinite(xmx) && isfinite(ymn) && isfinite(ymx);
+    for (int k = 0; k < 6; ++k) ok = ok && isfinite(inv[k]);
+    ok = ok && !(inv[0] == 0.0 && inv[1] == 0.0 && inv[3] == 0.0 && inv[4] == 0.0);     // singular map
+    int r[4] = {0, 0, W, H};                                                              // [x0, x1) x [y0, y1)
+    if (ok) {
+      r[0] = (int)fmin(fmax(floor(xmn) - 1.0, 0.0), (double)W);
+      r[1] = (int)fmin(fmax(floor(ymn) - 1.0, 0.0), (double)H);
+      r[2] = (int)fmin(fmax(ceil(xmx) + 2.0, 0.0), (double)W);
+      r[3] = (int)fmin(fmax(ceil(ymx) + 2.0, 0.0), (double)H);
+    }
+    for (int k = 0; k < 6; ++k) s_inv[k] = inv[k];
+    for (int k = 0; k < 4; ++k) s_rect[k] = r[k];
+  }
+  __syncthreads();
+  double inv[6];
+#pragma unroll
+  for (int k = 0; k < 6; ++k) inv[k] = s_inv[k];
+  const int x0 = s_rect[0], y0 = s_rect[1], rw = s_rect[2] - x0, rh = s_rect[3] - y0;
+  const int n = rw > 0 && rh > 0 ? rw * rh : 0;
+  const float* src = masks + (size_t)b * side * side;
+  const uint8_t* a = anno + (size_t)video[b] * H * W;
+  const int lane = threadIdx.x & 31;
+  int ci = 0, cu = 0;                                  // lane t < T: intersection / union-outside-target of threshold t
+  // warp-uniform loop: each warp takes 32 consecutive pixels of the rectangle per iteration
+  for (int base = blockIdx.x * MI_THREADS + (threadIdx.x & ~31); base < n; base += gridDim.x * MI_THREADS) {
+    const int i = base + lane;
+    bool touch = false, tgt = false;
+    double v = -1.0;
+    if (i < n) {
+      const int ry = i / rw;
+      const int x = x0 + (i - ry * rw), y = y0 + ry;
+      tgt = a[(size_t)y * W + x] != 0;
+      const WarpTap tp = warp_tap(inv, x, y);
+      if (tp.touches(side, side)) {
+        touch = true;
+        v = (double)warp_sample(src, side, side, tp, -1.f);
+      }
+    }
+    if (!__any_sync(0xffffffffu, touch)) continue;     // every value is -1: no threshold passes
+    for (int t = 0; t < T; ++t) {
+      const bool pred = v > s_thr[t] && !(s_thr[t] < -1.0);
+      const unsigned bi = __ballot_sync(0xffffffffu, pred && tgt), bu = __ballot_sync(0xffffffffu, pred && !tgt);
+      if (lane == t) { ci += __popc(bi); cu += __popc(bu); }
+    }
+  }
+  if (lane < T && (ci | cu)) {
+    atomicAdd(&s_cnt[lane][0], ci);
+    atomicAdd(&s_cnt[lane][1], cu);
+  }
+  __syncthreads();
+  if (threadIdx.x < T) {
+    int32_t* c = counts + 2 * ((size_t)b * T + threadIdx.x);
+    if (s_thr[threadIdx.x] < -1.0) {
+      if (blockIdx.x == 0) { c[0] = -1; c[1] = -1; }
+      return;
+    }
+    if (s_cnt[threadIdx.x][0]) atomicAdd(&c[0], s_cnt[threadIdx.x][0]);
+    if (s_cnt[threadIdx.x][1]) atomicAdd(&c[1], s_cnt[threadIdx.x][1]);
+  }
+}
+
 // cv2.boundingRect(anno[g] == id) for one (g, id) query per block: min / max of the matching pixels' x and y.
 constexpr int LB_THREADS = 512;
 
@@ -1100,9 +1240,13 @@ __global__ void tracker_prepare_kernel(int B, const double* __restrict__ state, 
 
 __global__ void tracker_update_kernel(int B, double* __restrict__ state, const float* __restrict__ rec,
                                       const double* __restrict__ aux, const int32_t* __restrict__ imsize, TrackerHp hp,
-                                      int A, int R, double* __restrict__ maps, double* __restrict__ out) {
+                                      int A, int R, double* __restrict__ maps, double* __restrict__ out,
+                                      const double* __restrict__ hp_table) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
+  // per-stream (penalty_k, window_influence, lr) rows replace the struct's penalty_k and lr (sm_tracker_update_hp)
+  const double penalty_k = hp_table != nullptr ? hp_table[3 * b] : hp.penalty_k;
+  const double hp_lr = hp_table != nullptr ? hp_table[3 * b + 2] : hp.lr;
   const double px = state[4 * b], py = state[4 * b + 1], sw = state[4 * b + 2], sh = state[4 * b + 3];
   const double scale_x = aux[4 * b], sxr = aux[4 * b + 1], cx0 = aux[4 * b + 2], cy0 = aux[4 * b + 3];
   const float* r = rec + 8 * b;
@@ -1116,8 +1260,8 @@ __global__ void tracker_update_kernel(int B, double* __restrict__ state, const f
   sc = fmax(sc, 1.0 / sc);
   double rc = (tw / th) / (double)(w / h);
   rc = fmax(rc, 1.0 / rc);
-  const double penalty = exp(-(rc * sc - 1.0) * hp.penalty_k);
-  const double lr = penalty * (double)score * hp.lr;            // :241
+  const double penalty = exp(-(rc * sc - 1.0) * penalty_k);
+  const double lr = penalty * (double)score * hp_lr;            // :241
   const double p0 = (double)r[0] / scale_x, p1 = (double)r[1] / scale_x, p2 = (double)w / scale_x, p3 = (double)h / scale_x;
   double res_x = p0 + px, res_y = p1 + py;
   // both products rounded before the sum, as numpy evaluates them (:245-246; no FMA contraction)
@@ -1387,8 +1531,9 @@ void launch_warp_affine(const float* src, int sh, int sw, const double* maps, fl
 
 void launch_select(const float* cls, const float* loc, const float* anchors, const float* window, const double* tsz,
                    int B, int A, int R, double penalty_k, double window_influence, int32_t* best_idx, int32_t* pos,
-                   float* rec, cudaStream_t st) {
-  select_kernel<<<B, SEL_THREADS, 0, st>>>(cls, loc, anchors, window, tsz, A, R, penalty_k, window_influence, best_idx, pos, rec);
+                   float* rec, cudaStream_t st, const double* hp) {
+  select_kernel<<<B, SEL_THREADS, 0, st>>>(cls, loc, anchors, window, tsz, A, R, penalty_k, window_influence, best_idx, pos,
+                                           rec, hp);
   SMK_CUDA(cudaGetLastError());
 }
 
@@ -1399,8 +1544,9 @@ void launch_tracker_prepare(int B, const double* state, const int32_t* avg, cons
 }
 
 void launch_tracker_update(int B, double* state, const float* rec, const double* aux, const int32_t* imsize,
-                           const TrackerHp& hp, int A, int R, double* maps, double* out, cudaStream_t st) {
-  tracker_update_kernel<<<(B + 127) / 128, 128, 0, st>>>(B, state, rec, aux, imsize, hp, A, R, maps, out);
+                           const TrackerHp& hp, int A, int R, double* maps, double* out, cudaStream_t st,
+                           const double* hp_table) {
+  tracker_update_kernel<<<(B + 127) / 128, 128, 0, st>>>(B, state, rec, aux, imsize, hp, A, R, maps, out, hp_table);
   SMK_CUDA(cudaGetLastError());
 }
 
@@ -1415,6 +1561,20 @@ void launch_paste_labels(const float* masks, int side, const double* maps, const
                          const int32_t* objects, int G, int H, int W, double seg_thr, uint8_t* labels, cudaStream_t st) {
   dim3 block(32, 8), grid((W + 31) / 32, (H + 7) / 8, G);
   paste_labels_kernel<<<grid, block, 0, st>>>(masks, side, maps, anno, obj_off, objects, H, W, seg_thr, labels);
+  SMK_CUDA(cudaGetLastError());
+}
+
+void launch_mask_iou(const float* masks, int side, const double* maps, const uint8_t* anno, const int32_t* video, int B,
+                     int H, int W, const double* thrs, int T, int32_t* counts, cudaStream_t st) {
+  SMK_CHECK(T >= 1 && T <= MI_MAX_T, "1 <= T <= 32 thresholds");
+  SMK_CUDA(cudaMemsetAsync(counts, 0, (size_t)B * T * 2 * sizeof(int32_t), st));
+  const size_t HW = (size_t)H * W;
+  mask_iou_target_kernel<<<dim3((unsigned)((HW + MI_TARGET_BYTES - 1) / MI_TARGET_BYTES), B), MI_THREADS, 0, st>>>(
+      anno, video, B, HW, thrs, T, counts);
+  SMK_CUDA(cudaGetLastError());
+  // a pasted 127x127 mask spans some 10^4..10^5 pixels: 16 blocks per stream keep every SM busy at a few streams
+  const int per_stream = (int)std::min<size_t>(16, (HW + MI_THREADS * 8 - 1) / (MI_THREADS * 8));
+  mask_iou_rect_kernel<<<dim3(per_stream, B), MI_THREADS, 0, st>>>(masks, side, maps, anno, video, H, W, thrs, T, counts);
   SMK_CUDA(cudaGetLastError());
 }
 

@@ -266,6 +266,27 @@ class Custom:
             return buf
         return slots
 
+    def _check_hp(self, hp, B: int) -> torch.Tensor:
+        """A per-stream hyper-parameter table: float64 CUDA tensor [B,3] of finite (penalty_k, window_influence, lr)
+        rows.  The finiteness check reads the table back to the host, so it runs before anything is enqueued."""
+        if not (isinstance(hp, torch.Tensor) and hp.is_cuda and hp.dtype == torch.float64):
+            raise ValueError("hp must be a float64 CUDA tensor")
+        if hp.device != self._device:
+            raise ValueError(f"hp lives on {hp.device}, the engine on {self._device}")
+        if tuple(hp.shape) != (B, 3):
+            raise ValueError(f"hp must have shape [{B}, 3], got {tuple(hp.shape)}")
+        if not bool(torch.isfinite(hp).all()):
+            raise ValueError("hp entries must be finite")
+        return hp.contiguous()
+
+    def _stage_hp(self, hp: torch.Tensor) -> torch.Tensor:
+        """`_stage_slots` for the hyper-parameter table."""
+        if self.graphs:
+            buf = self._buf(("hp", hp.shape[0]), tuple(hp.shape), torch.float64)
+            buf.copy_(hp)
+            return buf
+        return hp
+
     @torch.no_grad()
     def template(self, z, slot0: int = 0, slots=None):
         """slots (optional): int32 CUDA tensor [B] of distinct engine slots; stream b's template is cached in slots[b]
@@ -366,19 +387,29 @@ class Custom:
 
     @torch.no_grad()
     def step(self, x, anchors, window, target_sz_in_crop, penalty_k: float, window_influence: float, slot0: int = 0,
-             refine: bool = True, mask_head: bool = False, mask_col: bool = False, slots=None):
+             refine: bool = True, mask_head: bool = False, mask_col: bool = False, slots=None, hp=None):
         """One whole frame of siamese_track (tools/test.py:201-261) in ONE engine call (C ABI `sm_step`):
         track(_mask) -> on-device selection -> track_refine at the selected position.  Returns a dict with cls, loc,
         mask (raw head or None), best, pos, records, refine (or None), mask_col (or None).  slots (optional): int32
-        CUDA tensor [B]; stream b then uses the template cached in slots[b] (`sm_step_slots`) instead of slot0 + b."""
+        CUDA tensor [B]; stream b then uses the template cached in slots[b] (`sm_step_slots`) instead of slot0 + b.
+        hp (optional): float64 CUDA tensor [B,3] of per-stream (penalty_k, window_influence, lr); stream b's selection
+        then uses row b instead of the two scalars (`sm_step_slots_hp`; without `slots` the table is slot0 + b)."""
+        B = x.shape[0]
         if slots is not None:
-            slots = self._check_slots(slots, x.shape[0], distinct=False)
+            slots = self._check_slots(slots, B, distinct=False)
+        if hp is not None:
+            hp = self._check_hp(hp, B)
+            if slots is None:
+                if slot0 < 0 or slot0 + B > self.num_slots:
+                    raise ValueError(f"slots {slot0}..{slot0 + B - 1} outside [0, {self.num_slots})")
+                slots = torch.arange(slot0, slot0 + B, dtype=torch.int32, device=self._device)
         return self._step(x, anchors, window, target_sz_in_crop, penalty_k, window_influence, slot0, refine, mask_head,
-                          mask_col, slots)
+                          mask_col, slots, hp)
 
     def _step(self, x, anchors, window, target_sz_in_crop, penalty_k, window_influence, slot0=0, refine=True,
-              mask_head=False, mask_col=False, slots=None):
-        """`step` without the host-side check of `slots` (callers that own a table they have validated)."""
+              mask_head=False, mask_col=False, slots=None, hp=None):
+        """`step` without the host-side checks of `slots` and `hp` (callers that own tables they have validated;
+        `hp` needs `slots`)."""
         x = self._prep(x, self.search_size)
         dev = self._device
         B, A, R = x.shape[0], self.anchor_num, self.score_size
@@ -408,8 +439,14 @@ class Custom:
         with torch.cuda.device(dev):
             if slots is not None:
                 slots = self._stage_slots(slots)
+            if hp is not None:
+                hp = self._stage_hp(hp)
             self._fence_in()
-            if slots is None:
+            if hp is not None:
+                _lib.check(self._lib.sm_step_slots_hp(self._engine, B, slots.data_ptr(), hp.data_ptr(), x.data_ptr(),
+                                                      tsz.data_ptr(), anchors.data_ptr(), window.data_ptr(), flags,
+                                                      *outs))
+            elif slots is None:
                 _lib.check(self._lib.sm_step(self._engine, slot0, B, x.data_ptr(), tsz.data_ptr(), anchors.data_ptr(),
                                              window.data_ptr(), float(penalty_k), float(window_influence), flags, *outs))
             else:
@@ -418,7 +455,7 @@ class Custom:
                                                    float(window_influence), flags, *outs))
             self._fence_out()
         self._last_B = B
-        self._keep = (anchors, window, tsz, slots)       # alive until the next call (the work is asynchronous)
+        self._keep = (anchors, window, tsz, slots, hp)   # alive until the next call (the work is asynchronous)
         return out
 
     # ------------------------------------------------------------------ introspection used by tests / bench

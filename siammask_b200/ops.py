@@ -183,3 +183,53 @@ def label_boxes(anno: torch.Tensor, queries) -> torch.Tensor:
     with torch.cuda.device(dev):
         _lib.check(lib.sm_label_boxes(anno.data_ptr(), G, H, W, q.data_ptr(), q.shape[0], out.data_ptr(), _stream(dev)))
     return out
+
+
+def mask_iou(masks, maps, anno, video, thrs) -> torch.Tensor:
+    """Fused paste-back + IoU counts of the reference's IouMeter.add (utils/average_meter_helper.py:71-113), as
+    tools/tune_vos.py scores each frame (C ABI `sm_mask_iou`).  masks f32 CUDA [B,side,side] (sigmoid masks) and maps
+    f64 [B,6] (forward paste-back maps) of B streams; anno uint8 CUDA [G,H,W] annotations; video int [B]: the video in
+    [0, G) stream b is scored against; thrs: 1..32 thresholds >= -1.  Returns int32 [B,T,2] = (intersection, union) of
+    pred = v > thrs[t] (compared in float64) and target = anno > 0, where v is the cv2.warpAffine(INTER_LINEAR,
+    BORDER_CONSTANT, -1) value of the mask, bit for bit with `warp_affine`.  The checks read `video` and `thrs` on the
+    host (one D2H copy each if they live on the device)."""
+    if not (torch.is_tensor(masks) and masks.is_cuda and masks.dtype == torch.float32 and masks.dim() == 3
+            and masks.shape[1] == masks.shape[2]):
+        raise ValueError("masks must be a float32 CUDA tensor [B, side, side]")
+    if not (torch.is_tensor(anno) and anno.is_cuda and anno.dtype == torch.uint8 and anno.dim() == 3):
+        raise ValueError("anno must be a uint8 CUDA tensor [G, H, W]")
+    B, G = int(masks.shape[0]), int(anno.shape[0])
+    m = torch.as_tensor(maps)
+    if m.dtype != torch.float64 or tuple(m.shape) != (B, 6):
+        raise ValueError(f"maps must be float64 [{B}, 6]")
+    v = np.asarray(video.cpu() if torch.is_tensor(video) else video)
+    if v.shape != (B,) or not np.issubdtype(v.dtype, np.integer):
+        raise ValueError(f"video must be an integer array [{B}]")
+    if B and ((v < 0) | (v >= G)).any():
+        raise ValueError(f"video entries must lie in [0, {G})")
+    t = np.asarray(thrs.cpu() if torch.is_tensor(thrs) else thrs, dtype=np.float64).reshape(-1)
+    if not 1 <= t.size <= 32:
+        raise ValueError("1 to 32 thresholds expected")
+    if not (t >= -1.0).all():
+        raise ValueError("thresholds must be >= -1 (pixels the mask misses have the value -1)")
+    if B == 0:
+        return torch.zeros(0, t.size, 2, dtype=torch.int32, device=masks.device)
+    dev = masks.device
+    return _mask_iou(masks, m.to(dev), anno, torch.as_tensor(v.astype(np.int32), device=dev),
+                     torch.as_tensor(t, device=dev))
+
+
+def _mask_iou(masks, maps, anno, video, thrs) -> torch.Tensor:
+    """`mask_iou` without the host-side checks (callers that validated `video` and `thrs` once); every argument is a
+    CUDA tensor of the documented dtype."""
+    lib = _lib.load()
+    dev = masks.device
+    masks, maps, anno, video, thrs = (t.contiguous() for t in (masks, maps, anno, video, thrs))
+    B, side = int(masks.shape[0]), int(masks.shape[-1])
+    _, H, W = anno.shape
+    T = int(thrs.numel())
+    out = torch.empty(B, T, 2, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.sm_mask_iou(masks.data_ptr(), side, maps.data_ptr(), anno.data_ptr(), video.data_ptr(), B, H, W,
+                                   thrs.data_ptr(), T, out.data_ptr(), _stream(dev)))
+    return out

@@ -7,18 +7,20 @@ mask paste-back — runs here as a fixed sequence of kernels over all streams (C
 
     sm_tracker_prepare      state -> crop boxes, target size in the crop, scale          (tools/test.py:180-198, 71-76)
     sm_crop_resize_indexed  uint8 frames -> f32 [N,3,S,S] search crops (cv2-exact)        (:67-110)
-    sm_step_slots           track_mask -> select -> track_refine                          (:201-261)
-    sm_tracker_update       winner box + score -> new state (lr, clamps), paste-back map  (:239-249, 263-282, 305-315)
+    sm_step_slots_hp        track_mask -> select -> track_refine                          (:201-261)
+    sm_tracker_update_hp    winner box + score -> new state (lr, clamps), paste-back map  (:239-249, 263-282, 305-315)
     sm_warp_affine          127x127 sigmoid mask -> frame, threshold                      (:263-284)
 
 The state (target_pos, target_sz, float64) lives on the device; a frame costs one small D2H copy only if the caller
 asks for the numbers (`TrackResult.cpu()`).  Contour extraction / minAreaRect (:285-303) is not part of this module.
 
 Streams join and leave a running tracker: `add` templates new streams into free engine slots, `remove` frees them.  The
-active streams are kept as compact rows (state, slot, frame index), and every frame runs exactly those rows as one
-batch through the slot table (`sm_step_slots`) and the frame-index table (`sm_crop_resize_indexed`); both tables are
-uploaded only when the set changes.  Each stream reads one frame of the tensor passed to `track`: its frame index, set
-by `add` (for `init`, stream i reads frame i; a single [H,W,3] frame is shared by all streams).
+active streams are kept as compact rows (state, slot, frame index, hyper-parameters), and every frame runs exactly those
+rows as one batch through the slot table and the per-stream (penalty_k, window_influence, lr) table
+(`sm_step_slots_hp`, `sm_tracker_update_hp`) and the frame-index table (`sm_crop_resize_indexed`); the tables are
+uploaded only when the set changes.  A stream's hyper-parameters default to the tracker's `TrackerParams`.  Each stream
+reads one frame of the tensor passed to `track`: its frame index, set by `add` (for `init`, stream i reads frame i; a
+single [H,W,3] frame is shared by all streams).
 
 The arithmetic is pinned by `tests/test_batch_tracker.py` to the reference loop's golden trajectory and to
 single-stream runs of the host restatement in `oracle/ref_loop.py`.
@@ -63,8 +65,8 @@ class TrackerParams:
 @dataclass
 class TrackResult:
     """Per-frame outputs, all on the device, one row per active stream in the order of `BatchTracker.ids`.  state f64
-    [N,8] = x, y, w, h (new target_pos / target_sz), score, penalty, lr, best index; mask: bool [N,H,W] frame-sized masks
-    (or None).  With mask=True, extras also holds "mask_prob" f32 [N,side,side] (sigmoid masks) and "maps" f64 [N,6]
+    [N,8] = x, y, w, h (new target_pos / target_sz), score, penalty, lr (from the stream's own lr), best index; mask:
+    bool [N,H,W] frame-sized masks (or None).  With mask=True, extras also holds "mask_prob" f32 [N,side,side] (sigmoid masks) and "maps" f64 [N,6]
     (their paste-back maps, overwritten by the next frame)."""
     state: torch.Tensor
     mask: torch.Tensor | None = None
@@ -100,6 +102,7 @@ class BatchTracker:
         self._ids: list[int] = []
         self._slots: list[int] = []
         self._fidx: list[int] = []
+        self._hp: list[tuple[float, float, float]] = []
         self.im_w = self.im_h = None
         dev = self.dev
         self.state = torch.zeros(0, 4, dtype=torch.float64, device=dev)
@@ -150,6 +153,7 @@ class BatchTracker:
         self._slots_dev = torch.tensor(self._slots, dtype=torch.int32, device=dev)
         self._fidx_dev = torch.tensor(self._fidx, dtype=torch.int32, device=dev)
         self._max_fidx = max(self._fidx) if self._fidx else -1
+        self._hp_dev = torch.tensor(self._hp, dtype=torch.float64, device=dev).reshape(N, 3)
         self.boxes = torch.zeros(N, 8, dtype=torch.int32, device=dev)
         self.tsz = torch.zeros(N, 2, dtype=torch.float64, device=dev)
         self.aux = torch.zeros(N, 4, dtype=torch.float64, device=dev)
@@ -157,11 +161,12 @@ class BatchTracker:
 
     # ------------------------------------------------------------------ stream lifecycle
     @torch.no_grad()
-    def add(self, frames, boxes_xywh, frame_index=None) -> list[int]:
+    def add(self, frames, boxes_xywh, frame_index=None, hp=None) -> list[int]:
         """siamese_init (tools/test.py:132-169) for new streams, which join the running batch in free engine slots.
         frames: uint8 [F,H,W,3] (or one shared [H,W,3]); boxes_xywh: [n,4] top-left x, y, w, h of the targets;
         frame_index: [n] frame of `frames` each new stream reads, now and in every later `track` (default: stream i reads
-        frame i).  Returns the new streams' ids."""
+        frame i); hp: [n,3] per-stream (penalty_k, window_influence, lr) (default: the tracker's `TrackerParams`).
+        Returns the new streams' ids."""
         with torch.cuda.device(self.dev):
             fr = self._frames(frames)
             bx = torch.as_tensor(np.asarray(boxes_xywh, dtype=np.float64)).reshape(-1, 4).to(self.dev)
@@ -177,6 +182,15 @@ class BatchTracker:
                 raise ValueError(f"frame index out of range [0, {F})")
             if any(i < 0 for i in idx):
                 raise ValueError("frame indices must be >= 0")
+            if hp is None:
+                rows = [(float(self.p.penalty_k), float(self.p.window_influence), float(self.p.lr))] * n
+            else:
+                h = np.asarray(hp.cpu() if torch.is_tensor(hp) else hp, dtype=np.float64)
+                if h.shape != (n, 3):
+                    raise ValueError(f"hp must have shape [{n}, 3] (penalty_k, window_influence, lr), got {h.shape}")
+                if not np.isfinite(h).all():
+                    raise ValueError("hp entries must be finite")
+                rows = [tuple(float(v) for v in r) for r in h]
             used = set(self._slots)
             free = [s for s in range(self.slot0, self.net.num_slots) if s not in used][:n]
             if n == 0:
@@ -216,6 +230,7 @@ class BatchTracker:
             self._ids += ids
             self._slots += free
             self._fidx += idx
+            self._hp += rows
             self.N += n
             self._upload_tables()
         return ids
@@ -238,6 +253,7 @@ class BatchTracker:
             self._ids = [self._ids[r] for r in keep]
             self._slots = [self._slots[r] for r in keep]
             self._fidx = [self._fidx[r] for r in keep]
+            self._hp = [self._hp[r] for r in keep]
             self.N = len(keep)
             self._upload_tables()
 
@@ -275,11 +291,13 @@ class BatchTracker:
             use_refine = mask and refine
             use_head = mask and not refine
             out = self.net._step(x, self.anchors, self.window, self.tsz, p.penalty_k, p.window_influence,
-                                 refine=use_refine, mask_head=use_head, mask_col=use_head, slots=self._slots_dev)
+                                 refine=use_refine, mask_head=use_head, mask_col=use_head, slots=self._slots_dev,
+                                 hp=self._hp_dev)
             res = torch.empty(N, 8, dtype=torch.float64, device=self.dev)
-            _lib.check(self.lib.sm_tracker_update(N, self.state.data_ptr(), out["records"].data_ptr(), self.aux.data_ptr(),
-                                                  self.imsize.data_ptr(), C.byref(self.hp), self.net.anchor_num,
-                                                  p.score_size, self.maps.data_ptr() if mask else None, res.data_ptr(), st))
+            _lib.check(self.lib.sm_tracker_update_hp(N, self.state.data_ptr(), out["records"].data_ptr(),
+                                                     self.aux.data_ptr(), self.imsize.data_ptr(), C.byref(self.hp),
+                                                     self._hp_dev.data_ptr(), self.net.anchor_num, p.score_size,
+                                                     self.maps.data_ptr() if mask else None, res.data_ptr(), st))
             extras = {"records": out["records"], "pos": out["pos"], "x_crop": x, "ids": list(self._ids)}
             mask_out = None
             if mask:
