@@ -138,6 +138,24 @@ int sm_paste_labels(const float* masks, int32_t side, const double* maps, const 
                     const int32_t* objects, int32_t G, int32_t H, int32_t W, double seg_thr, uint8_t* labels,
                     void* stream);
 
+/* sm_paste_labels fused with the per-object IoU counts of MultiBatchIouMeter (tools/test.py:421-456), the score
+ * track_vos computes for a video, for one frame of G videos.  masks, side, maps, anno, obj_offsets, objects, seg_thr and
+ * labels are those of sm_paste_labels, and labels equals its output bit for bit; anno is required.  target_ids (device
+ * int32 [n], n = obj_offsets[G]) is the annotation value entry i is scored against (1..255), or -1 for an entry that is
+ * not scored (it matches no pixel).  For each of the T thresholds thrs (device f64 [T]), label_t = (first argmax + 1) *
+ * (max > thrs[t]) in double, and counts (device int32 [n][T][2]) = (intersection, union) of label_t == k+1 and
+ * anno[g] == target_ids[i], where k is entry i's position within its video.  The call sets counts itself.
+ * Preconditions:
+ *   - T <= 32 and thrs[t] >= -1: objects whose four taps all miss the mask are skipped, which is exact only for
+ *     thresholds >= -1; a threshold below -1 yields counts (-1, -1);
+ *   - the scored target ids of a video are unique;
+ *   - at most 255 objects per video (a video with more gets no labels and no counts).
+ * One pass over each frame; per-object frames are never materialised.  All pointers are device pointers. */
+int sm_paste_labels_iou(const float* masks, int32_t side, const double* maps, const uint8_t* anno,
+                        const int32_t* obj_offsets, const int32_t* objects, const int32_t* target_ids, int32_t G,
+                        int32_t H, int32_t W, double seg_thr, uint8_t* labels, const double* thrs, int32_t T,
+                        int32_t* counts, void* stream);
+
 /* Fused paste-back + IoU counts of IouMeter.add (utils/average_meter_helper.py:71-113), the per-frame score of
  * tools/tune_vos.py, for B streams of one frame size H x W.  Stream b's value v at a pixel is
  * cv2.warpAffine(masks[b], maps[b], (W, H), INTER_LINEAR, BORDER_CONSTANT, -1), bit for bit with sm_warp_affine

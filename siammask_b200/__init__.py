@@ -8,11 +8,11 @@ Public surface mirrors the reference's model object for that path:
 All compute lives in libsiammask_b200.so (C ABI: include/siammask_b200.h)."""
 from .custom import Custom, DEFAULT_ANCHORS
 from .ops import conv2d_dw_group, xcorr_depthwise, conv2d, crop_resize, warp_affine, paste_labels, label_boxes, \
-    mask_iou
+    mask_iou, paste_labels_iou
 from .checkpoint import synthetic_state_dict, load_checkpoint, expected_keys
-from .vos import VideoSegmenter
+from .vos import VideoSegmenter, VOS_THRESHOLDS
 from .tune import ParamSweep
 
 __all__ = ["Custom", "DEFAULT_ANCHORS", "conv2d_dw_group", "xcorr_depthwise", "conv2d", "crop_resize", "warp_affine",
-           "paste_labels", "label_boxes", "mask_iou", "VideoSegmenter", "ParamSweep", "synthetic_state_dict",
-           "load_checkpoint", "expected_keys"]
+           "paste_labels", "label_boxes", "mask_iou", "paste_labels_iou", "VideoSegmenter", "VOS_THRESHOLDS",
+           "ParamSweep", "synthetic_state_dict", "load_checkpoint", "expected_keys"]

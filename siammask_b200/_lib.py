@@ -80,6 +80,8 @@ SIGNATURES = {
                                          C.c_int32, C.c_void_p, C.c_void_p]),
     "sm_paste_labels": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 4 + [C.c_int32] * 3 +
                         [C.c_double, C.c_void_p, C.c_void_p]),
+    "sm_paste_labels_iou": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 5 + [C.c_int32] * 3 +
+                            [C.c_double, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "sm_label_boxes": (C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "sm_step_host_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(SmStepIO), C.c_void_p,
                                      C.POINTER(C.c_int32)]),

@@ -155,6 +155,11 @@ void launch_scatter_slots(const __half* src_hi, const __half* src_lo, __half* ds
 // sm_paste_labels / sm_label_boxes (include/siammask_b200.h)
 void launch_paste_labels(const float* masks, int side, const double* maps, const uint8_t* anno, const int32_t* obj_off,
                          const int32_t* objects, int G, int H, int W, double seg_thr, uint8_t* labels, cudaStream_t st);
+// sm_paste_labels_iou: the same labels plus per-entry IoU counts; counts must hold obj_off[G]*T*2 int32
+void launch_paste_labels_iou(const float* masks, int side, const double* maps, const uint8_t* anno,
+                             const int32_t* obj_off, const int32_t* objects, const int32_t* target_ids, int G, int H,
+                             int W, double seg_thr, uint8_t* labels, const double* thrs, int T, int32_t* counts,
+                             cudaStream_t st);
 void launch_label_boxes(const uint8_t* anno, int G, int H, int W, const int32_t* queries, int Q, int32_t* boxes,
                         cudaStream_t st);
 void launch_absmax(const Act& a, float* slot, cudaStream_t st);

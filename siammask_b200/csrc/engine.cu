@@ -1989,6 +1989,22 @@ int sm_paste_labels(const float* masks, int32_t side, const double* maps, const 
   SM_API_END
 }
 
+int sm_paste_labels_iou(const float* masks, int32_t side, const double* maps, const uint8_t* anno,
+                        const int32_t* obj_offsets, const int32_t* objects, const int32_t* target_ids, int32_t G,
+                        int32_t H, int32_t W, double seg_thr, uint8_t* labels, const double* thrs, int32_t T,
+                        int32_t* counts, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(anno && obj_offsets && objects && target_ids && labels && thrs && counts && G >= 1 && H > 0 && W > 0 &&
+            side > 0, "bad argument");
+  SMK_CHECK(seg_thr >= -1.0, "seg_thr must be >= -1 (objects that miss a pixel are skipped as value -1)");
+  SMK_CHECK((int64_t)H * W <= INT32_MAX, "frame too large for int32 counts");
+  SMK_CHECK(T >= 1 && T <= 32, "1 <= T <= 32 thresholds");
+  require_device();
+  smk::launch_paste_labels_iou(masks, side, maps, anno, obj_offsets, objects, target_ids, G, H, W, seg_thr, labels, thrs,
+                               T, counts, static_cast<cudaStream_t>(stream));
+  SM_API_END
+}
+
 int sm_mask_iou(const float* masks, int32_t side, const double* maps, const uint8_t* anno, const int32_t* video,
                 int32_t B, int32_t H, int32_t W, const double* thrs, int32_t T, int32_t* counts, void* stream) {
   SM_API_BEGIN

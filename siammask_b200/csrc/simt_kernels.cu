@@ -941,29 +941,37 @@ __global__ void warp_affine_kernel(const float* __restrict__ src, int sh, int sw
 // whose value at a pixel is -1 can never win for seg_thr >= -1 and are skipped: idle objects, and tracked objects none
 // of whose four taps falls inside the mask (per block first, conservatively, then exactly per pixel).  A NaN value makes
 // np.max NaN, hence label 0.  Block = 32 x 8 pixels of one video; objects are staged in shared memory in chunks, each
-// map inverted once per block.
+// map inverted once per block.  The per-pixel max / first argmax (paste_best) is shared with paste_labels_iou_kernel
+// (sm_paste_labels_iou), whose labels must equal these bit for bit.
 constexpr int PL_CHUNK = 64;
 
-__global__ void __launch_bounds__(256) paste_labels_kernel(const float* __restrict__ masks, int side,
-                                                           const double* __restrict__ maps, const uint8_t* __restrict__ anno,
-                                                           const int32_t* __restrict__ obj_off,
-                                                           const int32_t* __restrict__ objects, int H, int W,
-                                                           double seg_thr, uint8_t* __restrict__ labels) {
+// The objects of video blockIdx.z are entries [o0, o1) of the table: labels are uint8, so a video with more than 255
+// objects (a violated precondition) gets no objects, i.e. label 0, rather than wrapped labels.
+__device__ __forceinline__ int2 paste_range(const int32_t* __restrict__ obj_off, int g) {
+  const int o0 = obj_off[g];
+  return make_int2(o0, obj_off[g + 1] - o0 > 255 ? o0 : obj_off[g + 1]);
+}
+
+struct PasteBest {
+  double v;      // max over the visited objects' values
+  int k;         // its first argmax (video-local entry), -1 when no object was visited
+  bool nan;      // some visited value was NaN (np.max is NaN: label 0)
+  __device__ __forceinline__ bool passes(double thr) const { return !nan && k >= 0 && v > thr; }
+};
+
+// Max / first argmax of pixel (x, y) of video g over entries [o0, o1).  Block = 32 x 8 pixels at (bx0, by0); every
+// thread of the block calls it (objects are staged in shared memory between barriers).
+__device__ __forceinline__ PasteBest paste_best(const float* __restrict__ masks, int side, const double* __restrict__ maps,
+                                                const uint8_t* __restrict__ anno, const int32_t* __restrict__ objects,
+                                                int o0, int o1, int bx0, int by0, int x, int y, int H, int W,
+                                                size_t pix) {
   __shared__ double s_inv[PL_CHUNK][6];
   __shared__ int s_kind[PL_CHUNK], s_arg[PL_CHUNK];
-  const int g = blockIdx.z;
   const int tid = threadIdx.y * 32 + threadIdx.x;
-  const int bx0 = blockIdx.x * 32, by0 = blockIdx.y * 8;
-  const int x = bx0 + threadIdx.x, y = by0 + threadIdx.y;
   const bool inside = x < W && y < H;
-  const int o0 = obj_off[g];
-  // labels are uint8: a video with more than 255 objects (a violated precondition) gets no objects, i.e. label 0,
-  // rather than wrapped labels
-  const int o1 = obj_off[g + 1] - o0 > 255 ? o0 : obj_off[g + 1];
   double best = 0.0;
   int best_k = -1;
   bool nan = false;
-  const size_t pix = ((size_t)g * H + y) * W + x;
   for (int c0 = o0; c0 < o1; c0 += PL_CHUNK) {
     const int n = min(PL_CHUNK, o1 - c0);
     __syncthreads();                                   // the previous chunk is no longer read
@@ -1005,7 +1013,112 @@ __global__ void __launch_bounds__(256) paste_labels_kernel(const float* __restri
       if (best_k < 0 || v > best) { best = v; best_k = c0 - o0 + k; }
     }
   }
-  if (inside) labels[pix] = (!nan && best_k >= 0 && best > seg_thr) ? (uint8_t)(best_k + 1) : (uint8_t)0;
+  return PasteBest{best, best_k, nan};
+}
+
+__global__ void __launch_bounds__(256) paste_labels_kernel(const float* __restrict__ masks, int side,
+                                                           const double* __restrict__ maps, const uint8_t* __restrict__ anno,
+                                                           const int32_t* __restrict__ obj_off,
+                                                           const int32_t* __restrict__ objects, int H, int W,
+                                                           double seg_thr, uint8_t* __restrict__ labels) {
+  const int g = blockIdx.z;
+  const int bx0 = blockIdx.x * 32, by0 = blockIdx.y * 8;
+  const int x = bx0 + threadIdx.x, y = by0 + threadIdx.y;
+  const int2 o = paste_range(obj_off, g);
+  const size_t pix = ((size_t)g * H + y) * W + x;
+  const PasteBest b = paste_best(masks, side, maps, anno, objects, o.x, o.y, bx0, by0, x, y, H, W, pix);
+  if (x < W && y < H) labels[pix] = b.passes(seg_thr) ? (uint8_t)(b.k + 1) : (uint8_t)0;
+}
+
+// sm_paste_labels_iou: the label map of paste_labels_kernel plus, for T thresholds, the (intersection, union) of
+// label_t == k+1 (label_t = (first argmax + 1) * (max > thrs[t])) against anno[g] == target_ids[k] for every entry k of
+// video g — MultiBatchIouMeter of tools/test.py:421-456 for one frame.  Per pixel only two entries can count: the winner
+// w (pixels labelled w+1 at threshold t: into the intersection of w when anno names w's target, else into w's union)
+// and the entry a whose target anno names (a's target count, added to each of a's unions).  anno value -> entry is a
+// 256-byte shared table.  Counters live in shared memory for PL_CHUNK entries at a time (one pass per chunk over the
+// per-pixel results kept in registers); lanes of a warp that add to the same counters are aggregated with
+// __match_any_sync, and each non-zero block counter is one global atomic.  The counts are zeroed (or set to the marker
+// (-1, -1) for a threshold below -1) by paste_iou_init_kernel before.
+constexpr int PI_MAX_T = 32;
+constexpr uint8_t PI_NONE = 0xFF;                    // no entry (video-local entries are 0..254)
+
+__global__ void paste_iou_init_kernel(const int32_t* __restrict__ obj_off, int G, const double* __restrict__ thrs,
+                                      int T, int32_t* __restrict__ counts) {
+  const int n2 = obj_off[G] * T;
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n2; j += gridDim.x * blockDim.x) {
+    const int32_t v = thrs[j % T] < -1.0 ? -1 : 0;
+    counts[2 * (size_t)j] = v;
+    counts[2 * (size_t)j + 1] = v;
+  }
+}
+
+__global__ void __launch_bounds__(256) paste_labels_iou_kernel(const float* __restrict__ masks, int side,
+                                                               const double* __restrict__ maps,
+                                                               const uint8_t* __restrict__ anno,
+                                                               const int32_t* __restrict__ obj_off,
+                                                               const int32_t* __restrict__ objects,
+                                                               const int32_t* __restrict__ target_ids, int H, int W,
+                                                               double seg_thr, uint8_t* __restrict__ labels,
+                                                               const double* __restrict__ thrs, int T,
+                                                               int32_t* __restrict__ counts) {
+  __shared__ uint8_t s_entry[256];                   // anno value -> video-local entry scored against it
+  __shared__ double s_thr[PI_MAX_T];
+  __shared__ int s_int[PL_CHUNK][PI_MAX_T];          // pixels labelled k+1 inside k's target
+  __shared__ int s_out[PL_CHUNK][PI_MAX_T];          // pixels labelled k+1 outside k's target
+  __shared__ int s_tgt[PL_CHUNK];                    // k's target pixels
+  const int g = blockIdx.z;
+  const int tid = threadIdx.y * 32 + threadIdx.x, lane = threadIdx.x;
+  const int bx0 = blockIdx.x * 32, by0 = blockIdx.y * 8;
+  const int x = bx0 + threadIdx.x, y = by0 + threadIdx.y;
+  const bool inside = x < W && y < H;
+  const int2 o = paste_range(obj_off, g);
+  s_entry[tid] = PI_NONE;                            // 256 threads
+  if (tid < T) s_thr[tid] = thrs[tid];
+  __syncthreads();
+  for (int k = tid; k < o.y - o.x; k += 256) {
+    const int id = target_ids[o.x + k];
+    if (id >= 1 && id <= 255) s_entry[id] = (uint8_t)k;       // ids are unique within a video (precondition)
+  }
+  __syncthreads();
+  const size_t pix = ((size_t)g * H + y) * W + x;
+  const PasteBest b = paste_best(masks, side, maps, anno, objects, o.x, o.y, bx0, by0, x, y, H, W, pix);
+  if (inside) labels[pix] = b.passes(seg_thr) ? (uint8_t)(b.k + 1) : (uint8_t)0;
+  unsigned pm = 0;                                  // bit t: the pixel is labelled b.k + 1 at threshold t
+  for (int t = 0; t < T; ++t)
+    if (!(s_thr[t] < -1.0) && b.passes(s_thr[t])) pm |= 1u << t;
+  const int w = inside && pm ? b.k : -1;
+  const int a = inside ? (s_entry[anno[pix]] == PI_NONE ? -1 : (int)s_entry[anno[pix]]) : -1;
+  const bool hit = w >= 0 && w == a;
+  for (int c0 = 0; c0 < o.y - o.x; c0 += PL_CHUNK) {
+    const int n = min(PL_CHUNK, o.y - o.x - c0);
+    __syncthreads();                                 // the previous chunk's counters are flushed
+    for (int j = tid; j < n * PI_MAX_T; j += 256) {
+      (&s_int[0][0])[j] = 0;
+      (&s_out[0][0])[j] = 0;
+    }
+    if (tid < n) s_tgt[tid] = 0;
+    __syncthreads();
+    const int kw = w >= c0 && w < c0 + n ? w - c0 : -1;
+    const unsigned long long key = kw < 0 ? ~0ull : ((unsigned long long)pm << 32) | ((unsigned)kw << 1) | (hit ? 1u : 0u);
+    const unsigned gw = __match_any_sync(0xffffffffu, key);
+    if (kw >= 0 && lane == __ffs(gw) - 1) {
+      const int cnt = __popc(gw);
+      int* row = hit ? s_int[kw] : s_out[kw];
+      for (unsigned m = pm; m; m &= m - 1) atomicAdd(&row[__ffs(m) - 1], cnt);
+    }
+    const int ka = a >= c0 && a < c0 + n ? a - c0 : -1;
+    const unsigned ga = __match_any_sync(0xffffffffu, ka);
+    if (ka >= 0 && lane == __ffs(ga) - 1) atomicAdd(&s_tgt[ka], __popc(ga));
+    __syncthreads();
+    for (int j = tid; j < n * T; j += 256) {
+      const int k = j / T, t = j - k * T;
+      if (s_thr[t] < -1.0) continue;
+      const int ci = s_int[k][t], cu = s_out[k][t] + s_tgt[k];
+      int32_t* c = counts + 2 * ((size_t)(o.x + c0 + k) * T + t);
+      if (ci) atomicAdd(&c[0], ci);
+      if (cu) atomicAdd(&c[1], cu);
+    }
+  }
 }
 
 // Fused paste-back + IouMeter.add counts (utils/average_meter_helper.py:71-113, as tools/tune_vos.py scores a frame)
@@ -1561,6 +1674,20 @@ void launch_paste_labels(const float* masks, int side, const double* maps, const
                          const int32_t* objects, int G, int H, int W, double seg_thr, uint8_t* labels, cudaStream_t st) {
   dim3 block(32, 8), grid((W + 31) / 32, (H + 7) / 8, G);
   paste_labels_kernel<<<grid, block, 0, st>>>(masks, side, maps, anno, obj_off, objects, H, W, seg_thr, labels);
+  SMK_CUDA(cudaGetLastError());
+}
+
+void launch_paste_labels_iou(const float* masks, int side, const double* maps, const uint8_t* anno,
+                             const int32_t* obj_off, const int32_t* objects, const int32_t* target_ids, int G, int H,
+                             int W, double seg_thr, uint8_t* labels, const double* thrs, int T, int32_t* counts,
+                             cudaStream_t st) {
+  SMK_CHECK(T >= 1 && T <= PI_MAX_T, "1 <= T <= 32 thresholds");
+  // the number of entries lives on the device (obj_off[G]): a grid-stride init sized for a few hundred of them
+  paste_iou_init_kernel<<<std::min(G, 32), 256, 0, st>>>(obj_off, G, thrs, T, counts);
+  SMK_CUDA(cudaGetLastError());
+  dim3 block(32, 8), grid((W + 31) / 32, (H + 7) / 8, G);
+  paste_labels_iou_kernel<<<grid, block, 0, st>>>(masks, side, maps, anno, obj_off, objects, target_ids, H, W, seg_thr,
+                                                  labels, thrs, T, counts);
   SMK_CUDA(cudaGetLastError());
 }
 

@@ -124,12 +124,7 @@ def paste_labels(masks, maps, anno, obj_offsets, objects, size, seg_thr: float) 
     Returns labels uint8 [G,H,W] = (first argmax over the video's objects + 1) * (max > seg_thr) in float64.
     The offsets are checked on the host (one D2H copy if they live on the device): non-decreasing, covering `objects`,
     at most 255 objects per video (labels are uint8)."""
-    off = np.asarray(obj_offsets.cpu() if torch.is_tensor(obj_offsets) else obj_offsets, dtype=np.int64).reshape(-1)
-    n = int(np.prod(objects.shape[:-1])) if torch.is_tensor(objects) else len(np.asarray(objects).reshape(-1, 2))
-    if off.size < 2 or off[0] != 0 or off[-1] != n or (np.diff(off) < 0).any():
-        raise ValueError(f"obj_offsets must rise from 0 to the number of objects ({n})")
-    if (np.diff(off) > 255).any():
-        raise ValueError("at most 255 objects per video (labels are uint8)")
+    _check_offsets(obj_offsets, _num_entries(objects))
     return _paste_labels(masks, maps, anno, obj_offsets, objects, size, seg_thr)
 
 
@@ -164,6 +159,82 @@ def _paste_labels(masks, maps, anno, obj_offsets, objects, size, seg_thr: float)
                                        off.data_ptr(), obj.data_ptr(), G, H, W, float(seg_thr), out.data_ptr(),
                                        _stream(dev)))
     return out
+
+
+def _num_entries(objects) -> int:
+    return int(np.prod(objects.shape[:-1])) if torch.is_tensor(objects) else len(np.asarray(objects).reshape(-1, 2))
+
+
+def _check_offsets(obj_offsets, n: int) -> np.ndarray:
+    off = np.asarray(obj_offsets.cpu() if torch.is_tensor(obj_offsets) else obj_offsets, dtype=np.int64).reshape(-1)
+    if off.size < 2 or off[0] != 0 or off[-1] != n or (np.diff(off) < 0).any():
+        raise ValueError(f"obj_offsets must rise from 0 to the number of objects ({n})")
+    if (np.diff(off) > 255).any():
+        raise ValueError("at most 255 objects per video (labels are uint8)")
+    return off
+
+
+def paste_labels_iou(masks, maps, anno, obj_offsets, objects, target_ids, size, seg_thr: float, thrs):
+    """`paste_labels` fused with the per-object IoU counts of the reference's MultiBatchIouMeter (tools/test.py:421-456)
+    for one frame (C ABI `sm_paste_labels_iou`).  The arguments of `paste_labels` mean the same, but anno uint8 CUDA
+    [G,H,W] is required; target_ids int [n]: the annotation value entry i is scored against (1..255, unique within its
+    video) or -1 (not scored: it matches no pixel); thrs: 1..32 thresholds >= -1.  Returns (labels uint8 [G,H,W], equal
+    to `paste_labels` bit for bit, counts int32 [n,T,2]) where counts[i,t] = (intersection, union) of
+    label_t == k+1 and anno[g] == target_ids[i], label_t = (first argmax + 1) * (max > thrs[t]) in float64 and k the
+    entry's position within its video g.  The checks read the offsets, target_ids and thrs on the host."""
+    from .tune import _check_thresholds
+    n = _num_entries(objects)
+    off = _check_offsets(obj_offsets, n)
+    t = _check_thresholds(thrs.cpu() if torch.is_tensor(thrs) else thrs)
+    ids = np.asarray(target_ids.cpu() if torch.is_tensor(target_ids) else target_ids).reshape(-1)
+    if ids.size != n or (n and not np.issubdtype(ids.dtype, np.integer)):
+        raise ValueError(f"target_ids must be an integer array [{n}]")
+    if ((ids != -1) & ((ids < 1) | (ids > 255))).any():
+        raise ValueError("target_ids must lie in 1..255, or be -1 for an entry that is not scored")
+    for g in range(off.size - 1):
+        v = ids[off[g]:off[g + 1]]
+        v = v[v != -1]
+        if np.unique(v).size != v.size:
+            raise ValueError(f"video {g}: target_ids must be unique within a video")
+    G, H, W = off.size - 1, int(size[0]), int(size[1])
+    if not (torch.is_tensor(anno) and anno.is_cuda and anno.dtype == torch.uint8 and tuple(anno.shape) == (G, H, W)):
+        raise ValueError(f"anno must be a uint8 CUDA tensor [{G},{H},{W}]")
+    dev = anno.device
+    return _paste_labels_iou(masks, maps, anno, obj_offsets, objects,
+                             torch.as_tensor(ids.astype(np.int32), device=dev), size, seg_thr,
+                             torch.as_tensor(t, device=dev))
+
+
+def _paste_labels_iou(masks, maps, anno, obj_offsets, objects, target_ids, size, seg_thr: float, thrs, counts=None):
+    """`paste_labels_iou` without the host-side checks (callers that validated their tables once): anno uint8, target_ids
+    int32 and thrs float64 are CUDA tensors.  counts (optional): a contiguous int32 CUDA tensor [n,T,2] to write into."""
+    off = torch.as_tensor(obj_offsets, dtype=torch.int32).reshape(-1)
+    G = off.numel() - 1
+    H, W = int(size[0]), int(size[1])
+    dev = anno.device
+    anno = anno.contiguous()
+    lib = _lib.load()
+    off = off.to(dev).contiguous()
+    obj = torch.as_tensor(objects, dtype=torch.int32).reshape(-1, 2)
+    n, T = int(obj.shape[0]), int(thrs.numel())
+    obj = (obj if obj.numel() else torch.zeros(1, 2, dtype=torch.int32)).to(dev).contiguous()
+    tid = target_ids if n else torch.full((1,), -1, dtype=torch.int32, device=dev)
+    side = 1
+    if masks is not None:
+        masks = masks.to(dev, torch.float32).contiguous()
+        side = int(masks.shape[-1])
+        maps = torch.as_tensor(maps, dtype=torch.float64).reshape(-1, 6).to(dev).contiguous()
+    if counts is None:
+        counts = torch.empty(n, T, 2, dtype=torch.int32, device=dev)
+    cnt = counts if n else torch.empty(1, T, 2, dtype=torch.int32, device=dev)
+    labels = torch.empty(G, H, W, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.sm_paste_labels_iou(masks.data_ptr() if masks is not None else None, side,
+                                           maps.data_ptr() if masks is not None else None, anno.data_ptr(),
+                                           off.data_ptr(), obj.data_ptr(), tid.contiguous().data_ptr(), G, H, W,
+                                           float(seg_thr), labels.data_ptr(), thrs.contiguous().data_ptr(), T,
+                                           cnt.data_ptr(), _stream(dev)))
+    return labels, counts
 
 
 def label_boxes(anno: torch.Tensor, queries) -> torch.Tensor:

@@ -11,6 +11,16 @@ one label map, `(argmax_k + 1) * (max_k > seg_thr)` (:480, :504, :521-523).
 as one batch (each stream crops its own video's frame in place), objects join at their start frame (`add`, init boxes
 from `sm_label_boxes`) and leave after their end frame (`remove`), and the label maps of all videos come from one fused
 paste-back + argmax kernel (`sm_paste_labels`): the per-object float frames are never materialised.
+
+With `open(..., score=...)` it also computes the score `track_vos` returns for a video, `MultiBatchIouMeter`
+(tools/test.py:421-456): per object and threshold of `VOS_THRESHOLDS`, the mean over the object's scored frames of the IoU
+between the fused label `== k+1` and the object's annotation.  Scored frames go through `sm_paste_labels_iou`, the same
+kernel pass with (intersection, union) counts per object and threshold; the counts stay on the device until `result`.
+The reference has two branches, both restated as they are:
+  score="whole": no start_frame dict (DAVIS 2016/2017).  The k-th object of a video is scored against annotation id
+                 k+1 (by position, whatever id it was tracked with) on frames 1 .. num_frames-2;
+  score="spans": start_frame / end_frame dicts.  Each object is scored against its own id on frames
+                 start+1 .. end-2 (an empty window gives NaN).
 """
 from __future__ import annotations
 
@@ -20,8 +30,11 @@ import torch
 from . import ops
 from .ops import OBJ_IDLE, OBJ_INIT, OBJ_TRACKED
 from .tracker import BatchTracker, TrackerParams
+from .tune import _check_thresholds
 
 UNBOUNDED = np.iinfo(np.int64).max
+VOS_THRESHOLDS = np.arange(0.3, 0.5, 0.05)         # tools/test.py:30 thrs
+SCORE_MODES = (None, "whole", "spans")
 
 
 def schedule(start, end, f: int) -> np.ndarray:
@@ -34,6 +47,40 @@ def schedule(start, end, f: int) -> np.ndarray:
     return kind
 
 
+def score_windows(objects, num_frames: int, score: str):
+    """MultiBatchIouMeter's scoring plan for objects (video, id, start, end) in open order: target_ids int [n] (the
+    annotation value each object is scored against) and its scored frames [lo, hi) as int arrays [n].
+    "whole": the k-th object of a video (in this order) against id k+1 on [1, num_frames - 1);
+    "spans": each object against its own id on [start + 1, end - 1)."""
+    n, T = len(objects), int(num_frames)
+    if score == "whole":
+        seen = {}
+        ids = []
+        for o in objects:
+            seen[o[0]] = seen.get(o[0], 0) + 1
+            ids.append(seen[o[0]])
+        return np.array(ids, np.int64), np.full(n, 1, np.int64), np.full(n, T - 1, np.int64)
+    if score == "spans":
+        return (np.array([o[1] for o in objects], np.int64), np.array([o[2] + 1 for o in objects], np.int64),
+                np.array([o[3] - 1 for o in objects], np.int64))
+    raise ValueError(f"score must be one of {SCORE_MODES}, got {score!r}")
+
+
+def score_row(counts, lo: int, hi: int) -> np.ndarray:
+    """One object's row of MultiBatchIouMeter from its integer counts int [frames, thrs, 2] (intersection, union):
+    per threshold, np.mean of [intxn / union (float64), or 1 where union == 0] over frames lo .. hi-1, as float32; NaN for
+    an empty window."""
+    c = np.asarray(counts, dtype=np.int64)
+    res = np.full(c.shape[1], np.nan, dtype=np.float32)
+    if hi <= lo:
+        return res
+    inter, union = c[lo:hi, :, 0], c[lo:hi, :, 1]
+    iou = np.where(union > 0, inter / np.maximum(union, 1), 1.0)
+    for t in range(c.shape[1]):
+        res[t] = np.mean(np.ascontiguousarray(iou[:, t]))        # the 1-D reduction order of np.mean(list)
+    return res
+
+
 class VideoSegmenter:
     """track_vos for G videos on one engine.  `net` is a `siammask_b200.Custom` whose max_batch / num_slots cover the
     largest number of objects tracked at once; `params` the tracker hyper-parameters (seg_thr included)."""
@@ -43,12 +90,20 @@ class VideoSegmenter:
         self.p = self.tracker.p
         self.dev = self.tracker.dev
         self.objects: list[tuple[int, int, int, int]] = []
+        self.score = None
 
-    def open(self, objects, num_frames: int | None = None, num_videos: int | None = None):
+    def open(self, objects, num_frames: int | None = None, num_videos: int | None = None, score: str | None = None,
+             thrs=VOS_THRESHOLDS):
         """objects: (video, object_id, start_frame[, end_frame]) per object, in the reference's object order;
         end_frame defaults to the last frame (num_frames - 1, or never when num_frames is None).  Within a video the
         k-th object (in this order) gets label k + 1.  num_videos (default: largest video index + 1) is the G of every
-        later `frame` call.  Resets the frame counter to 0."""
+        later `frame` call.  score: None, "whole" or "spans" (module docstring) scores every video with the reference's
+        MultiBatchIouMeter at the thresholds thrs (1..32 values >= -1); it needs num_frames, and `result()` returns the
+        scores.  Resets the frame counter to 0."""
+        if score not in SCORE_MODES:
+            raise ValueError(f"score must be one of {SCORE_MODES}, got {score!r}")
+        if score is not None and num_frames is None:
+            raise ValueError("scoring needs num_frames (the scored windows end relative to the last frame)")
         last = UNBOUNDED if num_frames is None else int(num_frames) - 1
         objs = []
         for o in objects:
@@ -76,9 +131,31 @@ class VideoSegmenter:
         self._sid: list[int | None] = [None] * len(objs)     # tracker stream of each object (None: not tracked)
         self._offsets = torch.tensor(np.concatenate([[0], np.cumsum(counts)]), dtype=torch.int32, device=self.dev)
         self._table_key, self._table = None, None
+        self.score = score
+        if score is not None:
+            if any(o[3] > last for o in objs):
+                raise ValueError(f"scoring: every end_frame must be <= num_frames - 1 ({last})")
+            self.thrs = _check_thresholds(thrs)
+            target, self._lo, self._hi = score_windows(objs, int(num_frames), score)
+            for g in range(self.G):
+                v = target[[k for k in range(len(objs)) if objs[k][0] == g]]
+                if np.unique(v).size != v.size:
+                    raise ValueError(f"video {g}: scored object ids must be unique within a video")
+            self._target = target
+            self._thrs_dev = torch.as_tensor(self.thrs, device=self.dev)
+            self._tid_key, self._tid = None, None
+            # counts of frame f, entry i (kernel order, self.order[i]) and threshold t: (intersection, union)
+            self._counts = torch.zeros(int(num_frames), len(objs), self.thrs.size, 2, dtype=torch.int32, device=self.dev)
         self.tracker._clear()
         self.f = 0
         return self
+
+    def _target_ids(self, scored) -> torch.Tensor:
+        key = tuple(int(self._target[k]) if scored[k] else -1 for k in self.order)
+        if key != self._tid_key:              # changes only when an object's window opens or closes
+            self._tid_key = key
+            self._tid = torch.tensor(key, dtype=torch.int32, device=self.dev)
+        return self._tid
 
     def _entries(self, kinds, rows) -> torch.Tensor:
         ent = []
@@ -98,7 +175,8 @@ class VideoSegmenter:
     @torch.no_grad()
     def frame(self, frames, annos=None) -> torch.Tensor:
         """Advance every video by one frame.  frames: uint8 [G,H,W,3] (BGR); annos: uint8 [G,H,W] annotation label maps
-        of this frame, needed only when some object starts here.  Returns labels uint8 [G,H,W] on the device."""
+        of this frame, needed when some object starts here or, when scoring, when the frame lies in some object's
+        scored window.  Returns labels uint8 [G,H,W] on the device."""
         f = self.f
         fr = self.tracker._frames(frames)
         if fr.dim() != 4 or fr.shape[0] != self.G:
@@ -106,13 +184,23 @@ class VideoSegmenter:
         G, H, W = int(fr.shape[0]), int(fr.shape[1]), int(fr.shape[2])
         kinds = schedule(self._start, self._end, f)
         starting = [k for k in range(len(self.objects)) if kinds[k] == OBJ_INIT]
+        scored = None
+        if self.score is not None:
+            if f >= self._counts.shape[0]:
+                raise ValueError(f"scoring: at most num_frames ({self._counts.shape[0]}) frames")
+            scored = (self._lo <= f) & (f < self._hi)
+            if scored.any() and annos is None:
+                raise ValueError(f"frame {f} is scored: annotation label maps are required")
+            if not scored.any():
+                scored = None
         anno = None
-        if starting:
+        if starting or scored is not None:
             if annos is None:
                 raise ValueError(f"frame {f}: objects start here, annotation label maps are required")
             anno = torch.as_tensor(annos).to(self.dev).contiguous()
             if anno.dtype != torch.uint8 or tuple(anno.shape) != (G, H, W):
                 raise ValueError(f"annos must be uint8 [{G},{H},{W}]")
+        if starting:
             # init boxes (:494-496): one D2H copy, at init frames only
             boxes = ops.label_boxes(anno, [(self.objects[k][0], self.objects[k][1]) for k in starting]).cpu().numpy()
             missing = [self.objects[k][:2] for k, b in zip(starting, boxes) if b[2] == 0]
@@ -137,7 +225,11 @@ class VideoSegmenter:
             ids = bt.add(fr, xywh, frame_index=[self.objects[k][0] for k in starting])
             for k, sid in zip(starting, ids):
                 self._sid[k] = sid
-        labels = ops._paste_labels(masks, maps, anno, self._offsets, table, (H, W), self.p.seg_thr)
+        if scored is None:
+            labels = ops._paste_labels(masks, maps, anno, self._offsets, table, (H, W), self.p.seg_thr)
+        else:
+            labels, _ = ops._paste_labels_iou(masks, maps, anno, self._offsets, table, self._target_ids(scored), (H, W),
+                                              self.p.seg_thr, self._thrs_dev, counts=self._counts[f])
         self.f += 1
         return labels
 
@@ -152,3 +244,19 @@ class VideoSegmenter:
             if sid is not None:
                 pos[k], sz[k] = s[rows[sid], 0:2], s[rows[sid], 2:4]
         return {"target_pos": pos, "target_sz": sz}
+
+    def result(self) -> list[np.ndarray]:
+        """MultiBatchIouMeter of every video: a list of G float32 arrays [objects of video g, thresholds], the objects in
+        `open` order, from the counts of the frames processed so far.  One D2H copy; the IoU and the means are computed
+        from the integer counts with the reference's float64 arithmetic (`score_row`); NaN for an empty window."""
+        if self.score is None:
+            raise ValueError("open(..., score='whole' | 'spans') first")
+        counts = self._counts.cpu().numpy()
+        entry = {k: i for i, k in enumerate(self.order)}
+        rows = [score_row(counts[:, entry[k]], int(self._lo[k]), min(int(self._hi[k]), self.f))
+                for k in range(len(self.objects))]
+        out = []
+        for g in range(self.G):
+            r = [rows[k] for k in range(len(self.objects)) if self.objects[k][0] == g]
+            out.append(np.stack(r) if r else np.zeros((0, self.thrs.size), np.float32))
+        return out
