@@ -176,6 +176,18 @@ int sm_mask_iou(const float* masks, int32_t side, const double* maps, const uint
 int sm_label_boxes(const uint8_t* anno, int32_t G, int32_t H, int32_t W, const int32_t* queries, int32_t Q, int32_t* boxes,
                    void* stream);
 
+/* Region overlap of the VOT supervised protocol (tools/test.py:341-354): for each of B pairs, overlap[b] (device f32
+ * [B]) = the VOT toolkit's compute_polygon_overlap(poly_a[b], poly_b[b], bounds left 0, top 0, right W, bottom H) as
+ * pyvotkit's vot_overlap calls it (flags 0: the non-legacy rasteriser), bit for bit.  poly_a / poly_b are device f32
+ * [B][8] 4-point polygons x0, y0, .. x3, y3.  The restatement keeps C's types: float for the bounds, the offset into the
+ * union box, pixelY - y[i] and the edge deltas; double for the node x and the a1 / a2 ratio test; no FMA contraction;
+ * round() half away from zero; (int) truncating.  Each mask row is the union of its spans (a pixel covered twice counts
+ * once), and columns up to W inside the union box count.  Both early exits return 0; an empty union returns x86's 0/0
+ * NaN (0xFFC00000), which the protocol treats as "not lost".
+ * Precondition: every coordinate is finite and within +-2^20 px.  Beyond that C's (int) of an out-of-range double is
+ * undefined and x86 and the GPU disagree; the Python wrapper checks it.  (W+1)*(H+1) must fit in int32. */
+int sm_vot_overlap(const float* poly_a, const float* poly_b, int32_t B, int32_t W, int32_t H, float* overlap, void* stream);
+
 /* Score / box post-processing + argmax of siamese_track — tools/test.py:205-254 — on the device, so that
  * sm_track -> sm_select -> sm_refine needs no host round trip.  All pointers are device pointers:
  * cls/loc as returned by sm_track; anchors f32 [A*R*R][4] = (cx,cy,w,h) in generate_anchor order (tools/test.py:113-129);

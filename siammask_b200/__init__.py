@@ -5,14 +5,16 @@ Public surface mirrors the reference's model object for that path:
     conv2d_dw_group                                       (models/rpn.py:32-38)
     VideoSegmenter (multi-object track_vos on the device)  (tools/test.py:459-542)
     ParamSweep (tune_vos's hyper-parameter grid search)    (tools/tune_vos.py)
+    VotRunner (track_vot / tune_vot, VOT supervised protocol) (tools/test.py:318-418, tools/tune_vot.py)
 All compute lives in libsiammask_b200.so (C ABI: include/siammask_b200.h)."""
 from .custom import Custom, DEFAULT_ANCHORS
 from .ops import conv2d_dw_group, xcorr_depthwise, conv2d, crop_resize, warp_affine, paste_labels, label_boxes, \
-    mask_iou, paste_labels_iou
+    mask_iou, paste_labels_iou, vot_overlap
 from .checkpoint import synthetic_state_dict, load_checkpoint, expected_keys
 from .vos import VideoSegmenter, VOS_THRESHOLDS
 from .tune import ParamSweep
+from .vot import VotRunner
 
 __all__ = ["Custom", "DEFAULT_ANCHORS", "conv2d_dw_group", "xcorr_depthwise", "conv2d", "crop_resize", "warp_affine",
            "paste_labels", "label_boxes", "mask_iou", "paste_labels_iou", "VideoSegmenter", "VOS_THRESHOLDS",
-           "ParamSweep", "synthetic_state_dict", "load_checkpoint", "expected_keys"]
+           "ParamSweep", "VotRunner", "vot_overlap", "synthetic_state_dict", "load_checkpoint", "expected_keys"]

@@ -162,6 +162,8 @@ void launch_paste_labels_iou(const float* masks, int side, const double* maps, c
                              cudaStream_t st);
 void launch_label_boxes(const uint8_t* anno, int G, int H, int W, const int32_t* queries, int Q, int32_t* boxes,
                         cudaStream_t st);
+// sm_vot_overlap (include/siammask_b200.h): compute_polygon_overlap of B pairs of 4-point polygons, bounds (0, 0, W, H)
+void launch_vot_overlap(const float* poly_a, const float* poly_b, int B, int W, int H, float* overlap, cudaStream_t st);
 void launch_absmax(const Act& a, float* slot, cudaStream_t st);
 void launch_xcorr_nchw_f32(const float* x, const float* k, float* out, int planes, int H, int W, int kh, int kw,
                            cudaStream_t st);

@@ -2025,6 +2025,15 @@ int sm_label_boxes(const uint8_t* anno, int32_t G, int32_t H, int32_t W, const i
   SM_API_END
 }
 
+int sm_vot_overlap(const float* poly_a, const float* poly_b, int32_t B, int32_t W, int32_t H, float* overlap, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(poly_a && poly_b && overlap && B >= 1 && W > 0 && H > 0, "bad argument");
+  SMK_CHECK(((int64_t)W + 1) * ((int64_t)H + 1) <= INT32_MAX, "frame too large for int32 pixel counts");
+  require_device();
+  smk::launch_vot_overlap(poly_a, poly_b, B, W, H, overlap, static_cast<cudaStream_t>(stream));
+  SM_API_END
+}
+
 int sm_warp_affine(const float* src, int32_t src_h, int32_t src_w, const double* maps, float* dst, int32_t dst_h,
                    int32_t dst_w, float border_value, int32_t B, void* stream) {
   SM_API_BEGIN

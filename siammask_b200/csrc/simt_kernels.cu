@@ -6,6 +6,7 @@
 #include "common.cuh"
 
 #include <algorithm>
+#include <cfloat>
 #include <climits>
 #include <cmath>
 #include <type_traits>
@@ -1295,6 +1296,132 @@ __global__ void __launch_bounds__(LB_THREADS) label_boxes_kernel(const uint8_t* 
   }
 }
 
+// sm_vot_overlap: the VOT toolkit's compute_polygon_overlap (non-legacy rasterisation, bounds (0, 0, W, H)) restated
+// for one pair of 4-point polygons per block.  The arithmetic follows the C types it restates, without contraction:
+//   float:  bounds (min / max, floor / ceil, clipping), the offset p - (x, y) of both polygons into the union box, the
+//           box areas and the bounds_overlap ratio, pixelY - y[i] and the edge deltas y[j] - y[i], x[j] - x[i];
+//   double: the node x = x[i] + (pixelY - y[i]) / dy * dx, and a1 / a2 in the ratio test;
+//   int:    (int) truncates; round() is half away from zero (not rint).
+// Each thread takes rows of the union box.  A row's nodes (at most one per edge) are sorted and paired as the C loop
+// pairs them (a repeated node skips one, spans clip to [0, width-1]); a mask pixel is set once however many spans cover
+// it, so each polygon's row is the union of its spans.  Columns 0..width-1 of the box are counted, which reaches
+// column W when a polygon does.  No mask is materialised: the intersection / union counts are reduced per block.  The
+// result is (float)intersection / (float)union; an empty union gives x86's 0/0, the NaN 0xFFC00000.
+constexpr int VO_THREADS = 128;
+
+struct VotBounds { float left, top, right, bottom; };
+
+__device__ __forceinline__ float c_max(float a, float b) { return a > b ? a : b; }     // MAX / MIN of region.h
+__device__ __forceinline__ float c_min(float a, float b) { return a < b ? a : b; }
+
+__device__ __forceinline__ float c_roundf(float v) {     // C round(): half away from zero; v - trunc(v) is exact
+  const float t = truncf(v);
+  return fabsf(__fsub_rn(v, t)) >= 0.5f ? __fadd_rn(t, copysignf(1.f, v)) : t;
+}
+
+__device__ __forceinline__ VotBounds vot_bounds(const float* p, float W, float H) {
+  float l = FLT_MAX, t = FLT_MAX, r = -FLT_MAX, b = -FLT_MAX;
+  for (int i = 0; i < 4; ++i) {
+    t = c_min(t, p[2 * i + 1]); b = c_max(b, p[2 * i + 1]);
+    l = c_min(l, p[2 * i]);     r = c_max(r, p[2 * i]);
+  }
+  return {c_max(floorf(l), 0.f), c_max(floorf(t), 0.f), c_min(ceilf(r), W), c_min(ceilf(b), H)};
+}
+
+__device__ __forceinline__ float vot_area(const VotBounds& b) {
+  return __fmul_rn(__fsub_rn(b.right, b.left), __fsub_rn(b.bottom, b.top));
+}
+
+// Row pixelY of one rounded polygon (x0, y0, .. x3, y3 in box coordinates) clipped to [0, width): its spans [s, e]
+// merged into disjoint ones; returns their number (<= 2).
+__device__ __forceinline__ int vot_row(const float* poly, int pixelY, int width, int* s, int* e) {
+  int node[4], nodes = 0;
+#pragma unroll
+  for (int i = 0, j = 3; i < 4; j = i++) {
+    const float x[2] = {poly[2 * i], poly[2 * j]}, y[2] = {poly[2 * i + 1], poly[2 * j + 1]};
+    const int yi = (int)y[0], yj = (int)y[1];
+    if ((yi <= pixelY && yj > pixelY) || (yj <= pixelY && yi > pixelY) || (yi < pixelY && yj >= pixelY) ||
+        (yj < pixelY && yi >= pixelY) || (yi == yj && yi == pixelY)) {
+      const double r = (double)__fsub_rn(y[1], y[0]);
+      const double k = (double)__fsub_rn(x[1], x[0]);
+      if (r != 0.0)
+        node[nodes++] = (int)__dadd_rn((double)x[0],
+                                       __dmul_rn(__ddiv_rn((double)__fsub_rn((float)pixelY, y[0]), r), k));
+    }
+  }
+  for (int i = 1; i < nodes; ++i)                        // ascending, as the C bubble sort leaves them
+    for (int j = i; j > 0 && node[j - 1] > node[j]; --j) { const int t = node[j]; node[j] = node[j - 1]; node[j - 1] = t; }
+  int n = 0, i = 0;
+  while (i < nodes - 1) {
+    if (node[i] == node[i + 1]) { ++i; continue; }
+    if (node[i] >= width) break;
+    if (node[i + 1] >= 0) {
+      const int a = max(node[i], 0), b = min(node[i + 1], width - 1);
+      if (n && a <= e[n - 1]) e[n - 1] = max(e[n - 1], b);
+      else { s[n] = a; e[n] = b; ++n; }
+    }
+    i += 2;
+  }
+  return n;
+}
+
+__global__ void __launch_bounds__(VO_THREADS) vot_overlap_kernel(const float* __restrict__ poly_a,
+                                                                 const float* __restrict__ poly_b, int W, int H,
+                                                                 float* __restrict__ overlap) {
+  __shared__ int red[3][VO_THREADS / 32];
+  __shared__ float s_poly[2][8];
+  const int p = blockIdx.x;
+  const float* pa = poly_a + 8 * (size_t)p;
+  const float* pb = poly_b + 8 * (size_t)p;
+  const VotBounds b1 = vot_bounds(pa, (float)W, (float)H), b2 = vot_bounds(pb, (float)W, (float)H);
+  // The two early exits of the C code both return 0 and have no side effect, so they are tested together.  Ratio
+  // test: a1 / a2 or a2 / a1 < 1e-10 (float areas, double quotients).  bounds_overlap(b1, b2) == 0: MAX(0, q) is 0
+  // exactly when q <= 0 (a NaN q goes on to the rasteriser).
+  const double a1 = (double)vot_area(b1), a2 = (double)vot_area(b2);
+  const VotBounds bi = {c_max(b1.left, b2.left), c_max(b1.top, b2.top), c_min(b1.right, b2.right),
+                        c_min(b1.bottom, b2.bottom)};
+  const float inter = vot_area(bi);
+  const float q = __fdiv_rn(inter, __fsub_rn(__fadd_rn(vot_area(b1), vot_area(b2)), inter));
+  const bool empty = __ddiv_rn(a1, a2) < 1e-10 || __ddiv_rn(a2, a1) < 1e-10 || (0.f > q ? 0.f : q) == 0.f;
+  const float x0 = c_min(b1.left, b2.left), y0 = c_min(b1.top, b2.top);
+  const int width = (int)__fsub_rn(c_max(b1.right, b2.right), x0) + 1;
+  const int height = (int)__fsub_rn(c_max(b1.bottom, b2.bottom), y0) + 1;
+  if (empty || width < 1 || height < 1) {
+    if (threadIdx.x == 0) overlap[p] = 0.f;
+    return;
+  }
+  if (threadIdx.x < 16) {                              // offset_polygon(-x, -y), then round_polygon
+    const int k = threadIdx.x & 7;
+    s_poly[threadIdx.x >> 3][k] = c_roundf(__fadd_rn((threadIdx.x < 8 ? pa : pb)[k], (k & 1) ? -y0 : -x0));
+  }
+  __syncthreads();
+  int n_and = 0, n_a = 0, n_b = 0;
+  for (int y = threadIdx.x; y < height; y += VO_THREADS) {
+    int sa[2], ea[2], sb[2], eb[2];
+    const int na = vot_row(s_poly[0], y, width, sa, ea), nb = vot_row(s_poly[1], y, width, sb, eb);
+    for (int i = 0; i < na; ++i) {
+      n_a += ea[i] - sa[i] + 1;
+      for (int j = 0; j < nb; ++j) n_and += max(0, min(ea[i], eb[j]) - max(sa[i], sb[j]) + 1);
+    }
+    for (int j = 0; j < nb; ++j) n_b += eb[j] - sb[j] + 1;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    n_and += __shfl_xor_sync(0xffffffffu, n_and, o);
+    n_a += __shfl_xor_sync(0xffffffffu, n_a, o);
+    n_b += __shfl_xor_sync(0xffffffffu, n_b, o);
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) { red[0][warp] = n_and; red[1][warp] = n_a; red[2][warp] = n_b; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int c = 0, ca = 0, cb = 0;
+    for (int w = 0; w < VO_THREADS / 32; ++w) { c += red[0][w]; ca += red[1][w]; cb += red[2][w]; }
+    const int uni = ca + cb - c;                         // mask_1 + mask_2 + mask_intersect
+    overlap[p] = uni == 0 ? __int_as_float(0xFFC00000) : __fdiv_rn(__int2float_rn(c), __int2float_rn(uni));
+  }
+}
+
 // sm_template_slots: one slot's worth of cached kernel (n8 x 16 bytes per plane) per (block.y = stream)
 __global__ void scatter_slots_kernel(const __half* __restrict__ src_hi, const __half* __restrict__ src_lo,
                                      __half* __restrict__ dst_hi, __half* __restrict__ dst_lo,
@@ -1708,6 +1835,11 @@ void launch_mask_iou(const float* masks, int side, const double* maps, const uin
 void launch_label_boxes(const uint8_t* anno, int G, int H, int W, const int32_t* queries, int Q, int32_t* boxes,
                         cudaStream_t st) {
   label_boxes_kernel<<<Q, LB_THREADS, 0, st>>>(anno, G, H, W, queries, boxes);
+  SMK_CUDA(cudaGetLastError());
+}
+
+void launch_vot_overlap(const float* poly_a, const float* poly_b, int B, int W, int H, float* overlap, cudaStream_t st) {
+  vot_overlap_kernel<<<B, VO_THREADS, 0, st>>>(poly_a, poly_b, W, H, overlap);
   SMK_CUDA(cudaGetLastError());
 }
 

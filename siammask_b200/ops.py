@@ -304,3 +304,44 @@ def _mask_iou(masks, maps, anno, video, thrs) -> torch.Tensor:
         _lib.check(lib.sm_mask_iou(masks.data_ptr(), side, maps.data_ptr(), anno.data_ptr(), video.data_ptr(), B, H, W,
                                    thrs.data_ptr(), T, out.data_ptr(), _stream(dev)))
     return out
+
+
+VOT_COORD_LIMIT = 2.0 ** 20       # |coordinate| bound of sm_vot_overlap's precondition
+
+
+def vot_overlap(poly_a, poly_b, size) -> torch.Tensor:
+    """Region overlap of the VOT supervised protocol (tools/test.py:341-354, C ABI `sm_vot_overlap`): pyvotkit's
+    vot_overlap(poly_a[b], poly_b[b], (W, H)) for B pairs, bit for bit.  poly_a, poly_b: float32 CUDA [B,8] 4-point
+    polygons x0, y0, .. x3, y3; size = (H, W).  Returns float32 [B]; NaN where both rasterised polygons are empty inside
+    the frame (the protocol does not count that as a loss).  The checks read both polygon tensors on the host: shapes,
+    dtype, device, and every coordinate finite and within +-2^20 px."""
+    for name, p in (("poly_a", poly_a), ("poly_b", poly_b)):
+        if not (torch.is_tensor(p) and p.is_cuda and p.dtype == torch.float32 and p.dim() == 2 and p.shape[1] == 8):
+            raise ValueError(f"{name} must be a float32 CUDA tensor [B, 8]")
+    if poly_a.shape != poly_b.shape or poly_a.device != poly_b.device:
+        raise ValueError("poly_a and poly_b must have the same shape and device")
+    H, W = int(size[0]), int(size[1])
+    if H < 1 or W < 1 or (W + 1) * (H + 1) > 2 ** 31 - 1:
+        raise ValueError("size must be (H, W) with H, W >= 1 and (W+1)*(H+1) < 2^31")
+    for name, p in (("poly_a", poly_a), ("poly_b", poly_b)):
+        v = p.cpu().numpy()
+        if not (np.isfinite(v).all() and (np.abs(v) <= VOT_COORD_LIMIT).all()):
+            raise ValueError(f"{name}: coordinates must be finite and within +-2^20 px")
+    if poly_a.shape[0] == 0:
+        return torch.empty(0, dtype=torch.float32, device=poly_a.device)
+    return _vot_overlap(poly_a, poly_b, (H, W))
+
+
+def _vot_overlap(poly_a, poly_b, size, out=None) -> torch.Tensor:
+    """`vot_overlap` without the host-side checks: poly_a, poly_b float32 CUDA [B,8] with B >= 1 inside the
+    precondition.  out (optional): a contiguous float32 CUDA tensor [B] to write into."""
+    lib = _lib.load()
+    dev = poly_a.device
+    poly_a, poly_b = poly_a.contiguous(), poly_b.contiguous()
+    B = int(poly_a.shape[0])
+    if out is None:
+        out = torch.empty(B, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.sm_vot_overlap(poly_a.data_ptr(), poly_b.data_ptr(), B, int(size[1]), int(size[0]),
+                                      out.data_ptr(), _stream(dev)))
+    return out

@@ -20,7 +20,9 @@ rows as one batch through the slot table and the per-stream (penalty_k, window_i
 (`sm_step_slots_hp`, `sm_tracker_update_hp`) and the frame-index table (`sm_crop_resize_indexed`); the tables are
 uploaded only when the set changes.  A stream's hyper-parameters default to the tracker's `TrackerParams`.  Each stream
 reads one frame of the tensor passed to `track`: its frame index, set by `add` (for `init`, stream i reads frame i; a
-single [H,W,3] frame is shared by all streams).
+single [H,W,3] frame is shared by all streams).  `add_state` starts streams from the centre form siamese_init receives
+(target_pos, target_sz), and `reinit` runs siamese_init again for running streams in their own slots (the VOT
+protocol's restart after a failure) without changing the active set; all three template through `_template`.
 
 The arithmetic is pinned by `tests/test_batch_tracker.py` to the reference loop's golden trajectory and to
 single-stream runs of the host restatement in `oracle/ref_loop.py`.
@@ -159,6 +161,43 @@ class BatchTracker:
         self.aux = torch.zeros(N, 4, dtype=torch.float64, device=dev)
         self.maps = torch.zeros(N, 6, dtype=torch.float64, device=dev)
 
+    def _template(self, fr: torch.Tensor, src: list[int], state: torch.Tensor, slots: list[int]) -> torch.Tensor:
+        """The template half of siamese_init (tools/test.py:142-155) for n streams: fr uint8 frames on the device, src
+        [n] the frame of `fr` each stream reads, state f64 [n,4] (target_pos, target_sz) exactly as siamese_init
+        receives them, slots [n] the engine slots to write.  Returns the streams' avg_chans, int32 [n,3]."""
+        n = len(src)
+        H, W = self._hw(fr)
+        src_dev = torch.tensor(src, dtype=torch.int32, device=self.dev)
+        # avg_chans = np.mean(im, axis=(0, 1)); written into a uint8 image it truncates (:146, :89-100).
+        # Sums of < 2^53 integers are exact in float64, so sum / n equals numpy's mean bit for bit.
+        f4 = fr if fr.dim() == 4 else fr.unsqueeze(0)
+        uniq = sorted(set(src))
+        mean = f4[uniq].to(torch.float64).sum(dim=(1, 2)) / float(H * W)
+        where = torch.tensor([uniq.index(i) for i in src], device=self.dev)
+        avg = mean[where].to(torch.uint8).to(torch.int32).contiguous()
+        # template window (:149-155): s_z = round(sqrt(wc_z * hc_z)), crop around target_pos, resize to 127
+        sw, sh = state[:, 2], state[:, 3]
+        wc_z = sw + self.p.context_amount * (sw + sh)
+        hc_z = sh + self.p.context_amount * (sw + sh)
+        s_z = torch.round(torch.sqrt(wc_z * hc_z))                  # half-to-even, like Python's round()
+        c = (s_z + 1) / 2
+        zb = torch.zeros(n, 8, dtype=torch.int32, device=self.dev)
+        zb[:, 0] = torch.round(state[:, 0] - c).to(torch.int32)
+        zb[:, 1] = torch.round(state[:, 1] - c).to(torch.int32)
+        zb[:, 2] = s_z.to(torch.int32)
+        zb[:, 3:6] = avg
+        z = self._crop(fr, src_dev, zb, self.p.exemplar_size)
+        self.net.template(z, slots=torch.tensor(slots, dtype=torch.int32, device=self.dev))
+        return avg
+
+    def _state(self, target_pos, target_sz) -> torch.Tensor:
+        """f64 [n,4] device rows (target_pos, target_sz) from host or device [n,2] arrays, values unchanged."""
+        t = [(v if torch.is_tensor(v) else torch.as_tensor(np.asarray(v, dtype=np.float64))).to(self.dev, torch.float64)
+             for v in (target_pos, target_sz)]
+        if t[0].numel() % 2 or t[0].numel() != t[1].numel():
+            raise ValueError("target_pos and target_sz must both be [n, 2]")
+        return torch.cat([t[0].reshape(-1, 2), t[1].reshape(-1, 2)], 1).contiguous()
+
     # ------------------------------------------------------------------ stream lifecycle
     @torch.no_grad()
     def add(self, frames, boxes_xywh, frame_index=None, hp=None) -> list[int]:
@@ -168,72 +207,93 @@ class BatchTracker:
         frame i); hp: [n,3] per-stream (penalty_k, window_influence, lr) (default: the tracker's `TrackerParams`).
         Returns the new streams' ids."""
         with torch.cuda.device(self.dev):
-            fr = self._frames(frames)
             bx = torch.as_tensor(np.asarray(boxes_xywh, dtype=np.float64)).reshape(-1, 4).to(self.dev)
-            n = bx.shape[0]
-            H, W = self._hw(fr)
-            if self.N and (H, W) != (self.im_h, self.im_w):
-                raise ValueError(f"all streams of a tracker share one frame size ({self.im_h}x{self.im_w})")
-            idx = list(range(n)) if frame_index is None else [int(i) for i in np.asarray(frame_index).reshape(-1)]
-            if len(idx) != n:
-                raise ValueError("one frame index per new stream expected")
-            F = 1 if fr.dim() == 3 else int(fr.shape[0])
-            if fr.dim() == 4 and any(i < 0 or i >= F for i in idx):
-                raise ValueError(f"frame index out of range [0, {F})")
-            if any(i < 0 for i in idx):
-                raise ValueError("frame indices must be >= 0")
-            if hp is None:
-                rows = [(float(self.p.penalty_k), float(self.p.window_influence), float(self.p.lr))] * n
-            else:
-                h = np.asarray(hp.cpu() if torch.is_tensor(hp) else hp, dtype=np.float64)
-                if h.shape != (n, 3):
-                    raise ValueError(f"hp must have shape [{n}, 3] (penalty_k, window_influence, lr), got {h.shape}")
-                if not np.isfinite(h).all():
-                    raise ValueError("hp entries must be finite")
-                rows = [tuple(float(v) for v in r) for r in h]
-            used = set(self._slots)
-            free = [s for s in range(self.slot0, self.net.num_slots) if s not in used][:n]
-            if n == 0:
-                return []
-            if self.N + n > self.net.max_batch or len(free) < n:
-                raise ValueError("more streams than the engine was built for")
-            src = idx if fr.dim() == 4 else [0] * n          # frame each new stream reads in this call
-            src_dev = torch.tensor(src, dtype=torch.int32, device=self.dev)
             # target_pos = box centre, target_sz = (w, h)  (tools/test.py:338-339 / demo.py)
             state = torch.stack([bx[:, 0] + bx[:, 2] / 2, bx[:, 1] + bx[:, 3] / 2, bx[:, 2], bx[:, 3]], 1).contiguous()
-            # avg_chans = np.mean(im, axis=(0, 1)); written into a uint8 image it truncates (:146, :89-100).
-            # Sums of < 2^53 integers are exact in float64, so sum / n equals numpy's mean bit for bit.
-            f4 = fr if fr.dim() == 4 else fr.unsqueeze(0)
-            uniq = sorted(set(src))
-            mean = f4[uniq].to(torch.float64).sum(dim=(1, 2)) / float(H * W)
-            where = torch.tensor([uniq.index(i) for i in src], device=self.dev)
-            avg = mean[where].to(torch.uint8).to(torch.int32).contiguous()
-            # template window (:149-155): s_z = round(sqrt(wc_z * hc_z)), crop around target_pos, resize to 127
-            sw, sh = state[:, 2], state[:, 3]
-            wc_z = sw + self.p.context_amount * (sw + sh)
-            hc_z = sh + self.p.context_amount * (sw + sh)
-            s_z = torch.round(torch.sqrt(wc_z * hc_z))                  # half-to-even, like Python's round()
-            c = (s_z + 1) / 2
-            zb = torch.zeros(n, 8, dtype=torch.int32, device=self.dev)
-            zb[:, 0] = torch.round(state[:, 0] - c).to(torch.int32)
-            zb[:, 1] = torch.round(state[:, 1] - c).to(torch.int32)
-            zb[:, 2] = s_z.to(torch.int32)
-            zb[:, 3:6] = avg
-            z = self._crop(fr, src_dev, zb, self.p.exemplar_size)
-            self.net.template(z, slots=torch.tensor(free, dtype=torch.int32, device=self.dev))
-            ids = list(range(self._next_id, self._next_id + n))
-            self._next_id += n
-            self.im_w, self.im_h = W, H
-            self.state = torch.cat([self.state, state], 0).contiguous()
-            self.avg = torch.cat([self.avg, avg], 0).contiguous()
-            self.imsize = torch.tensor([[W, H]] * (self.N + n), dtype=torch.int32, device=self.dev)
-            self._ids += ids
-            self._slots += free
-            self._fidx += idx
-            self._hp += rows
-            self.N += n
-            self._upload_tables()
+            return self._join(frames, state, frame_index, hp)
+
+    @torch.no_grad()
+    def add_state(self, frames, target_pos, target_sz, frame_index=None, hp=None) -> list[int]:
+        """`add` from the centre form siamese_init receives: target_pos, target_sz float64 [n,2] (host or device).  A
+        box round trip is not exact ((cx - w/2) + w/2 need not be cx in float64) and the tracker amplifies the ulp, so
+        callers that hold centre-form state (the VOT protocol's get_axis_aligned_bbox) start streams here."""
+        with torch.cuda.device(self.dev):
+            return self._join(frames, self._state(target_pos, target_sz), frame_index, hp)
+
+    def _join(self, frames, state: torch.Tensor, frame_index, hp) -> list[int]:
+        fr = self._frames(frames)
+        n = state.shape[0]
+        H, W = self._hw(fr)
+        if self.N and (H, W) != (self.im_h, self.im_w):
+            raise ValueError(f"all streams of a tracker share one frame size ({self.im_h}x{self.im_w})")
+        idx = list(range(n)) if frame_index is None else [int(i) for i in np.asarray(frame_index).reshape(-1)]
+        if len(idx) != n:
+            raise ValueError("one frame index per new stream expected")
+        F = 1 if fr.dim() == 3 else int(fr.shape[0])
+        if fr.dim() == 4 and any(i < 0 or i >= F for i in idx):
+            raise ValueError(f"frame index out of range [0, {F})")
+        if any(i < 0 for i in idx):
+            raise ValueError("frame indices must be >= 0")
+        if hp is None:
+            rows = [(float(self.p.penalty_k), float(self.p.window_influence), float(self.p.lr))] * n
+        else:
+            h = np.asarray(hp.cpu() if torch.is_tensor(hp) else hp, dtype=np.float64)
+            if h.shape != (n, 3):
+                raise ValueError(f"hp must have shape [{n}, 3] (penalty_k, window_influence, lr), got {h.shape}")
+            if not np.isfinite(h).all():
+                raise ValueError("hp entries must be finite")
+            rows = [tuple(float(v) for v in r) for r in h]
+        used = set(self._slots)
+        free = [s for s in range(self.slot0, self.net.num_slots) if s not in used][:n]
+        if n == 0:
+            return []
+        if self.N + n > self.net.max_batch or len(free) < n:
+            raise ValueError("more streams than the engine was built for")
+        src = idx if fr.dim() == 4 else [0] * n          # frame each new stream reads in this call
+        avg = self._template(fr, src, state, free)
+        ids = list(range(self._next_id, self._next_id + n))
+        self._next_id += n
+        self.im_w, self.im_h = W, H
+        self.state = torch.cat([self.state, state], 0).contiguous()
+        self.avg = torch.cat([self.avg, avg], 0).contiguous()
+        self.imsize = torch.tensor([[W, H]] * (self.N + n), dtype=torch.int32, device=self.dev)
+        self._ids += ids
+        self._slots += free
+        self._fidx += idx
+        self._hp += rows
+        self.N += n
+        self._upload_tables()
         return ids
+
+    @torch.no_grad()
+    def reinit(self, ids, frames, target_pos, target_sz) -> None:
+        """siamese_init again for running streams, in their own engine slots: the streams `ids` are templated from
+        `frames` (read like `track` reads them: each stream its own frame index) at target_pos, target_sz float64 [n,2]
+        (host or device), and their state rows are overwritten.  The set of active streams, their rows, slots, frame
+        indices and hyper-parameters stay as they are, so no table is uploaded."""
+        ids = [int(i) for i in np.asarray(ids).reshape(-1)]
+        unknown = set(ids) - set(self._ids)
+        if unknown:
+            raise ValueError(f"unknown stream ids {sorted(unknown)}")
+        if len(set(ids)) != len(ids):
+            raise ValueError("stream ids must be unique")
+        if not ids:
+            return
+        with torch.cuda.device(self.dev):
+            fr = self._frames(frames)
+            if self._hw(fr) != (self.im_h, self.im_w):
+                raise ValueError(f"frames must be {self.im_h}x{self.im_w}")
+            rows = [self._ids.index(i) for i in ids]
+            src = [self._fidx[r] for r in rows] if fr.dim() == 4 else [0] * len(rows)
+            if fr.dim() == 4 and max(src) >= fr.shape[0]:
+                raise ValueError(f"a stream reads frame {max(src)}, but only {fr.shape[0]} frames were given")
+            state = self._state(target_pos, target_sz)
+            if state.shape[0] != len(ids):
+                raise ValueError(f"target_pos and target_sz must be [{len(ids)}, 2]")
+            avg = self._template(fr, src, state, [self._slots[r] for r in rows])
+            r_dev = torch.tensor(rows, dtype=torch.long, device=self.dev)
+            self.state.index_copy_(0, r_dev, state)
+            self.avg.index_copy_(0, r_dev, avg)
 
     @torch.no_grad()
     def remove(self, ids) -> None:
