@@ -164,7 +164,8 @@ class Engine {
     auto it = tscale_.find(name);
     return it == tscale_.end() ? 0 : it->second;
   }
-  void note_tensor(const Act& a, const std::string& name, cudaStream_t st);
+  void note_tensor(const Act& a, const std::string& name, cudaStream_t st, const Act* same_scale_as = nullptr);
+  void note_tensor(const F32T& t, const std::string& name);
   // ---- schedule
   Act alloc_act(Arena& ar, int B, int H, int W, int C);
   F32T alloc_f32(Arena& ar, int B, int H, int W, int C);
@@ -246,11 +247,18 @@ class Engine {
   int* maps_dev_ = nullptr;
   std::map<int, const int*> maps_;
 
-  Act zf_;                             // template feature of the last sm_template (export)
-  bool have_zf_ = false;
-  // state of the last track (Custom.feature / .search / .corr_feature, custom.py:182-184), read by refine / export
+  // every named tensor of the last sm_template (zf, the backbone's layer outputs, each branch's conv_kernel.0 output
+  // as written: slot-cache rows or the pre-scatter buffer), read by export under "zf" / "template:<name>"
+  std::map<std::string, Act> templ_named_;
+  // where note_tensor records the layer outputs of the call being enqueued (null: nowhere)
+  std::map<std::string, Act>* taps_ = nullptr;
+  std::map<std::string, F32T>* taps_f32_ = nullptr;
+  // state of the last track (Custom.feature / .search / .corr_feature, custom.py:182-184), read by refine / export.
+  // The arenas are reset once per call, so every layer output of the last track / refine stays valid until the next.
   struct CallState {
-    std::map<std::string, Act> named[kMaxLanes];   // per lane: p0, p1, p2, search, corr_* of its share of the batch
+    std::map<std::string, Act> named[kMaxLanes];   // per lane: p0..p3, search, corr_* and every layer output of its
+                                                   // share of the batch (refine: crops and split-fp16 conv outputs)
+    std::map<std::string, F32T> named_f32[kMaxLanes];   // per lane: the refine stage's fp32 NHWC tensors
     int split_n = 1;                               // lane l got streams [split_off[l], split_off[l + 1])
     int split_off[kMaxLanes + 1] = {};
     int last_B = 0;
@@ -376,12 +384,13 @@ class Engine {
     return e;
   }
   // enqueue() issues n kernel launches on st.  Nothing happens while measuring (the arena dry runs); when profiling,
-  // the launches are timed as one row (name, category, flops, bytes) — an empty name means no row.
+  // the launches are timed as one row (name, category, flops, bytes).  Every launch has a name, so a profiled call
+  // lists all of its kernels.
   template <typename F>
   void launch(cudaStream_t st, int n, const std::string& name, const char* cat, double flops, double bytes,
               F&& enqueue) {
     if (measuring_) return;
-    const bool row = profiling_ && !name.empty();
+    const bool row = profiling_;
     const size_t idx = prof_.size();
     if (row) {
       prof_.push_back(ProfRec{name, cat, flops, bytes, get_event(), get_event()});
@@ -391,8 +400,6 @@ class Engine {
     if (row) cudaEventRecord(prof_[idx].e1, st);
     launches_ += n;
   }
-  template <typename F>
-  void launch(cudaStream_t st, int n, F&& enqueue) { launch(st, n, std::string(), nullptr, 0, 0, enqueue); }
 };
 
 // ================================================================================================
@@ -737,6 +744,14 @@ void Engine::fold_layer(ConvW& L, const std::map<std::string, const sm_tensor_de
         w_ref[((size_t)t * g.Cin + c) * g.Cout + n] = (float)((double)w[((size_t)n * g.Cin + c) * HW + t] * scale[n]);
 }
 
+namespace {
+// power-of-two exponent that brings a weight column's max |w| to ~2^14 (|e| <= 24, as the standalone conv operator)
+int weight_exp(float amax) {
+  const int e = amax > 0.f ? (int)std::floor(std::log2(16384.0 / (double)amax)) : 0;
+  return std::max(-24, std::min(24, e));
+}
+}  // namespace
+
 // Step 2: tensor-core operands for the layer's current activation scales.  With inputs stored as a * 2^s_in (a2 * 2^s_in2,
 // r * 2^s_res) the accumulator of output channel n is 2^(e_n + s_in) * sum(w a) when
 //   * the first conv's weights are scaled by 2^e_n (per-channel, keeps hi AND lo fp16 parts normal),
@@ -766,11 +781,11 @@ void Engine::quantize_layer(ConvW& L, uint8_t* host) {
     beta2[n] = (float)std::ldexp(L.shift[n] + (L2 ? L2->shift[n] : 0.0), L.s_out);
     alpha[n] = std::ldexp(1.f, L.s_out - L.s_in);
     if (!L.gemm_ok) continue;
-    // per-output-channel power-of-two scaling keeps hi AND lo fp16 parts in the normal range; |e| <= 14, and with a
-    // residual the diag entry 2^(e + s_in - s_res) must itself be a normal fp16
-    int e = 0;
-    if (amax > 0.f) e = (int)std::floor(std::log2(16384.0 / (double)amax));
-    e = std::max(-14, std::min(14, e));
+    // per-output-channel power-of-two scaling keeps hi AND lo fp16 parts in the normal range for max |w| down to
+    // ~2^-24 (a clamp at 14 left the planes of a channel whose weights are all below ~2^-14 subnormal).  With a
+    // residual the diag entry 2^(e + s_in - s_res) must itself be a normal fp16, so there e stays within 14 - d and
+    // a channel of such tiny weights keeps subnormal planes.
+    int e = weight_exp(amax);
     if (L.has_diag) {
       const int d = L.s_in - L.s_res;
       e = std::max(-14 - d, std::min(14 - d, e));
@@ -808,8 +823,7 @@ void Engine::quantize_stem(uint8_t* host) {
   for (int n = 0; n < 64; ++n) {
     float amax = 0.f;
     for (int k = 0; k < 147; ++k) amax = std::max(amax, std::fabs(wref[(size_t)k * 64 + n]));
-    int e = amax > 0.f ? (int)std::floor(std::log2(16384.0 / (double)amax)) : 0;
-    e = std::max(-14, std::min(14, e));
+    const int e = weight_exp(amax);
     sa[n] = std::ldexp(1.f, s_out - e);
     sb[n] = (float)std::ldexp(stem.shift[n], s_out);
     for (int k = 0; k < 147; ++k) {
@@ -978,9 +992,14 @@ void Engine::calibrate(int B, const float* z, const float* x, cudaStream_t st) {
       if (v == 0.f) any_zero = true;
     }
     if (any_inf || (any_zero && iter < 8)) {
-      // out of range somewhere: everything downstream of it is meaningless — move ALL scales and look again
-      const int step = any_inf ? -10 : +10;
-      for (size_t i = 0; i < mx.size(); ++i) set_scale(absmax_names_[i], scale_of(absmax_names_[i]) + step);
+      // out of range somewhere: move the scale of every tensor that overflowed (everything downstream of an overflow
+      // overflows too, so it moves with it) down, and of every tensor that read all zero up, then look again.  Each
+      // tensor moves on its own: one common step cannot fit a network whose tensors span more than fp16's range, and
+      // a tensor pushed below fp16's smallest subnormal by another tensor's step would be left flushed to zero.
+      for (size_t i = 0; i < mx.size(); ++i) {
+        const int step = !(mx[i] <= 65504.f) ? -10 : (mx[i] == 0.f && iter < 8) ? +10 : 0;
+        if (step != 0) set_scale(absmax_names_[i], std::max(-60, std::min(60, scale_of(absmax_names_[i]) + step)));
+      }
       rewire_and_upload();
       continue;
     }
@@ -1095,9 +1114,17 @@ void Engine::conv_into(const Act& in, const ConvW& Lw, Epilogue ep, cudaStream_t
   });
 }
 
-// calibration pass: remember which tensor lives in this buffer and fold its max |value| into the tensor's slot
-void Engine::note_tensor(const Act& a, const std::string& name, cudaStream_t st) {
-  if (!calibrating_ || measuring_) return;
+// A named layer output: recorded for export under `name`; in the calibration pass, remember which tensor lives in this
+// buffer and fold its max |value| into the tensor's slot.  same_scale_as: `a` is a copy of (part of) that tensor
+// (max-pool, crops) and is stored at its scale.
+void Engine::note_tensor(const Act& a, const std::string& name, cudaStream_t st, const Act* same_scale_as) {
+  if (measuring_) return;
+  if (taps_ != nullptr) (*taps_)[name] = a;
+  if (!calibrating_) return;
+  if (same_scale_as != nullptr) {
+    tensor_name_[a.hi] = tensor_name_[same_scale_as->hi];
+    return;
+  }
   tensor_name_[a.hi] = name;
   size_t slot = 0;
   for (; slot < absmax_names_.size(); ++slot)
@@ -1107,6 +1134,11 @@ void Engine::note_tensor(const Act& a, const std::string& name, cudaStream_t st)
     absmax_names_.push_back(name);
   }
   launch_absmax(a, absmax_dev_ + slot, st);
+}
+
+// fp32 NHWC outputs (refine stage): recorded for export; they are unscaled, so calibration does not track them
+void Engine::note_tensor(const F32T& t, const std::string& name) {
+  if (!measuring_ && taps_f32_ != nullptr) (*taps_f32_)[name] = t;
 }
 
 Act Engine::conv(const Act& in, const ConvW& Lw, bool relu, const Act* res, Arena& ar, cudaStream_t st,
@@ -1130,6 +1162,7 @@ F32T Engine::conv_f32(const Act& in, const ConvW& Lw, bool relu, Arena& ar, cuda
   ep.out_mode = OUT_NHWC_F32;
   ep.out_f32 = out.p;
   conv_into(in, Lw, ep, st);
+  note_tensor(out, Lw.conv_key);
   return out;
 }
 
@@ -1149,8 +1182,8 @@ Act Engine::backbone(const float* x, int B, int S, Arena& ar, std::map<std::stri
   const int Sp = (So + 2 - 3) / 2 + 1;
   Act y = alloc_act(ar, B, Sp, Sp, 64);
   y.sexp = p0.sexp;                    // max-pool commutes with a positive scale
-  if (calibrating_) tensor_name_[y.hi] = "stem";
   launch(st, 1, "maxpool", "pool", 0, 4.0 * (p0.numel() + y.numel()), [&] { launch_maxpool3s2(p0, y, st); });
+  note_tensor(y, "maxpool", st, &p0);
   last_end_[p0.hi] = +1;       // stem and pool write front to back
   last_end_[y.hi] = +1;
   if (keep) (*keep)["p0"] = p0;
@@ -1176,8 +1209,8 @@ Act Engine::backbone(const float* x, int B, int S, Arena& ar, std::map<std::stri
   if (xf.W < 20) {   // custom.py:21-24
     Act c = alloc_act(ar, B, xf.H - 8, xf.W - 8, xf.C);
     c.sexp = xf.sexp;
-    if (calibrating_) tensor_name_[c.hi] = tensor_name_[xf.hi];
-    launch(st, 1, [&] { launch_crop_center(xf, 4, c, st); });
+    launch(st, 1, "crop_center", "misc", 0, 4.0 * (xf.numel() + c.numel()), [&] { launch_crop_center(xf, 4, c, st); });
+    note_tensor(c, "crop_center", st, &xf);
     xf = c;
   }
   return xf;
@@ -1198,10 +1231,12 @@ void Engine::do_template(int slot0, int B, const float* z, cudaStream_t st, cons
     total_bytes_ += 2 * n * sizeof(__half);
   }
   templ_arena_.reset();
+  templ_named_.clear();
+  taps_ = &templ_named_;
+  taps_f32_ = nullptr;
   Act zf = backbone(z, B, 127, templ_arena_, nullptr, st);
   SMK_CHECK(zf.H == 7 && zf.W == 7, "template feature must be 7x7");
-  zf_ = zf;
-  have_zf_ = true;
+  templ_named_["zf"] = zf;
   for (int br = 0; br < n_branches_; ++br) {
     const ConvW& ck = L(std::string(kBranch[br]) + "conv_kernel.0");
     Epilogue ep;
@@ -1224,12 +1259,11 @@ void Engine::do_template(int slot0, int B, const float* z, cudaStream_t st, cons
                              slots, B, cfg_.num_slots, (int)kslot, ovf_flag_, st);
       });
     }
-    if (calibrating_) {
-      Act kc;
-      kc.hi = ep.out_hi; kc.lo = ep.out_lo; kc.B = B; kc.H = 5; kc.W = 5; kc.C = 256;
-      note_tensor(kc, ck.conv_key, st);
-    }
+    Act kc;
+    kc.hi = ep.out_hi; kc.lo = ep.out_lo; kc.B = B; kc.H = 5; kc.W = 5; kc.C = 256; kc.sexp = ck.s_out;
+    note_tensor(kc, ck.conv_key, st);
   }
+  taps_ = nullptr;
 }
 
 // Runs body(lane, b0, nbat, stream) for every lane's block [b0, b0 + nbat) of the batch split_batch() divided, last
@@ -1301,6 +1335,9 @@ void Engine::track_lane(Lane& ln, int slot0, int B, const float* x, float* cls, 
   search_arena.reset();
   std::map<std::string, Act>& named = state_.named[ln.id];
   named.clear();
+  state_.named_f32[ln.id].clear();
+  taps_ = &named;
+  taps_f32_ = nullptr;
   Act xf = backbone(x, B, cfg_.search_size, search_arena, &named, st);
   named["search"] = xf;
   const int nb = (want_feats || want_mask_head) ? 3 : 2;
@@ -1339,6 +1376,7 @@ void Engine::track_lane(Lane& ln, int slot0, int B, const float* x, float* cls, 
     }
   }
   for (int br = 1; br < nb; ++br) order_after((concurrent()) ? ln.aux[br - 1] : st, st);
+  taps_ = nullptr;
 }
 
 F32T Engine::small(const F32T& a, const F32T* b, int Ho, const ConvW& Lw, bool relu, float* out_override, Arena& ar,
@@ -1354,6 +1392,7 @@ F32T Engine::small(const F32T& a, const F32T* b, int Ho, const ConvW& Lw, bool r
     launch_small_conv3x3_maps(a.p, b ? b->p : nullptr, a.B, a.H, a.W, Ho, Ho, a.C, Lw.g.Cout, map, map, Lw.w_ref,
                               Lw.beta, relu ? 1 : 0, out.p, st);
   });
+  if (out_override == nullptr) note_tensor(out, Lw.conv_key);
   return out;
 }
 
@@ -1382,6 +1421,8 @@ void Engine::refine_lane(Lane& ln, int B, const int32_t* pos, float* out, cudaSt
   const Act& p1 = named["p1"];
   const Act& p2 = named["p2"];
   const Act& corr = named["corr_mask"];
+  taps_ = &named;
+  taps_f32_ = &state_.named_f32[ln.id];
   // The three v-branches (crop -> conv -> conv on p2 / p1 / p0) depend only on the cached pyramid: they run on
   // auxiliary streams while the main stream walks deconv -> h2 -> post0 -> h1 -> post1 -> h0 -> post2.
   cudaStream_t s2 = concurrent() ? ln.aux[0] : st, s1 = concurrent() ? ln.aux[1] : st,
@@ -1392,31 +1433,31 @@ void Engine::refine_lane(Lane& ln, int B, const int32_t* pos, float* out, cudaSt
   // level 2 branch (15x15)
   Act c2 = alloc_act(ar, B, 15, 15, 512);
   c2.sexp = p2.sexp;
-  if (calibrating_) tensor_name_[c2.hi] = tensor_name_[p2.hi];
   launch(s2, 1, "crop_p2", "refine_misc", 0, 8.0 * c2.numel(), [&] {
     last_end_[c2.hi] = +1;
     launch_refine_crop(p2, pos, R_ - 1, 1, 4, 15, c2, s2);
   });
+  note_tensor(c2, "refine:crop_p2", s2, &p2);
   Act v2a = conv(c2, L(R + "v2.0"), true, nullptr, ar, s2);
   F32T v2b = conv_f32(v2a, L(R + "v2.2"), true, ar, s2);
   // level 1 branch (31x31)
   Act c1 = alloc_act(ar, B, 31, 31, 256);
   c1.sexp = p1.sexp;
-  if (calibrating_) tensor_name_[c1.hi] = tensor_name_[p1.hi];
   launch(s1, 1, "crop_p1", "refine_misc", 0, 8.0 * c1.numel(), [&] {
     last_end_[c1.hi] = +1;
     launch_refine_crop(p1, pos, R_ - 1, 2, 8, 31, c1, s1);
   });
+  note_tensor(c1, "refine:crop_p1", s1, &p1);
   Act v1a = conv(c1, L(R + "v1.0"), true, nullptr, ar, s1);
   F32T v1b = conv_f32(v1a, L(R + "v1.2"), true, ar, s1);
   // level 0 branch (61x61)
   Act c0 = alloc_act(ar, B, 61, 61, 64);
   c0.sexp = p0.sexp;
-  if (calibrating_) tensor_name_[c0.hi] = tensor_name_[p0.hi];
   launch(s0, 1, "crop_p0", "refine_misc", 0, 8.0 * c0.numel(), [&] {
     last_end_[c0.hi] = +1;
     launch_refine_crop(p0, pos, R_ - 1, 4, 16, 61, c0, s0);
   });
+  note_tensor(c0, "refine:crop_p0", s0, &p0);
   F32T v0a = conv_f32(c0, L(R + "v0.0"), true, ar, s0);
   F32T v0b = small(v0a, nullptr, 61, L(R + "v0.2"), true, nullptr, ar, s0);
   // main chain: p3 = corr_feature[:, :, dy, dx]; out = deconv(p3)
@@ -1426,6 +1467,8 @@ void Engine::refine_lane(Lane& ln, int B, const int32_t* pos, float* out, cudaSt
     launch_gather_corr(corr, pos, p3, std::ldexp(1.f, -corr.sexp), st);
     launch_deconv(p3, deconv_w_, deconv_b_, d.p, B, 256, 7200, 32, st);
   });
+  note_tensor(F32T{p3, B, 1, 1, 256}, "refine:p3");
+  note_tensor(d, "refine:deconv");
   F32T h2a = small(d, nullptr, 15, L(R + "h2.0"), true, nullptr, ar, st);
   F32T h2b = small(h2a, nullptr, 15, L(R + "h2.2"), true, nullptr, ar, st);
   order_after(s2, st);
@@ -1438,6 +1481,8 @@ void Engine::refine_lane(Lane& ln, int B, const int32_t* pos, float* out, cudaSt
   F32T h0b = small(h0a, nullptr, 61, L(R + "h0.2"), true, nullptr, ar, st);
   order_after(s0, st);
   small(h0b, &v0b, 127, L(R + "post2"), false, out, ar, st);                // (B,127,127,1) == (B,127*127)
+  taps_ = nullptr;
+  taps_f32_ = nullptr;
 }
 
 int Engine::next_set() {
@@ -1547,7 +1592,9 @@ void Engine::step_lane(Lane& ln, int slot0, int B, const StepIO& io, cudaStream_
   });
   if (io.refine != nullptr) refine_lane(ln, B, io.pos, io.refine, st);
   if (io.mask_col != nullptr)
-    launch(st, 1, [&] { launch_gather_mask_col(io.mask, io.pos, B, 3969, R_, io.mask_col, st); });
+    launch(st, 1, "mask_col", "misc", 0, 8.0 * B * 3969, [&] {
+      launch_gather_mask_col(io.mask, io.pos, B, 3969, R_, io.mask_col, st);
+    });
 }
 
 void Engine::do_step(int slot0, int B, const StepIO& io, cudaStream_t st, const int32_t* slots) {
@@ -1620,24 +1667,55 @@ int Engine::step_host_async(int slot0, int B, const sm_step_io& h, cudaStream_t 
       });
 }
 
+// Any recorded tensor as f32 NCHW, unscaled: "zf" / "template:<name>" from the last template, else the last track /
+// refine's tensor of that name, concatenated over the lanes.
 void Engine::do_export(const char* what, float* out, int64_t* shape4, cudaStream_t st) {
   join_lanes(st);
-  if (std::string(what) == "zf") {
-    SMK_CHECK(have_zf_, "no cached tensor named 'zf'");
-    if (shape4 != nullptr) { shape4[0] = zf_.B; shape4[1] = zf_.C; shape4[2] = zf_.H; shape4[3] = zf_.W; }
-    if (out != nullptr) launch(st, 1, [&] { launch_split_to_f32(zf_, out, st, std::ldexp(1.f, -zf_.sexp)); });
+  const std::string name = what;
+  const std::string missing = "no cached tensor named '" + name + "'";
+  auto put_act = [&](const Act& a, float* dst) {
+    if (dst != nullptr)
+      launch(st, 1, "export", "misc", 0, 8.0 * a.numel(), [&] { launch_split_to_f32(a, dst, st, std::ldexp(1.f, -a.sexp)); });
+  };
+  if (name == "zf" || name.rfind("template:", 0) == 0) {
+    auto it = templ_named_.find(name == "zf" ? name : name.substr(9));
+    SMK_CHECK(it != templ_named_.end(), missing);
+    const Act& a = it->second;
+    if (shape4 != nullptr) { shape4[0] = a.B; shape4[1] = a.C; shape4[2] = a.H; shape4[3] = a.W; }
+    put_act(a, out);
     return;
   }
   int total_B = 0;
   for (int l = 0; l < state_.split_n; ++l) {       // the lanes hold consecutive blocks of streams
     const std::map<std::string, Act>& named = state_.named[l];
-    auto it = named.find(what);
-    SMK_CHECK(it != named.end(), std::string("no cached tensor named '") + what + "'");
-    const Act& a = it->second;
-    if (shape4 != nullptr) { shape4[1] = a.C; shape4[2] = a.H; shape4[3] = a.W; }
-    if (out != nullptr)
-      launch(st, 1, [&] { launch_split_to_f32(a, out + (size_t)total_B * a.C * a.H * a.W, st, std::ldexp(1.f, -a.sexp)); });
-    total_B += a.B;
+    const std::map<std::string, F32T>& named_f32 = state_.named_f32[l];
+    auto it = named.find(name);
+    auto jt = named_f32.find(name);
+    SMK_CHECK(it != named.end() || jt != named_f32.end(), missing);
+    int B, C, H, W;
+    if (it != named.end()) {
+      const Act& a = it->second;
+      B = a.B; C = a.C; H = a.H; W = a.W;
+      put_act(a, out != nullptr ? out + (size_t)total_B * C * H * W : nullptr);
+    } else {
+      // fp32 NHWC: transposed on the host (an introspection path, not worth a kernel)
+      const F32T& t = jt->second;
+      B = t.B; C = t.C; H = t.H; W = t.W;
+      if (out != nullptr) {
+        const size_t n = (size_t)B * H * W * C, hw = (size_t)H * W;
+        std::vector<float> nhwc(n), nchw(n);
+        SMK_CUDA(cudaMemcpyAsync(nhwc.data(), t.p, n * sizeof(float), cudaMemcpyDeviceToHost, st));
+        SMK_CUDA(cudaStreamSynchronize(st));
+        for (size_t b = 0; b < (size_t)B; ++b)
+          for (size_t p = 0; p < hw; ++p)
+            for (size_t c = 0; c < (size_t)C; ++c) nchw[(b * C + c) * hw + p] = nhwc[(b * hw + p) * C + c];
+        SMK_CUDA(cudaMemcpyAsync(out + (size_t)total_B * C * hw, nchw.data(), n * sizeof(float), cudaMemcpyHostToDevice,
+                                 st));
+        SMK_CUDA(cudaStreamSynchronize(st));
+      }
+    }
+    if (shape4 != nullptr) { shape4[1] = C; shape4[2] = H; shape4[3] = W; }
+    total_B += B;
   }
   if (shape4 != nullptr) shape4[0] = total_B;
 }
@@ -1689,8 +1767,7 @@ static void conv2d_op(const float* x, const float* w, const float* scale, const 
     beta[n] = hb[n];
     alpha[n] = 1.f;
     if (use_gemm) {
-      int e = amax > 0.f ? (int)std::floor(std::log2(16384.0 / (double)amax)) : 0;
-      e = std::max(-24, std::min(24, e));
+      const int e = weight_exp(amax);
       alpha[n] = std::ldexp(1.f, -e);
       for (int c = 0; c < Cin; ++c)
         for (int t = 0; t < HW; ++t) {

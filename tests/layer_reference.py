@@ -1,0 +1,336 @@
+"""Float64 restatement of the engine's layers, one op at a time, with a per-element error bound.  TEST SUPPORT ONLY.
+
+Three parts:
+
+* `wiring(...)`: for every tensor the engine records under a name (`Custom.export`), the op that produced it, the
+  names of the tensors that feed it (the block input as residual or as the fused downsample input included) and the
+  checkpoint keys and geometry.  Built by walking `oracle.siammask_oracle._LAYERS` the way `Oracle.features` /
+  `Oracle.refine` do, not from the engine's layer table.
+* `run(tap, inputs)`: the op in float64 on the CPU, returning `(ref, scale)`, where `scale` is the same op on absolute
+  values (sum |x||w| + |shift| + |residual|).  It restates what the layer computes, not the kernel's arithmetic: BN is
+  folded in float64 as the engine's `fold_affine` does, nothing is rounded.
+* `ratio(got, ref, scale, gamma, rho, tau)`: the gate |got - ref| <= gamma * scale + rho * |ref| + tau per element.
+  gamma covers operand quantisation and accumulation, rho the output's storage format, tau the fp16 subnormal floor.
+  Because the bound is per element and scaled by that element's own terms, a low-magnitude channel, a ragged tile or
+  one stream's rows in a shared tile count as much as the tensor's maximum.
+
+The mutation helpers (`round_sig`, `drop_k_block`, ...) build what a plausible kernel defect would produce from the
+same inputs; the GPU tests assert that each layer's gate rejects them.
+"""
+from __future__ import annotations
+
+from dataclasses import dataclass, field
+
+import numpy as np
+import torch
+import torch.nn.functional as F
+
+from oracle.siammask_oracle import BN_EPS, _LAYERS, nearest_upsample_index
+
+BRANCHES = ("rpn_model.cls.", "rpn_model.loc.", "mask_model.mask.")
+CORR = {"rpn_model.cls.": "corr_cls", "rpn_model.loc.": "corr_loc", "mask_model.mask.": "corr_mask"}
+SEARCH_CAT = "heads.conv_search_cat"
+HEAD_OUT = {"rpn_model.cls.": "cls", "rpn_model.loc.": "loc", "mask_model.mask.": "mask"}
+
+
+@dataclass
+class Tap:
+    """One recorded tensor.  `inputs` name the tensors it reads ('x' / 'z': the API input; 'pos': refine positions)."""
+    name: str
+    op: str                      # conv | maxpool | crop_center | refine_crop | gather | deconv | small | xcorr
+    inputs: tuple
+    keys: tuple = ()             # conv: ((conv_key, bn_key or None), ...) concatenated along Cout
+    stride: int = 1
+    pad: int = 0
+    dil: int = 1
+    relu: bool = False
+    second: tuple | None = None  # fused second conv: (conv_key, bn_key, stride, pad, dil), input = inputs[1]
+    residual: bool = False       # inputs[-1] is added before the ReLU
+    c_off: int = 0               # xcorr: channel offset into the (concatenated) search-side conv output
+    geom: dict = field(default_factory=dict)   # crops / small convs: sizes
+
+
+def fold(sd, conv_key, bn_key):
+    """Folded weight (OIHW) and shift in float64: y = conv(x, w) + shift (engine.cu fold_affine)."""
+    w = sd[conv_key + ".weight"].double()
+    if bn_key is None:
+        return w, sd[conv_key + ".bias"].double()
+    eps = float(np.float32(BN_EPS))
+    scale = sd[bn_key + ".weight"].double() / torch.sqrt(sd[bn_key + ".running_var"].double() + eps)
+    shift = sd[bn_key + ".bias"].double() - sd[bn_key + ".running_mean"].double() * scale
+    return w * scale.view(-1, 1, 1, 1), shift
+
+
+# ---------------------------------------------------------------------------------------------------- wiring table
+def backbone_taps(search: bool, backend: str = "tensor"):
+    """ResNet.forward + ResDownS (Oracle.features / resdown).  Returns (taps, name of the backbone output)."""
+    P = "features.features."
+    taps = [Tap("stem", "conv", ("x" if search else "z",), ((P + "conv1", P + "bn1"),), 2, 0, 1, True),
+            Tap("maxpool", "maxpool", ("stem",))]
+    y = "maxpool"
+    for name, planes, blocks, stride, dilation in _LAYERS:
+        for i in range(blocks):
+            p = f"{P}{name}.{i}."
+            if i == 0:                                   # Oracle.features: the first block's dilation and downsample
+                if stride == 1 and dilation == 1:
+                    ds, d0 = (1, 1, 0), 1
+                elif dilation > 1:
+                    ds, d0 = (3, stride, dilation // 2), dilation // 2
+                else:
+                    ds, d0 = (3, stride, 0), 1
+                s, d = stride, d0
+            else:
+                ds, s, d = None, 1, dilation
+            pad = d if d > 1 else 2 - s                   # Oracle._bottleneck
+            taps.append(Tap(p + "conv1", "conv", (y,), ((p + "conv1", p + "bn1"),), 1, 0, 1, True))
+            taps.append(Tap(p + "conv2", "conv", (p + "conv1",), ((p + "conv2", p + "bn2"),), s, pad, d, True))
+            c3 = ((p + "conv3", p + "bn3"),)
+            if ds is None:
+                taps.append(Tap(p + "conv3", "conv", (p + "conv2", y), c3, relu=True, residual=True))
+            elif backend == "tensor":                    # conv3 and the downsample branch in one GEMM
+                taps.append(Tap(p + "conv3", "conv", (p + "conv2", y), c3, relu=True,
+                                second=(p + "downsample.0", p + "downsample.1", ds[1], ds[2], 1)))
+            else:
+                taps.append(Tap(p + "downsample.0", "conv", (y,), ((p + "downsample.0", p + "downsample.1"),),
+                                ds[1], ds[2], 1, False))
+                taps.append(Tap(p + "conv3", "conv", (p + "conv2", p + "downsample.0"), c3, relu=True, residual=True))
+            y = p + "conv3"
+    D = "features.downsample.downsample."
+    taps.append(Tap(D + "0", "conv", (y,), ((D + "0", D + "1"),)))
+    out = D + "0"
+    if not search:                                       # ResDownS: x[:, :, 4:-4, 4:-4] when W < 20
+        taps.append(Tap("crop_center", "crop_center", (out,)))
+        out = "crop_center"
+    return taps, out
+
+
+def template_taps(backend="tensor", with_mask=True):
+    """Template side, names without the 'template:' prefix."""
+    taps, zf = backbone_taps(False, backend)
+    for br in BRANCHES[:3 if with_mask else 2]:
+        taps.append(Tap(br + "conv_kernel.0", "conv", (zf,), ((br + "conv_kernel.0", br + "conv_kernel.1"),),
+                        relu=True))
+    return taps
+
+
+def search_taps(anchor_num=5, backend="tensor", with_mask=True, mask_head=True):
+    """Search side of track / track_mask (all branches the engine runs when the mask features are requested)."""
+    taps, xf = backbone_taps(True, backend)
+    branches = BRANCHES[:3 if with_mask else 2]
+    cat = backend == "tensor"
+    if cat:
+        taps.append(Tap(SEARCH_CAT, "conv", (xf,), tuple((b + "conv_search.0", b + "conv_search.1") for b in branches),
+                        relu=True))
+    for i, br in enumerate(branches):
+        cs = SEARCH_CAT if cat else br + "conv_search.0"
+        if not cat:
+            taps.append(Tap(cs, "conv", (xf,), ((br + "conv_search.0", br + "conv_search.1"),), relu=True))
+        taps.append(Tap(CORR[br], "xcorr", (cs, "template:" + br + "conv_kernel.0"), c_off=256 * i if cat else 0))
+        if br == "mask_model.mask." and not mask_head:
+            continue
+        taps.append(Tap(br + "head.0", "conv", (CORR[br],), ((br + "head.0", br + "head.1"),), relu=True))
+        taps.append(Tap(HEAD_OUT[br], "conv", (br + "head.0",), ((br + "head.3", None),)))
+    return taps
+
+
+def refine_taps():
+    """Refine.forward(test=True) as Oracle.refine restates it; 'post2' is the API output of track_refine."""
+    R = "refine_model."
+    src = {"p0": "features.features.conv1", "p1": "features.features.layer1.2.conv3",
+           "p2": "features.features.layer2.3.conv3"}
+    taps = []
+    for lvl, (scale, pad, size) in {"p0": (4, 16, 61), "p1": (2, 8, 31), "p2": (1, 4, 15)}.items():
+        taps.append(Tap("refine:crop_" + lvl, "refine_crop", (src[lvl] if lvl != "p0" else "stem", "pos"),
+                        geom=dict(scale=scale, pad=pad, size=size)))
+    taps.append(Tap("refine:p3", "gather", ("corr_mask", "pos")))
+    taps.append(Tap("refine:deconv", "deconv", ("refine:p3",)))
+
+    def c3(name, inp, relu=True, other=None, out=None):
+        ins = (inp,) if other is None else (inp, other)
+        taps.append(Tap(R + name if out is None else out, "small", ins, ((R + name, None),), 1, 1, 1, relu,
+                        geom=dict(up=0)))
+    c3("v2.0", "refine:crop_p2"); c3("v2.2", R + "v2.0")
+    c3("v1.0", "refine:crop_p1"); c3("v1.2", R + "v1.0")
+    c3("v0.0", "refine:crop_p0"); c3("v0.2", R + "v0.0")
+    c3("h2.0", "refine:deconv"); c3("h2.2", R + "h2.0")
+    c3("post0", R + "h2.2", False, R + "v2.2")
+    taps[-1].geom = dict(up=31)
+    c3("h1.0", R + "post0"); c3("h1.2", R + "h1.0")
+    c3("post1", R + "h1.2", False, R + "v1.2")
+    taps[-1].geom = dict(up=61)
+    c3("h0.0", R + "post1"); c3("h0.2", R + "h0.0")
+    c3("post2", R + "h0.2", False, R + "v0.2", out="refine")
+    taps[-1].geom = dict(up=127)
+    return taps
+
+
+# ---------------------------------------------------------------------------------------------------- the ops
+def _conv_terms(sd, tap, x, x2=None, res=None, w_mut=None, w2_mut=None):
+    """(ref, scale) of conv [+ second conv] + shift [+ residual], before the ReLU.  w_mut(w) mutates the weights of the
+    first conv, w2_mut those of the fused second conv."""
+    ws, shifts = zip(*(fold(sd, c, b) for c, b in tap.keys))
+    w, shift = torch.cat(ws, 0), torch.cat(shifts, 0)
+    if w_mut is not None:
+        w = w_mut(w)
+    ref = F.conv2d(x, w, None, tap.stride, tap.pad, tap.dil)
+    scale = F.conv2d(x.abs(), w.abs(), None, tap.stride, tap.pad, tap.dil)
+    if tap.second is not None:
+        c, b, s, p, d = tap.second
+        w2, sh2 = fold(sd, c, b)
+        if w2_mut is not None:
+            w2 = w2_mut(w2)
+        ref = ref + F.conv2d(x2, w2, None, s, p, d)
+        scale = scale + F.conv2d(x2.abs(), w2.abs(), None, s, p, d)
+        shift = shift + sh2
+    ref = ref + shift.view(1, -1, 1, 1)
+    scale = scale + shift.abs().view(1, -1, 1, 1)
+    if res is not None:
+        ref = ref + res
+        scale = scale + res.abs()
+    return ref, scale
+
+
+def refine_crop(f, pos, scale, pad, size):
+    """pad(f, pad)[:, :, scale*dy : scale*dy + size, scale*dx : ...] per stream (Oracle.refine, custom.py:133-135)."""
+    out = []
+    for b in range(f.shape[0]):
+        dy, dx = int(pos[b][0]), int(pos[b][1])
+        out.append(F.pad(f[b:b + 1], [pad] * 4)[:, :, scale * dy:scale * dy + size, scale * dx:scale * dx + size])
+    return torch.cat(out, 0)
+
+
+def nearest_up(t, size):
+    """F.interpolate(size=(size, size)) through the oracle's index table."""
+    idx = torch.from_numpy(nearest_upsample_index(size, t.shape[-1]))
+    return t[:, :, idx][:, :, :, idx]
+
+
+def xcorr(x, k):
+    """Depthwise valid cross-correlation (conv2d_dw_group, rpn.py:32-38), paired batch."""
+    b, c = k.shape[:2]
+    out = F.conv2d(x.reshape(1, b * c, *x.shape[2:]), k.reshape(b * c, 1, *k.shape[2:]), groups=b * c)
+    return out.view(b, c, *out.shape[2:])
+
+
+def run(sd, tap, ins, w_mut=None, k_mut=None, w2_mut=None):
+    """Float64 reference of one tap: (ref, scale) with the op's own output nonlinearity applied to ref.
+    ins: name -> tensor (float64 NCHW; 'pos': int array [B,2]).  Exact ops return scale None."""
+    a = [ins[n] for n in tap.inputs]
+    if tap.op == "conv":
+        x2 = a[1] if tap.second is not None else None
+        res = a[-1] if tap.residual else None
+        ref, scale = _conv_terms(sd, tap, a[0], x2, res, w_mut, w2_mut)
+    elif tap.op == "small":
+        # conv3x3(nearest_up(a (+ b))) + bias: the add happens in fp32 before the conv, so scale takes |a| + |b|
+        x = a[0] if len(a) == 1 else a[0] + a[1]
+        xs = a[0].abs() if len(a) == 1 else a[0].abs() + a[1].abs()
+        if tap.geom.get("up"):
+            x, xs = nearest_up(x, tap.geom["up"]), nearest_up(xs, tap.geom["up"])
+        ref, _ = _conv_terms(sd, tap, x, w_mut=w_mut)
+        _, scale = _conv_terms(sd, tap, xs, w_mut=w_mut)
+    elif tap.op == "deconv":
+        w = sd["refine_model.deconv.weight"].double()
+        b = sd["refine_model.deconv.bias"].double()
+        if w_mut is not None:
+            w = w_mut(w)
+        p3 = a[0].reshape(-1, 256, 1, 1)
+        ref = F.conv_transpose2d(p3, w, b, 15)
+        scale = F.conv_transpose2d(p3.abs(), w.abs(), b.abs(), 15)
+    elif tap.op == "xcorr":
+        x = a[0][:, tap.c_off:tap.c_off + 256]
+        k = a[1] if k_mut is None else k_mut(a[1])
+        if w_mut is not None:
+            x = w_mut(x)
+        ref, scale = xcorr(x, k), xcorr(x.abs(), k.abs())
+        return ref, scale
+    elif tap.op == "maxpool":
+        return F.max_pool2d(a[0], 3, 2, 1), None
+    elif tap.op == "crop_center":
+        return a[0][:, :, 4:-4, 4:-4], None
+    elif tap.op == "refine_crop":
+        return refine_crop(a[0], a[1], **tap.geom), None
+    elif tap.op == "gather":
+        pos = a[1]
+        return torch.stack([a[0][b, :, int(pos[b][0]), int(pos[b][1])] for b in range(a[0].shape[0])])\
+            .reshape(-1, 256, 1, 1), None
+    else:
+        raise ValueError(tap.op)
+    if tap.relu:
+        ref = ref.relu()
+    return ref, scale
+
+
+# ---------------------------------------------------------------------------------------------------- the gate
+# refine convs the engine runs on the fp32 small_conv3x3 kernels (Cin not a multiple of 64; upsample maps, two operands)
+SMALL_SIMT = {"refine_model." + k for k in ("v0.2", "h2.0", "h2.2", "h1.0", "h1.2", "h0.0", "h0.2", "post0", "post1")} | {
+    "refine"}
+F32_OUT = SMALL_SIMT | {"refine_model.v2.2", "refine_model.v1.2", "refine_model.v0.0", "refine:deconv", "refine:p3",
+                        "cls", "loc", "mask"}
+
+
+def family(tap, backend="tensor"):
+    """Which kernel family computes the tap: 'gemm' (tensor-core conv, patch conv, stem), 'simt' (fp32 CUDA-core convs,
+    deconv), 'xcorr', or 'exact' (copies: must match bit for bit)."""
+    if tap.op in ("maxpool", "crop_center", "refine_crop", "gather"):
+        return "exact"
+    if tap.op == "xcorr":
+        return "xcorr"
+    if tap.op == "deconv" or backend != "tensor" or tap.name in SMALL_SIMT:
+        return "simt"
+    return "gemm"
+
+
+def out_format(tap, precision):
+    """Storage of the tap's output: 'f32', 'split' (exact mode hi + lo) or 'hi' (fast mode, fp16 only)."""
+    if tap.name in F32_OUT:
+        return "f32"
+    return "split" if precision == "exact" else "hi"
+
+
+def evaluate(sd, tap, fetch, **mut):
+    """run() with the tap's inputs taken from fetch(name) (float64 NCHW) and 'pos' from fetch('pos')."""
+    return run(sd, tap, {n: fetch(n) for n in tap.inputs}, **mut)
+
+
+def ratio(got, ref, scale, gamma, rho, tau):
+    """(measured gamma, gate use): the worst (|got - ref| - rho|ref| - tau) / scale over the elements, i.e. the error
+    left for the gamma term in units of each element's own scale, and that number over gamma.  The gate holds when the
+    gate use is <= 1."""
+    got, ref = got.double().reshape(ref.shape), ref.double()
+    excess = ((got - ref).abs() - rho * ref.abs() - tau) / scale.clamp_min(1e-300)
+    worst = float(excess.max())
+    return worst, worst / gamma
+
+
+def tau_for(peak, fmt, calibrated):
+    """Subnormal floor of the output's storage: fp16 planes hold value * 2^s, so one fp16 subnormal step is 2^-24 * 2^-s.
+    Uncalibrated, s = 0.  After calibrate() every tensor's stored maximum lies in [2^8, 2^12], so 2^-s <= peak / 2^8,
+    where peak is the tensor's max |value| over everything that shares its scale (template and search side of a
+    backbone layer).  fp32 outputs: none."""
+    if fmt == "f32":
+        return 1e-30
+    return 2.0 ** -24 * (peak / 256.0 if calibrated else 1.0)
+
+
+# ---------------------------------------------------------------------------------------------------- mutations
+def round_sig(t, bits=11):
+    """Round the significand to `bits` significant bits, round-to-nearest-even, no exponent range (nothing is flushed):
+    what dropping the lo plane of a hi+lo pair leaves.  The error is at most 2^-bits relative."""
+    t = t.double()
+    m, e = torch.frexp(t)                       # t = m * 2^e, 0.5 <= |m| < 1
+    return torch.ldexp(torch.round(torch.ldexp(m, torch.full_like(e, bits))), e - bits)
+
+
+def drop_k_block(w, tap_yx=(0, 0), c0=0, width=64):
+    """Weights (OIHW) with one `width`-channel k-block of one kernel tap missing: a skipped K tile."""
+    w = w.clone()
+    ky, kx = min(tap_yx[0], w.shape[2] - 1), min(tap_yx[1], w.shape[3] - 1)
+    w[:, c0:c0 + width, ky, kx] = 0
+    return w
+
+
+def drop_xcorr_tap(k, u=2, v=2):
+    """Template kernel with one of its 5 x 5 taps missing."""
+    k = k.clone()
+    k[:, :, u, v] = 0
+    return k
