@@ -114,11 +114,32 @@ int sm_crop_resize(const uint8_t* frames, size_t frame_stride, int32_t H, int32_
 int sm_crop_resize_indexed(const uint8_t* frames, size_t frame_stride, int32_t H, int32_t W, const int32_t* frame_idx,
                            const int32_t* boxes, int32_t B, int32_t model_size, float* out, void* stream);
 
+/* Images of different sizes in one packed buffer (the *_ragged / *_sized entry points below): the images are
+ * concatenated into one contiguous device buffer, and a device table of sm_image_desc locates each.  offset counts
+ * elements of the buffer's type from the buffer's start: a uint8 HWC/BGR frame is h*w*3 bytes, an annotation or label
+ * map h*w bytes, a pasted mask h*w floats.  An entry with h == 0 or w == 0 is an empty image (nothing reads it). */
+typedef struct sm_image_desc {
+  int64_t offset;
+  int32_t h, w;
+} sm_image_desc;
+
+/* sm_crop_resize_indexed over frames of different sizes: stream b crops the frame frame_desc[frame_idx[b]] (base
+ * frames + offset, h rows, w columns) of the packed uint8 buffer `frames`.  Arithmetic and output as sm_crop_resize.
+ * frame_desc, frame_idx (device int32 [B]) and boxes are device tables; B == 0 is a no-op. */
+int sm_crop_resize_ragged(const uint8_t* frames, const sm_image_desc* frame_desc, const int32_t* frame_idx,
+                          const int32_t* boxes, int32_t B, int32_t model_size, float* out, void* stream);
+
 /* Mask paste-back — crop_back() in siamese_track, tools/test.py:263-282: cv2.warpAffine(src f32 [B][src_h][src_w],
  * maps f64 [B][6] (forward 2x3 maps, device), (dst_w, dst_h), INTER_LINEAR, BORDER_CONSTANT, border_value), bit-exact
  * with OpenCV's fixed-point coordinate generation.  dst f32 [B][dst_h][dst_w].  All device pointers. */
 int sm_warp_affine(const float* src, int32_t src_h, int32_t src_w, const double* maps, float* dst, int32_t dst_h,
                    int32_t dst_w, float border_value, int32_t B, void* stream);
+
+/* sm_warp_affine for B square side x side sources into destinations of different sizes: image b is written at
+ * dst + dst_desc[b].offset, dst_desc[b].h x dst_desc[b].w floats (device table).  max_h / max_w bound every h / w
+ * (they size the grid).  Each image equals sm_warp_affine's output for its own size, bit for bit. */
+int sm_warp_affine_ragged(const float* src, int32_t side, const double* maps, float* dst, const sm_image_desc* dst_desc,
+                          int32_t B, int32_t max_h, int32_t max_w, float border_value, void* stream);
 
 /* Multi-object label map of track_vos — tools/test.py:480-523 — fused with the paste-back, for G videos of one frame
  * size H x W.  The objects of video g are entries obj_offsets[g] .. obj_offsets[g+1]-1 (device int32 [G+1]) of objects
@@ -176,6 +197,20 @@ int sm_mask_iou(const float* masks, int32_t side, const double* maps, const uint
 int sm_label_boxes(const uint8_t* anno, int32_t G, int32_t H, int32_t W, const int32_t* queries, int32_t Q, int32_t* boxes,
                    void* stream);
 
+/* sm_paste_labels / sm_paste_labels_iou / sm_label_boxes for G videos of different sizes: video g's annotation is read
+ * from, and its labels are written to, anno / labels + video_desc[g].offset (h x w bytes; video_desc is a device
+ * table of G entries).  max_h / max_w bound every h / w (they size the grid).  Each video's labels, counts and boxes
+ * equal those of the uniform entry point run on that video alone, bit for bit.  G == 0 / Q == 0 is a no-op. */
+int sm_paste_labels_ragged(const float* masks, int32_t side, const double* maps, const uint8_t* anno,
+                           const int32_t* obj_offsets, const int32_t* objects, const sm_image_desc* video_desc, int32_t G,
+                           int32_t max_h, int32_t max_w, double seg_thr, uint8_t* labels, void* stream);
+int sm_paste_labels_iou_ragged(const float* masks, int32_t side, const double* maps, const uint8_t* anno,
+                               const int32_t* obj_offsets, const int32_t* objects, const int32_t* target_ids,
+                               const sm_image_desc* video_desc, int32_t G, int32_t max_h, int32_t max_w, double seg_thr,
+                               uint8_t* labels, const double* thrs, int32_t T, int32_t* counts, void* stream);
+int sm_label_boxes_ragged(const uint8_t* anno, const sm_image_desc* video_desc, int32_t G, const int32_t* queries,
+                          int32_t Q, int32_t* boxes, void* stream);
+
 /* Region overlap of the VOT supervised protocol (tools/test.py:341-354): for each of B pairs, overlap[b] (device f32
  * [B]) = the VOT toolkit's compute_polygon_overlap(poly_a[b], poly_b[b], bounds left 0, top 0, right W, bottom H) as
  * pyvotkit's vot_overlap calls it (flags 0: the non-legacy rasteriser), bit for bit.  poly_a / poly_b are device f32
@@ -187,6 +222,11 @@ int sm_label_boxes(const uint8_t* anno, int32_t G, int32_t H, int32_t W, const i
  * Precondition: every coordinate is finite and within +-2^20 px.  Beyond that C's (int) of an out-of-range double is
  * undefined and x86 and the GPU disagree; the Python wrapper checks it.  (W+1)*(H+1) must fit in int32. */
 int sm_vot_overlap(const float* poly_a, const float* poly_b, int32_t B, int32_t W, int32_t H, float* overlap, void* stream);
+
+/* sm_vot_overlap with per-pair bounds: pair b uses (W, H) = wh[b] (device int32 [B][2]), same types and rounding.
+ * Each (W+1)*(H+1) must fit in int32 and W, H >= 1 (not checked on the device; the Python wrapper checks them). */
+int sm_vot_overlap_sized(const float* poly_a, const float* poly_b, int32_t B, const int32_t* wh, float* overlap,
+                         void* stream);
 
 /* Score / box post-processing + argmax of siamese_track — tools/test.py:205-254 — on the device, so that
  * sm_track -> sm_select -> sm_refine needs no host round trip.  All pointers are device pointers:

@@ -84,6 +84,16 @@ SIGNATURES = {
                             [C.c_double, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "sm_label_boxes": (C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "sm_vot_overlap": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_void_p]),
+    "sm_vot_overlap_sized": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sm_crop_resize_ragged": (C.c_int, [C.c_void_p] * 4 + [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "sm_warp_affine_ragged": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 3 + [C.c_int32] * 3 +
+                              [C.c_float, C.c_void_p]),
+    "sm_paste_labels_ragged": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 5 + [C.c_int32] * 3 +
+                               [C.c_double, C.c_void_p, C.c_void_p]),
+    "sm_paste_labels_iou_ragged": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 6 + [C.c_int32] * 3 +
+                                   [C.c_double, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "sm_label_boxes_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                        C.c_void_p]),
     "sm_step_host_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(SmStepIO), C.c_void_p,
                                      C.POINTER(C.c_int32)]),
     "sm_xcorr_depthwise": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int32] * 6 + [C.c_void_p]),

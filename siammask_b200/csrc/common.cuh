@@ -9,6 +9,8 @@
 #include <string>
 #include <vector>
 
+struct sm_image_desc;      // include/siammask_b200.h: one image of a packed buffer (offset, h, w)
+
 namespace smk {
 
 // NHWC activation.  Exact precision mode keeps every activation as two fp16 planes,
@@ -152,18 +154,22 @@ void launch_xcorr_nhwc(const Act& x, int c_off, const __half* k_hi, const __half
 // sm_template_slots: src [B][n] split planes -> dst + slots[b] * n (guarded like launch_xcorr_nhwc)
 void launch_scatter_slots(const __half* src_hi, const __half* src_lo, __half* dst_hi, __half* dst_lo,
                           const int32_t* slots, int B, int num_slots, int n, int* status, cudaStream_t st);
-// sm_paste_labels / sm_label_boxes (include/siammask_b200.h)
+// sm_paste_labels / sm_label_boxes (include/siammask_b200.h).  desc (optional, the *_ragged entry points): video g's
+// anno / labels live at desc[g].offset with desc[g].h x desc[g].w pixels, and H, W are the largest h, w.
 void launch_paste_labels(const float* masks, int side, const double* maps, const uint8_t* anno, const int32_t* obj_off,
-                         const int32_t* objects, int G, int H, int W, double seg_thr, uint8_t* labels, cudaStream_t st);
+                         const int32_t* objects, int G, int H, int W, double seg_thr, uint8_t* labels, cudaStream_t st,
+                         const sm_image_desc* desc = nullptr);
 // sm_paste_labels_iou: the same labels plus per-entry IoU counts; counts must hold obj_off[G]*T*2 int32
 void launch_paste_labels_iou(const float* masks, int side, const double* maps, const uint8_t* anno,
                              const int32_t* obj_off, const int32_t* objects, const int32_t* target_ids, int G, int H,
                              int W, double seg_thr, uint8_t* labels, const double* thrs, int T, int32_t* counts,
-                             cudaStream_t st);
+                             cudaStream_t st, const sm_image_desc* desc = nullptr);
 void launch_label_boxes(const uint8_t* anno, int G, int H, int W, const int32_t* queries, int Q, int32_t* boxes,
-                        cudaStream_t st);
+                        cudaStream_t st, const sm_image_desc* desc = nullptr);
 // sm_vot_overlap (include/siammask_b200.h): compute_polygon_overlap of B pairs of 4-point polygons, bounds (0, 0, W, H)
-void launch_vot_overlap(const float* poly_a, const float* poly_b, int B, int W, int H, float* overlap, cudaStream_t st);
+// or, with wh (device int32 [B][2]), pair b's own (W, H) = wh[b]
+void launch_vot_overlap(const float* poly_a, const float* poly_b, int B, int W, int H, float* overlap, cudaStream_t st,
+                        const int32_t* wh = nullptr);
 void launch_absmax(const Act& a, float* slot, cudaStream_t st);
 void launch_xcorr_nchw_f32(const float* x, const float* k, float* out, int planes, int H, int W, int kh, int kw,
                            cudaStream_t st);
@@ -178,17 +184,21 @@ void launch_deconv(const float* p3, const float* w, const float* bias, float* ou
                    int cout, cudaStream_t st);
 void launch_split_to_f32(const Act& in, float* out, cudaStream_t st, float mul = 1.f);
 void launch_import_nchw(const float* x_nchw, Act out, cudaStream_t st);
+// dst_desc (optional, sm_warp_affine_ragged): image b is dst_desc[b].h x dst_desc[b].w at dst + dst_desc[b].offset,
+// and dh, dw are the largest h, w
 void launch_warp_affine(const float* src, int sh, int sw, const double* maps, float* dst, int dh, int dw, float border,
-                        int B, cudaStream_t st);
+                        int B, cudaStream_t st, const sm_image_desc* dst_desc = nullptr);
 void launch_tracker_prepare(int B, const double* state, const int32_t* avg, const TrackerHp& hp, int32_t* boxes,
                             double* tsz, double* aux, cudaStream_t st);
 // hp_table (optional): device f64 [B][3] = (penalty_k, window_influence, lr) per stream, replacing hp.penalty_k / hp.lr
 void launch_tracker_update(int B, double* state, const float* rec, const double* aux, const int32_t* imsize,
                            const TrackerHp& hp, int A, int R, double* maps, double* out, cudaStream_t st,
                            const double* hp_table = nullptr);
-// frame_idx == nullptr: stream b crops frames + b * frame_stride; else frames + frame_idx[b] * frame_stride
+// frame_idx == nullptr: stream b crops frames + b * frame_stride; else frames + frame_idx[b] * frame_stride, or, with
+// desc (sm_crop_resize_ragged), the frame desc[frame_idx[b]] (frame_stride, H and W are then unused)
 void launch_crop_resize(const uint8_t* frames, size_t frame_stride, int H, int W, const int32_t* box, int B, int model,
-                        float* out, cudaStream_t st, const int32_t* frame_idx = nullptr);
+                        float* out, cudaStream_t st, const int32_t* frame_idx = nullptr,
+                        const sm_image_desc* desc = nullptr);
 // hp (optional): device f64 [B][3] per-stream table; stream b then uses hp[b][0] / hp[b][1] instead of the scalars
 void launch_select(const float* cls, const float* loc, const float* anchors, const float* window, const double* tsz,
                    int B, int A, int R, double penalty_k, double window_influence, int32_t* best_idx, int32_t* pos,

@@ -2054,6 +2054,83 @@ int sm_crop_resize_indexed(const uint8_t* frames, size_t frame_stride, int32_t H
   SM_API_END
 }
 
+int sm_crop_resize_ragged(const uint8_t* frames, const sm_image_desc* frame_desc, const int32_t* frame_idx,
+                          const int32_t* boxes, int32_t B, int32_t model_size, float* out, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(B >= 0 && model_size > 0, "bad argument");
+  if (B == 0) return 0;
+  SMK_CHECK(frames && frame_desc && frame_idx && boxes && out, "null argument");
+  require_device();
+  smk::launch_crop_resize(frames, 0, 0, 0, boxes, B, model_size, out, static_cast<cudaStream_t>(stream), frame_idx,
+                          frame_desc);
+  SM_API_END
+}
+
+int sm_paste_labels_ragged(const float* masks, int32_t side, const double* maps, const uint8_t* anno,
+                           const int32_t* obj_offsets, const int32_t* objects, const sm_image_desc* video_desc, int32_t G,
+                           int32_t max_h, int32_t max_w, double seg_thr, uint8_t* labels, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(G >= 0 && max_h >= 1 && max_w >= 1 && side > 0, "bad argument");
+  SMK_CHECK(seg_thr >= -1.0, "seg_thr must be >= -1 (objects that miss a pixel are skipped as value -1)");
+  if (G == 0) return 0;
+  SMK_CHECK(obj_offsets && objects && video_desc && labels, "null argument");
+  require_device();
+  smk::launch_paste_labels(masks, side, maps, anno, obj_offsets, objects, G, max_h, max_w, seg_thr, labels,
+                           static_cast<cudaStream_t>(stream), video_desc);
+  SM_API_END
+}
+
+int sm_paste_labels_iou_ragged(const float* masks, int32_t side, const double* maps, const uint8_t* anno,
+                               const int32_t* obj_offsets, const int32_t* objects, const int32_t* target_ids,
+                               const sm_image_desc* video_desc, int32_t G, int32_t max_h, int32_t max_w, double seg_thr,
+                               uint8_t* labels, const double* thrs, int32_t T, int32_t* counts, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(G >= 0 && max_h >= 1 && max_w >= 1 && side > 0, "bad argument");
+  SMK_CHECK(seg_thr >= -1.0, "seg_thr must be >= -1 (objects that miss a pixel are skipped as value -1)");
+  SMK_CHECK((int64_t)max_h * max_w <= INT32_MAX, "frame too large for int32 counts");
+  SMK_CHECK(T >= 1 && T <= 32, "1 <= T <= 32 thresholds");
+  if (G == 0) return 0;
+  SMK_CHECK(anno && obj_offsets && objects && target_ids && video_desc && labels && thrs && counts, "null argument");
+  require_device();
+  smk::launch_paste_labels_iou(masks, side, maps, anno, obj_offsets, objects, target_ids, G, max_h, max_w, seg_thr,
+                               labels, thrs, T, counts, static_cast<cudaStream_t>(stream), video_desc);
+  SM_API_END
+}
+
+int sm_label_boxes_ragged(const uint8_t* anno, const sm_image_desc* video_desc, int32_t G, const int32_t* queries,
+                          int32_t Q, int32_t* boxes, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(G >= 0 && Q >= 0, "bad argument");
+  if (Q == 0) return 0;
+  SMK_CHECK(anno && video_desc && queries && boxes, "null argument");
+  require_device();
+  smk::launch_label_boxes(anno, G, 0, 0, queries, Q, boxes, static_cast<cudaStream_t>(stream), video_desc);
+  SM_API_END
+}
+
+int sm_vot_overlap_sized(const float* poly_a, const float* poly_b, int32_t B, const int32_t* wh, float* overlap,
+                         void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(B >= 0, "bad argument");
+  if (B == 0) return 0;
+  SMK_CHECK(poly_a && poly_b && wh && overlap, "null argument");
+  require_device();
+  smk::launch_vot_overlap(poly_a, poly_b, B, 0, 0, overlap, static_cast<cudaStream_t>(stream), wh);
+  SM_API_END
+}
+
+int sm_warp_affine_ragged(const float* src, int32_t side, const double* maps, float* dst, const sm_image_desc* dst_desc,
+                          int32_t B, int32_t max_h, int32_t max_w, float border_value, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(B >= 0 && side > 0 && max_h >= 1 && max_w >= 1, "bad argument");
+  if (B == 0) return 0;
+  SMK_CHECK(src && maps && dst && dst_desc, "null argument");
+  require_device();
+  smk::launch_warp_affine(src, side, side, maps, dst, max_h, max_w, border_value, B, static_cast<cudaStream_t>(stream),
+                          dst_desc);
+  SM_API_END
+}
+
 int sm_paste_labels(const float* masks, int32_t side, const double* maps, const uint8_t* anno, const int32_t* obj_offsets,
                     const int32_t* objects, int32_t G, int32_t H, int32_t W, double seg_thr, uint8_t* labels,
                     void* stream) {

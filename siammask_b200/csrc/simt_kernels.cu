@@ -834,17 +834,26 @@ __device__ __forceinline__ void cv_coeff(int d, double scale, int src_n, bool cl
   a1 = __float2int_rn(f * 2048.f);
 }
 
-// frame_idx (optional, sm_crop_resize_indexed): stream b crops frame frame_idx[b] instead of frame b.
+// frame_idx (optional, sm_crop_resize_indexed): stream b crops frame frame_idx[b] instead of frame b.  desc (optional,
+// sm_crop_resize_ragged, with frame_idx): the frame is desc[frame_idx[b]] of a packed buffer, with its own H and W.
 __global__ void crop_resize_kernel(const uint8_t* __restrict__ frames, size_t frame_stride, int H, int W,
                                    const int32_t* __restrict__ box, int model, float* __restrict__ out,
-                                   const int32_t* __restrict__ frame_idx) {
+                                   const int32_t* __restrict__ frame_idx, const sm_image_desc* __restrict__ desc) {
   const int b = blockIdx.z;
   const int dx = blockIdx.x * blockDim.x + threadIdx.x;
   const int dy = blockIdx.y * blockDim.y + threadIdx.y;
   if (dx >= model || dy >= model) return;
   const int32_t* bx = box + 8 * b;
   const int xmin = bx[0], ymin = bx[1], sz = bx[2];
-  const uint8_t* fr = frames + (size_t)(frame_idx != nullptr ? frame_idx[b] : b) * frame_stride;
+  const uint8_t* fr;
+  if (desc != nullptr) {
+    const sm_image_desc d = desc[frame_idx[b]];
+    fr = frames + d.offset;
+    H = d.h;
+    W = d.w;
+  } else {
+    fr = frames + (size_t)(frame_idx != nullptr ? frame_idx[b] : b) * frame_stride;
+  }
   auto px = [&](int y, int x, int c) -> int {      // pixel of the (virtual, padded) patch
     const int fy = y + ymin, fx = x + xmin;
     if (fy < 0 || fy >= H || fx < 0 || fx >= W) return bx[3 + c];
@@ -923,15 +932,25 @@ __device__ __forceinline__ float warp_sample(const float* __restrict__ s, int sh
   return v;
 }
 
+// dst_desc (optional, sm_warp_affine_ragged): image b is dst_desc[b].h x dst_desc[b].w at dst + dst_desc[b].offset; the
+// grid covers the largest size (dh x dw) and threads outside image b return.
 __global__ void warp_affine_kernel(const float* __restrict__ src, int sh, int sw, const double* __restrict__ maps,
-                                   float* __restrict__ dst, int dh, int dw, float border) {
+                                   float* __restrict__ dst, int dh, int dw, float border,
+                                   const sm_image_desc* __restrict__ dst_desc) {
   const int b = blockIdx.z;
   const int x = blockIdx.x * blockDim.x + threadIdx.x;
   const int y = blockIdx.y * blockDim.y + threadIdx.y;
+  size_t base = (size_t)b * dh * dw;
+  if (dst_desc != nullptr) {
+    const sm_image_desc d = dst_desc[b];
+    base = (size_t)d.offset;
+    dh = d.h;
+    dw = d.w;
+  }
   if (x >= dw || y >= dh) return;
   double inv[6];
   warp_invert_map(maps + 6 * b, inv);
-  dst[((size_t)b * dh + y) * dw + x] = warp_sample(src + (size_t)b * sh * sw, sh, sw, warp_tap(inv, x, y), border);
+  dst[base + (size_t)y * dw + x] = warp_sample(src + (size_t)b * sh * sw, sh, sw, warp_tap(inv, x, y), border);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -960,16 +979,16 @@ struct PasteBest {
   __device__ __forceinline__ bool passes(double thr) const { return !nan && k >= 0 && v > thr; }
 };
 
-// Max / first argmax of pixel (x, y) of video g over entries [o0, o1).  Block = 32 x 8 pixels at (bx0, by0); every
-// thread of the block calls it (objects are staged in shared memory between barriers).
+// Max / first argmax of pixel (x, y) of video g over entries [o0, o1); `inside`: the pixel lies in the video.  Block =
+// 32 x 8 pixels at (bx0, by0); every thread of the block calls it (objects are staged in shared memory between
+// barriers).  H, W bound the block for the cull only: any bounds that contain the video's pixels give the same result.
 __device__ __forceinline__ PasteBest paste_best(const float* __restrict__ masks, int side, const double* __restrict__ maps,
                                                 const uint8_t* __restrict__ anno, const int32_t* __restrict__ objects,
                                                 int o0, int o1, int bx0, int by0, int x, int y, int H, int W,
-                                                size_t pix) {
+                                                size_t pix, bool inside) {
   __shared__ double s_inv[PL_CHUNK][6];
   __shared__ int s_kind[PL_CHUNK], s_arg[PL_CHUNK];
   const int tid = threadIdx.y * 32 + threadIdx.x;
-  const bool inside = x < W && y < H;
   double best = 0.0;
   int best_k = -1;
   bool nan = false;
@@ -1017,18 +1036,37 @@ __device__ __forceinline__ PasteBest paste_best(const float* __restrict__ masks,
   return PasteBest{best, best_k, nan};
 }
 
+// desc (optional, the *_ragged entry points): video g is desc[g] of a packed buffer.  video_size replaces H, W (the
+// grid's bounds) by video g's own size; video_pixel is the index of (x, y) in video g's anno / labels.  The paste
+// kernels keep the grid's bounds for paste_best's block cull (kernel parameters: nothing stays live in registers
+// across its calls).
+__device__ __forceinline__ void video_size(const sm_image_desc* __restrict__ desc, int g, int& H, int& W) {
+  if (desc == nullptr) return;
+  H = desc[g].h;
+  W = desc[g].w;
+}
+
+__device__ __forceinline__ size_t video_pixel(const sm_image_desc* __restrict__ desc, int g, int x, int y, int H, int W) {
+  return desc == nullptr ? ((size_t)g * H + y) * W + x : (size_t)desc[g].offset + (size_t)y * W + x;
+}
+
 __global__ void __launch_bounds__(256) paste_labels_kernel(const float* __restrict__ masks, int side,
                                                            const double* __restrict__ maps, const uint8_t* __restrict__ anno,
                                                            const int32_t* __restrict__ obj_off,
                                                            const int32_t* __restrict__ objects, int H, int W,
-                                                           double seg_thr, uint8_t* __restrict__ labels) {
+                                                           double seg_thr, uint8_t* __restrict__ labels,
+                                                           const sm_image_desc* __restrict__ desc) {
   const int g = blockIdx.z;
   const int bx0 = blockIdx.x * 32, by0 = blockIdx.y * 8;
   const int x = bx0 + threadIdx.x, y = by0 + threadIdx.y;
+  int Hg = H, Wg = W;
+  video_size(desc, g, Hg, Wg);
+  if (bx0 >= Wg || by0 >= Hg) return;                // block-uniform: a block outside video g (paste_best has barriers)
+  const bool inside = x < Wg && y < Hg;
   const int2 o = paste_range(obj_off, g);
-  const size_t pix = ((size_t)g * H + y) * W + x;
-  const PasteBest b = paste_best(masks, side, maps, anno, objects, o.x, o.y, bx0, by0, x, y, H, W, pix);
-  if (x < W && y < H) labels[pix] = b.passes(seg_thr) ? (uint8_t)(b.k + 1) : (uint8_t)0;
+  const size_t pix = video_pixel(desc, g, x, y, Hg, Wg);
+  const PasteBest b = paste_best(masks, side, maps, anno, objects, o.x, o.y, bx0, by0, x, y, H, W, pix, inside);
+  if (inside) labels[pix] = b.passes(seg_thr) ? (uint8_t)(b.k + 1) : (uint8_t)0;
 }
 
 // sm_paste_labels_iou: the label map of paste_labels_kernel plus, for T thresholds, the (intersection, union) of
@@ -1061,7 +1099,8 @@ __global__ void __launch_bounds__(256) paste_labels_iou_kernel(const float* __re
                                                                const int32_t* __restrict__ target_ids, int H, int W,
                                                                double seg_thr, uint8_t* __restrict__ labels,
                                                                const double* __restrict__ thrs, int T,
-                                                               int32_t* __restrict__ counts) {
+                                                               int32_t* __restrict__ counts,
+                                                               const sm_image_desc* __restrict__ desc) {
   __shared__ uint8_t s_entry[256];                   // anno value -> video-local entry scored against it
   __shared__ double s_thr[PI_MAX_T];
   __shared__ int s_int[PL_CHUNK][PI_MAX_T];          // pixels labelled k+1 inside k's target
@@ -1071,7 +1110,10 @@ __global__ void __launch_bounds__(256) paste_labels_iou_kernel(const float* __re
   const int tid = threadIdx.y * 32 + threadIdx.x, lane = threadIdx.x;
   const int bx0 = blockIdx.x * 32, by0 = blockIdx.y * 8;
   const int x = bx0 + threadIdx.x, y = by0 + threadIdx.y;
-  const bool inside = x < W && y < H;
+  int Hg = H, Wg = W;
+  video_size(desc, g, Hg, Wg);
+  if (bx0 >= Wg || by0 >= Hg) return;                // block-uniform, before the first barrier: nothing to count
+  const bool inside = x < Wg && y < Hg;
   const int2 o = paste_range(obj_off, g);
   s_entry[tid] = PI_NONE;                            // 256 threads
   if (tid < T) s_thr[tid] = thrs[tid];
@@ -1081,8 +1123,8 @@ __global__ void __launch_bounds__(256) paste_labels_iou_kernel(const float* __re
     if (id >= 1 && id <= 255) s_entry[id] = (uint8_t)k;       // ids are unique within a video (precondition)
   }
   __syncthreads();
-  const size_t pix = ((size_t)g * H + y) * W + x;
-  const PasteBest b = paste_best(masks, side, maps, anno, objects, o.x, o.y, bx0, by0, x, y, H, W, pix);
+  const size_t pix = video_pixel(desc, g, x, y, Hg, Wg);
+  const PasteBest b = paste_best(masks, side, maps, anno, objects, o.x, o.y, bx0, by0, x, y, H, W, pix, inside);
   if (inside) labels[pix] = b.passes(seg_thr) ? (uint8_t)(b.k + 1) : (uint8_t)0;
   unsigned pm = 0;                                  // bit t: the pixel is labelled b.k + 1 at threshold t
   for (int t = 0; t < T; ++t)
@@ -1262,13 +1304,15 @@ constexpr int LB_THREADS = 512;
 
 __global__ void __launch_bounds__(LB_THREADS) label_boxes_kernel(const uint8_t* __restrict__ anno, int G, int H, int W,
                                                                  const int32_t* __restrict__ queries,
-                                                                 int32_t* __restrict__ boxes) {
+                                                                 int32_t* __restrict__ boxes,
+                                                                 const sm_image_desc* __restrict__ desc) {
   __shared__ int red[4][LB_THREADS / 32];
   const int q = blockIdx.x;
   const int g = queries[2 * q], id = queries[2 * q + 1];
   int xmn = INT_MAX, ymn = INT_MAX, xmx = -1, ymx = -1;
   if (g >= 0 && g < G) {
-    const uint8_t* a = anno + (size_t)g * H * W;
+    video_size(desc, g, H, W);
+    const uint8_t* a = anno + video_pixel(desc, g, 0, 0, H, W);
     for (int y = 0; y < H; ++y)
       for (int x = threadIdx.x; x < W; x += LB_THREADS)
         if (a[(size_t)y * W + x] == id) {
@@ -1367,10 +1411,15 @@ __device__ __forceinline__ int vot_row(const float* poly, int pixelY, int width,
 
 __global__ void __launch_bounds__(VO_THREADS) vot_overlap_kernel(const float* __restrict__ poly_a,
                                                                  const float* __restrict__ poly_b, int W, int H,
-                                                                 float* __restrict__ overlap) {
+                                                                 float* __restrict__ overlap,
+                                                                 const int32_t* __restrict__ wh) {
   __shared__ int red[3][VO_THREADS / 32];
   __shared__ float s_poly[2][8];
   const int p = blockIdx.x;
+  if (wh != nullptr) {                                 // sm_vot_overlap_sized: pair p's own bounds
+    W = wh[2 * p];
+    H = wh[2 * p + 1];
+  }
   const float* pa = poly_a + 8 * (size_t)p;
   const float* pb = poly_b + 8 * (size_t)p;
   const VotBounds b1 = vot_bounds(pa, (float)W, (float)H), b2 = vot_bounds(pb, (float)W, (float)H);
@@ -1763,9 +1812,9 @@ void launch_import_nchw(const float* x, Act out, cudaStream_t st) {
 }
 
 void launch_warp_affine(const float* src, int sh, int sw, const double* maps, float* dst, int dh, int dw, float border,
-                        int B, cudaStream_t st) {
+                        int B, cudaStream_t st, const sm_image_desc* dst_desc) {
   dim3 block(32, 8), grid((dw + 31) / 32, (dh + 7) / 8, B);
-  warp_affine_kernel<<<grid, block, 0, st>>>(src, sh, sw, maps, dst, dh, dw, border);
+  warp_affine_kernel<<<grid, block, 0, st>>>(src, sh, sw, maps, dst, dh, dw, border, dst_desc);
   SMK_CUDA(cudaGetLastError());
 }
 
@@ -1791,30 +1840,31 @@ void launch_tracker_update(int B, double* state, const float* rec, const double*
 }
 
 void launch_crop_resize(const uint8_t* frames, size_t frame_stride, int H, int W, const int32_t* box, int B, int model,
-                        float* out, cudaStream_t st, const int32_t* frame_idx) {
+                        float* out, cudaStream_t st, const int32_t* frame_idx, const sm_image_desc* desc) {
   dim3 block(32, 8), grid((model + 31) / 32, (model + 7) / 8, B);
-  crop_resize_kernel<<<grid, block, 0, st>>>(frames, frame_stride, H, W, box, model, out, frame_idx);
+  crop_resize_kernel<<<grid, block, 0, st>>>(frames, frame_stride, H, W, box, model, out, frame_idx, desc);
   SMK_CUDA(cudaGetLastError());
 }
 
 void launch_paste_labels(const float* masks, int side, const double* maps, const uint8_t* anno, const int32_t* obj_off,
-                         const int32_t* objects, int G, int H, int W, double seg_thr, uint8_t* labels, cudaStream_t st) {
+                         const int32_t* objects, int G, int H, int W, double seg_thr, uint8_t* labels, cudaStream_t st,
+                         const sm_image_desc* desc) {
   dim3 block(32, 8), grid((W + 31) / 32, (H + 7) / 8, G);
-  paste_labels_kernel<<<grid, block, 0, st>>>(masks, side, maps, anno, obj_off, objects, H, W, seg_thr, labels);
+  paste_labels_kernel<<<grid, block, 0, st>>>(masks, side, maps, anno, obj_off, objects, H, W, seg_thr, labels, desc);
   SMK_CUDA(cudaGetLastError());
 }
 
 void launch_paste_labels_iou(const float* masks, int side, const double* maps, const uint8_t* anno,
                              const int32_t* obj_off, const int32_t* objects, const int32_t* target_ids, int G, int H,
                              int W, double seg_thr, uint8_t* labels, const double* thrs, int T, int32_t* counts,
-                             cudaStream_t st) {
+                             cudaStream_t st, const sm_image_desc* desc) {
   SMK_CHECK(T >= 1 && T <= PI_MAX_T, "1 <= T <= 32 thresholds");
   // the number of entries lives on the device (obj_off[G]): a grid-stride init sized for a few hundred of them
   paste_iou_init_kernel<<<std::min(G, 32), 256, 0, st>>>(obj_off, G, thrs, T, counts);
   SMK_CUDA(cudaGetLastError());
   dim3 block(32, 8), grid((W + 31) / 32, (H + 7) / 8, G);
   paste_labels_iou_kernel<<<grid, block, 0, st>>>(masks, side, maps, anno, obj_off, objects, target_ids, H, W, seg_thr,
-                                                  labels, thrs, T, counts);
+                                                  labels, thrs, T, counts, desc);
   SMK_CUDA(cudaGetLastError());
 }
 
@@ -1833,13 +1883,14 @@ void launch_mask_iou(const float* masks, int side, const double* maps, const uin
 }
 
 void launch_label_boxes(const uint8_t* anno, int G, int H, int W, const int32_t* queries, int Q, int32_t* boxes,
-                        cudaStream_t st) {
-  label_boxes_kernel<<<Q, LB_THREADS, 0, st>>>(anno, G, H, W, queries, boxes);
+                        cudaStream_t st, const sm_image_desc* desc) {
+  label_boxes_kernel<<<Q, LB_THREADS, 0, st>>>(anno, G, H, W, queries, boxes, desc);
   SMK_CUDA(cudaGetLastError());
 }
 
-void launch_vot_overlap(const float* poly_a, const float* poly_b, int B, int W, int H, float* overlap, cudaStream_t st) {
-  vot_overlap_kernel<<<B, VO_THREADS, 0, st>>>(poly_a, poly_b, W, H, overlap);
+void launch_vot_overlap(const float* poly_a, const float* poly_b, int B, int W, int H, float* overlap, cudaStream_t st,
+                        const int32_t* wh) {
+  vot_overlap_kernel<<<B, VO_THREADS, 0, st>>>(poly_a, poly_b, W, H, overlap, wh);
   SMK_CUDA(cudaGetLastError());
 }
 

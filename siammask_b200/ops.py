@@ -128,8 +128,11 @@ def paste_labels(masks, maps, anno, obj_offsets, objects, size, seg_thr: float) 
     return _paste_labels(masks, maps, anno, obj_offsets, objects, size, seg_thr)
 
 
-def _paste_labels(masks, maps, anno, obj_offsets, objects, size, seg_thr: float) -> torch.Tensor:
-    """`paste_labels` without the host-side check of the offsets (callers that validated their tables once)."""
+def _paste_labels(masks, maps, anno, obj_offsets, objects, size, seg_thr: float, ragged=None) -> torch.Tensor:
+    """`paste_labels` without the host-side check of the offsets (callers that validated their tables once).
+    ragged = (desc, total): videos of different sizes (`sm_paste_labels_ragged`): desc the device sm_image_desc table of
+    the G videos, total the packed label buffer's length; anno (if given) is that packed uint8 buffer, size = (max_h,
+    max_w), and the packed labels uint8 [total] are returned."""
     off = torch.as_tensor(obj_offsets, dtype=torch.int32).reshape(-1)
     G = off.numel() - 1
     H, W = int(size[0]), int(size[1])
@@ -146,18 +149,24 @@ def _paste_labels(masks, maps, anno, obj_offsets, objects, size, seg_thr: float)
         masks = masks.to(dev, torch.float32).contiguous()
         side = int(masks.shape[-1])
         maps = torch.as_tensor(maps, dtype=torch.float64).reshape(-1, 6).to(dev).contiguous()
+    shape = (G, H, W) if ragged is None else (int(ragged[1]),)
     if anno is not None:
         anno = anno.to(dev).contiguous()
-        if anno.dtype != torch.uint8 or tuple(anno.shape) != (G, H, W):
-            raise ValueError(f"anno must be uint8 [{G},{H},{W}]")
-    out = torch.empty(G, H, W, dtype=torch.uint8, device=dev)
+        if anno.dtype != torch.uint8 or tuple(anno.shape) != shape:
+            raise ValueError(f"anno must be uint8 {list(shape)}")
+    out = torch.empty(shape, dtype=torch.uint8, device=dev)
 
     def ptr(t):
         return t.data_ptr() if t is not None else None
     with torch.cuda.device(dev):
-        _lib.check(lib.sm_paste_labels(ptr(masks), side, ptr(maps) if masks is not None else None, ptr(anno),
-                                       off.data_ptr(), obj.data_ptr(), G, H, W, float(seg_thr), out.data_ptr(),
-                                       _stream(dev)))
+        if ragged is None:
+            _lib.check(lib.sm_paste_labels(ptr(masks), side, ptr(maps) if masks is not None else None, ptr(anno),
+                                           off.data_ptr(), obj.data_ptr(), G, H, W, float(seg_thr), out.data_ptr(),
+                                           _stream(dev)))
+        else:
+            _lib.check(lib.sm_paste_labels_ragged(ptr(masks), side, ptr(maps) if masks is not None else None, ptr(anno),
+                                                  off.data_ptr(), obj.data_ptr(), ragged[0].data_ptr(), G, H, W,
+                                                  float(seg_thr), out.data_ptr(), _stream(dev)))
     return out
 
 
@@ -205,9 +214,12 @@ def paste_labels_iou(masks, maps, anno, obj_offsets, objects, target_ids, size, 
                              torch.as_tensor(t, device=dev))
 
 
-def _paste_labels_iou(masks, maps, anno, obj_offsets, objects, target_ids, size, seg_thr: float, thrs, counts=None):
+def _paste_labels_iou(masks, maps, anno, obj_offsets, objects, target_ids, size, seg_thr: float, thrs, counts=None,
+                      ragged=None):
     """`paste_labels_iou` without the host-side checks (callers that validated their tables once): anno uint8, target_ids
-    int32 and thrs float64 are CUDA tensors.  counts (optional): a contiguous int32 CUDA tensor [n,T,2] to write into."""
+    int32 and thrs float64 are CUDA tensors.  counts (optional): a contiguous int32 CUDA tensor [n,T,2] to write into.
+    ragged = (desc, total) as in `_paste_labels` (`sm_paste_labels_iou_ragged`): anno and the returned labels are packed
+    uint8 [total], size = (max_h, max_w)."""
     off = torch.as_tensor(obj_offsets, dtype=torch.int32).reshape(-1)
     G = off.numel() - 1
     H, W = int(size[0]), int(size[1])
@@ -227,13 +239,19 @@ def _paste_labels_iou(masks, maps, anno, obj_offsets, objects, target_ids, size,
     if counts is None:
         counts = torch.empty(n, T, 2, dtype=torch.int32, device=dev)
     cnt = counts if n else torch.empty(1, T, 2, dtype=torch.int32, device=dev)
-    labels = torch.empty(G, H, W, dtype=torch.uint8, device=dev)
+    labels = torch.empty((G, H, W) if ragged is None else (int(ragged[1]),), dtype=torch.uint8, device=dev)
+    mp = masks.data_ptr() if masks is not None else None
+    mpp = maps.data_ptr() if masks is not None else None
     with torch.cuda.device(dev):
-        _lib.check(lib.sm_paste_labels_iou(masks.data_ptr() if masks is not None else None, side,
-                                           maps.data_ptr() if masks is not None else None, anno.data_ptr(),
-                                           off.data_ptr(), obj.data_ptr(), tid.contiguous().data_ptr(), G, H, W,
-                                           float(seg_thr), labels.data_ptr(), thrs.contiguous().data_ptr(), T,
-                                           cnt.data_ptr(), _stream(dev)))
+        if ragged is None:
+            _lib.check(lib.sm_paste_labels_iou(mp, side, mpp, anno.data_ptr(), off.data_ptr(), obj.data_ptr(),
+                                               tid.contiguous().data_ptr(), G, H, W, float(seg_thr), labels.data_ptr(),
+                                               thrs.contiguous().data_ptr(), T, cnt.data_ptr(), _stream(dev)))
+        else:
+            _lib.check(lib.sm_paste_labels_iou_ragged(mp, side, mpp, anno.data_ptr(), off.data_ptr(), obj.data_ptr(),
+                                                      tid.contiguous().data_ptr(), ragged[0].data_ptr(), G, H, W,
+                                                      float(seg_thr), labels.data_ptr(), thrs.contiguous().data_ptr(),
+                                                      T, cnt.data_ptr(), _stream(dev)))
     return labels, counts
 
 
@@ -253,6 +271,55 @@ def label_boxes(anno: torch.Tensor, queries) -> torch.Tensor:
     G, H, W = anno.shape
     with torch.cuda.device(dev):
         _lib.check(lib.sm_label_boxes(anno.data_ptr(), G, H, W, q.data_ptr(), q.shape[0], out.data_ptr(), _stream(dev)))
+    return out
+
+
+def _label_boxes_ragged(anno: torch.Tensor, desc: torch.Tensor, G: int, queries) -> torch.Tensor:
+    """`label_boxes` for G videos of different sizes (C ABI `sm_label_boxes_ragged`): anno the packed uint8 CUDA buffer
+    and desc its device sm_image_desc table; queries int [Q,2] (g, id).  No host-side checks."""
+    lib = _lib.load()
+    dev = anno.device
+    q = torch.as_tensor(queries, dtype=torch.int32).reshape(-1, 2).to(dev).contiguous()
+    out = torch.zeros(q.shape[0], 4, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.sm_label_boxes_ragged(anno.contiguous().data_ptr(), desc.data_ptr(), int(G), q.data_ptr(),
+                                             q.shape[0], out.data_ptr(), _stream(dev)))
+    return out
+
+
+def _crop_resize_ragged(frames: torch.Tensor, desc: torch.Tensor, frame_idx, boxes, model_size: int) -> torch.Tensor:
+    """`crop_resize` over a packed uint8 CUDA frame buffer (C ABI `sm_crop_resize_ragged`): stream b crops frame
+    desc[frame_idx[b]]; boxes int [B,6] as in `crop_resize`.  No host-side checks."""
+    lib = _lib.load()
+    dev = frames.device
+    bx = torch.as_tensor(boxes, dtype=torch.int32).reshape(-1, 6)
+    B = bx.shape[0]
+    full = torch.zeros(B, 8, dtype=torch.int32)
+    full[:, :6] = bx
+    full = full.to(dev)
+    idx = torch.as_tensor(frame_idx, dtype=torch.int32).reshape(-1).to(dev).contiguous()
+    out = torch.empty(B, 3, model_size, model_size, device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        _lib.check(lib.sm_crop_resize_ragged(frames.contiguous().data_ptr(), desc.data_ptr(), idx.data_ptr(),
+                                             full.data_ptr(), B, model_size, out.data_ptr(), _stream(dev)))
+    return out
+
+
+def _warp_affine_ragged(src: torch.Tensor, maps, desc: torch.Tensor, max_hw, total: int,
+                        border_value: float = -1.0) -> torch.Tensor:
+    """`warp_affine` of B square masks src f32 CUDA [B,side,side] into destinations of different sizes (C ABI
+    `sm_warp_affine_ragged`): desc the device sm_image_desc table of the B destinations in a packed f32 buffer of
+    `total` elements, max_hw = (max_h, max_w).  Returns that buffer (elements outside every image are left as they
+    were allocated).  No host-side checks."""
+    lib = _lib.load()
+    dev = src.device
+    s3 = src.to(torch.float32).contiguous()
+    m = torch.as_tensor(maps, dtype=torch.float64).reshape(-1, 6).to(dev).contiguous()
+    out = torch.empty(int(total), device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        _lib.check(lib.sm_warp_affine_ragged(s3.data_ptr(), int(s3.shape[-1]), m.data_ptr(), out.data_ptr(),
+                                             desc.data_ptr(), int(s3.shape[0]), int(max_hw[0]), int(max_hw[1]),
+                                             float(border_value), _stream(dev)))
     return out
 
 
@@ -312,16 +379,22 @@ VOT_COORD_LIMIT = 2.0 ** 20       # |coordinate| bound of sm_vot_overlap's preco
 def vot_overlap(poly_a, poly_b, size) -> torch.Tensor:
     """Region overlap of the VOT supervised protocol (tools/test.py:341-354, C ABI `sm_vot_overlap`): pyvotkit's
     vot_overlap(poly_a[b], poly_b[b], (W, H)) for B pairs, bit for bit.  poly_a, poly_b: float32 CUDA [B,8] 4-point
-    polygons x0, y0, .. x3, y3; size = (H, W).  Returns float32 [B]; NaN where both rasterised polygons are empty inside
-    the frame (the protocol does not count that as a loss).  The checks read both polygon tensors on the host: shapes,
-    dtype, device, and every coordinate finite and within +-2^20 px."""
+    polygons x0, y0, .. x3, y3; size = (H, W), or an int array [B,2] of per-pair (H, W) (`sm_vot_overlap_sized`).
+    Returns float32 [B]; NaN where both rasterised polygons are empty inside the frame (the protocol does not count that
+    as a loss).  The checks read both polygon tensors on the host: shapes, dtype, device, and every coordinate finite and
+    within +-2^20 px."""
     for name, p in (("poly_a", poly_a), ("poly_b", poly_b)):
         if not (torch.is_tensor(p) and p.is_cuda and p.dtype == torch.float32 and p.dim() == 2 and p.shape[1] == 8):
             raise ValueError(f"{name} must be a float32 CUDA tensor [B, 8]")
     if poly_a.shape != poly_b.shape or poly_a.device != poly_b.device:
         raise ValueError("poly_a and poly_b must have the same shape and device")
-    H, W = int(size[0]), int(size[1])
-    if H < 1 or W < 1 or (W + 1) * (H + 1) > 2 ** 31 - 1:
+    sz = np.asarray(size.cpu() if torch.is_tensor(size) else size)
+    per_pair = sz.ndim == 2
+    if per_pair and (sz.shape != (poly_a.shape[0], 2) or not np.issubdtype(sz.dtype, np.integer)):
+        raise ValueError(f"per-pair sizes must be an int array [{poly_a.shape[0]}, 2] of (H, W)")
+    hw = sz.reshape(-1, 2).astype(np.int64) if per_pair else np.array([[int(size[0]), int(size[1])]], np.int64)
+    H, W = hw[:, 0], hw[:, 1]
+    if (H < 1).any() or (W < 1).any() or ((W + 1) * (H + 1) > 2 ** 31 - 1).any():
         raise ValueError("size must be (H, W) with H, W >= 1 and (W+1)*(H+1) < 2^31")
     for name, p in (("poly_a", poly_a), ("poly_b", poly_b)):
         v = p.cpu().numpy()
@@ -329,7 +402,10 @@ def vot_overlap(poly_a, poly_b, size) -> torch.Tensor:
             raise ValueError(f"{name}: coordinates must be finite and within +-2^20 px")
     if poly_a.shape[0] == 0:
         return torch.empty(0, dtype=torch.float32, device=poly_a.device)
-    return _vot_overlap(poly_a, poly_b, (H, W))
+    if per_pair:
+        wh = torch.as_tensor(np.stack([W, H], 1).astype(np.int32), device=poly_a.device)
+        return _vot_overlap_sized(poly_a, poly_b, wh)
+    return _vot_overlap(poly_a, poly_b, (int(H[0]), int(W[0])))
 
 
 def _vot_overlap(poly_a, poly_b, size, out=None) -> torch.Tensor:
@@ -344,4 +420,19 @@ def _vot_overlap(poly_a, poly_b, size, out=None) -> torch.Tensor:
     with torch.cuda.device(dev):
         _lib.check(lib.sm_vot_overlap(poly_a.data_ptr(), poly_b.data_ptr(), B, int(size[1]), int(size[0]),
                                       out.data_ptr(), _stream(dev)))
+    return out
+
+
+def _vot_overlap_sized(poly_a, poly_b, wh, out=None) -> torch.Tensor:
+    """`_vot_overlap` with per-pair bounds (C ABI `sm_vot_overlap_sized`): wh int32 CUDA [B,2] = (W, H) of each pair,
+    inside the precondition.  No host-side checks."""
+    lib = _lib.load()
+    dev = poly_a.device
+    poly_a, poly_b = poly_a.contiguous(), poly_b.contiguous()
+    B = int(poly_a.shape[0])
+    if out is None:
+        out = torch.empty(B, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.sm_vot_overlap_sized(poly_a.data_ptr(), poly_b.data_ptr(), B, wh.contiguous().data_ptr(),
+                                            out.data_ptr(), _stream(dev)))
     return out

@@ -24,6 +24,11 @@ single [H,W,3] frame is shared by all streams).  `add_state` starts streams from
 (target_pos, target_sz), and `reinit` runs siamese_init again for running streams in their own slots (the VOT
 protocol's restart after a failure) without changing the active set; all three template through `_template`.
 
+Frames of different sizes run in one batch: a list of frames (numpy arrays or CUDA tensors, any mix of sizes) is packed
+by `FramePacker` into one device buffer plus an `sm_image_desc` table (offset, h, w per frame), and the crop and the
+paste-back read each stream's own frame from it (`sm_crop_resize_ragged`, `sm_warp_affine_ragged`).  A stream is bound
+to the size of the frame it was added from; the per-stream (W, H) table that the state update clamps against holds it.
+
 The arithmetic is pinned by `tests/test_batch_tracker.py` to the reference loop's golden trajectory and to
 single-stream runs of the host restatement in `oracle/ref_loop.py`.
 """
@@ -64,14 +69,103 @@ class TrackerParams:
                                 self.instance_size, self.total_stride, self.base_size, self.out_size, 0)
 
 
+IMAGE_DESC = np.dtype([("offset", "<i8"), ("h", "<i4"), ("w", "<i4")])      # sm_image_desc of include/siammask_b200.h
+
+
+def image_table(shapes, channels: int) -> np.ndarray:
+    """sm_image_desc rows of images packed back to back: shapes (h, w) per image, None for an empty entry (h = w = 0,
+    occupying nothing); channels elements per pixel."""
+    t = np.zeros(len(shapes), IMAGE_DESC)
+    off = 0
+    for i, s in enumerate(shapes):
+        if s is not None:
+            t[i] = (off, s[0], s[1])
+            off += s[0] * s[1] * channels
+    return t
+
+
+@dataclass
+class Packed:
+    """Images of different sizes in one contiguous device buffer: data (flat, uint8 for frames and label maps), desc
+    the device sm_image_desc table (raw bytes, one row per entry), shapes the host (h, w) per entry (None for a skipped
+    entry), channels the elements per pixel."""
+    data: torch.Tensor
+    desc: torch.Tensor
+    shapes: list
+    channels: int
+    table: np.ndarray
+
+    def view(self, i: int) -> torch.Tensor:
+        """Entry i as a [h,w,channels] (or [h,w] for one channel) view of the buffer."""
+        h, w = self.shapes[i]
+        o = int(self.table[i]["offset"])
+        v = self.data[o:o + h * w * self.channels]
+        return v.view(h, w, self.channels) if self.channels > 1 else v.view(h, w)
+
+
+class FramePacker:
+    """Packs lists of images that differ in size (uint8 numpy arrays or CUDA tensors, [h,w,3] frames or [h,w] label
+    maps) into one device buffer plus an sm_image_desc table.  The table depends only on the sequence of shapes and is
+    uploaded only when that changes, asynchronously from pinned memory, so packing never waits for the device.  Host
+    arrays are concatenated on the host and copied in one transfer; CUDA tensors are concatenated on the device."""
+
+    def __init__(self, dev):
+        self.dev = dev
+        self._tables: dict = {}                     # channels -> (shapes key, device table, host table)
+
+    def table(self, shapes, channels: int):
+        """(device sm_image_desc table, host table) of `shapes` at `channels` elements per pixel."""
+        key = tuple(None if s is None else (int(s[0]), int(s[1])) for s in shapes)
+        hit = self._tables.get(channels)
+        if hit is not None and hit[0] == key:
+            return hit[1], hit[2]
+        t = image_table(key, channels)
+        host = torch.from_numpy(t.view(np.uint8).reshape(-1).copy())
+        if torch.device(self.dev).type == "cuda":
+            host = host.pin_memory()                # the copy below then queues without waiting for the device
+        dev = host.to(self.dev, non_blocking=True)
+        self._tables[channels] = (key, dev, t)
+        return dev, t
+
+    def pack(self, images, channels: int = 3) -> Packed:
+        """images: a list of uint8 [h,w,3] (channels 3) or [h,w] (channels 1) arrays / tensors, or None (skipped)."""
+        if not isinstance(images, (list, tuple)):
+            raise ValueError("expected a list of images")
+        want = "[h,w,3]" if channels == 3 else "[h,w]"
+        shapes, present = [], []
+        for i, im in enumerate(images):
+            if im is None:
+                shapes.append(None)
+                continue
+            t = im if torch.is_tensor(im) else np.asarray(im)
+            if t.dtype not in (np.uint8, torch.uint8):
+                raise ValueError(f"image {i}: uint8 expected (frames are HWC BGR as cv2.imread returns them)")
+            shape = tuple(int(v) for v in t.shape)
+            if len(shape) != (3 if channels == 3 else 2) or (channels == 3 and shape[2] != 3) or min(shape[:2]) < 1:
+                raise ValueError(f"image {i} must be {want} with h, w >= 1, got {shape}")
+            shapes.append(shape[:2])
+            present.append(t)
+        desc, table = self.table(shapes, channels)
+        if present and all(torch.is_tensor(t) and t.is_cuda for t in present):
+            data = torch.cat([t.to(self.dev).reshape(-1) for t in present])
+        elif present:
+            host = np.concatenate([np.ascontiguousarray(t.cpu().numpy() if torch.is_tensor(t) else t).reshape(-1)
+                                   for t in present])
+            data = torch.from_numpy(host).to(self.dev)
+        else:
+            data = torch.zeros(1, dtype=torch.uint8, device=self.dev)
+        return Packed(data, desc, shapes, channels, table)
+
+
 @dataclass
 class TrackResult:
     """Per-frame outputs, all on the device, one row per active stream in the order of `BatchTracker.ids`.  state f64
     [N,8] = x, y, w, h (new target_pos / target_sz), score, penalty, lr (from the stream's own lr), best index; mask:
-    bool [N,H,W] frame-sized masks (or None).  With mask=True, extras also holds "mask_prob" f32 [N,side,side] (sigmoid masks) and "maps" f64 [N,6]
-    (their paste-back maps, overwritten by the next frame)."""
+    bool [N,H,W] frame-sized masks (or None), or, when the streams' frames differ in size, a list of N bool [H_i,W_i]
+    views of one packed buffer in row order.  With mask=True, extras also holds "mask_prob" f32 [N,side,side] (sigmoid
+    masks) and "maps" f64 [N,6] (their paste-back maps, overwritten by the next frame)."""
     state: torch.Tensor
-    mask: torch.Tensor | None = None
+    mask: torch.Tensor | list | None = None
     extras: dict = field(default_factory=dict)
 
     def cpu(self):
@@ -96,6 +190,7 @@ class BatchTracker:
         self.anchors = torch.from_numpy(generate_anchor(net.anchors, R)).to(self.dev)
         self.window = torch.from_numpy(cosine_window(R, A, self.p.windowing).astype(np.float32)).to(self.dev)
         self.hp = self.p.c_struct()
+        self.packer = FramePacker(self.dev)
         self._next_id = 0
         self._clear()
 
@@ -105,7 +200,8 @@ class BatchTracker:
         self._slots: list[int] = []
         self._fidx: list[int] = []
         self._hp: list[tuple[float, float, float]] = []
-        self.im_w = self.im_h = None
+        self._size: list[tuple[int, int]] = []         # (H, W) of the frames each stream reads
+        self.im_w = self.im_h = None                   # the streams' common frame size (None when they differ)
         dev = self.dev
         self.state = torch.zeros(0, 4, dtype=torch.float64, device=dev)
         self.avg = torch.zeros(0, 3, dtype=torch.int32, device=dev)
@@ -135,15 +231,49 @@ class BatchTracker:
             raise ValueError(f"frames must be [H,W,3] or [F,H,W,3], got {tuple(t.shape)}")
         return t.to(self.dev).contiguous()
 
+    def _input(self, frames):
+        """The frames of a call: a list (or tuple) of frames, which may differ in size, is packed (`Packed`, None
+        entries skipped); anything else goes through `_frames`."""
+        if isinstance(frames, Packed):
+            return frames
+        if isinstance(frames, (list, tuple)):
+            return self.packer.pack(frames, 3)
+        return self._frames(frames)
+
     @staticmethod
     def _hw(fr: torch.Tensor):
         return (int(fr.shape[0]), int(fr.shape[1])) if fr.dim() == 3 else (int(fr.shape[1]), int(fr.shape[2]))
 
-    def _crop(self, frames: torch.Tensor, frame_idx: torch.Tensor, boxes: torch.Tensor, size: int) -> torch.Tensor:
+    def _sizes_read(self, fr, src: list[int]) -> list:
+        """(H, W) of the frame each of the streams reading frames `src` of `fr` gets; ValueError for a missing one."""
+        if isinstance(fr, Packed):
+            bad = [i for i in src if not 0 <= i < len(fr.shapes) or fr.shapes[i] is None]
+            if bad:
+                raise ValueError(f"a stream reads frame {bad[0]}, but {len(fr.shapes)} frames were given "
+                                 "(or that entry is None)")
+            return [fr.shapes[i] for i in src]
+        if fr.dim() == 4 and any(i >= fr.shape[0] for i in src):
+            raise ValueError(f"a stream reads frame {max(src)}, but only {fr.shape[0]} frames were given")
+        return [self._hw(fr)] * len(src)
+
+    def _check_sizes(self, fr, rows: list[int], src: list[int]):
+        """A stream is bound to the frame size it was added with: ValueError when rows read frames of another size."""
+        got = self._sizes_read(fr, src)
+        for r, hw in zip(rows, got):
+            if hw != self._size[r]:
+                raise ValueError(f"stream {self._ids[r]} tracks {self._size[r][0]}x{self._size[r][1]} frames, "
+                                 f"got {hw[0]}x{hw[1]}")
+
+    def _crop(self, frames, frame_idx: torch.Tensor, boxes: torch.Tensor, size: int) -> torch.Tensor:
         N = boxes.shape[0]
+        out = torch.empty(N, 3, size, size, device=self.dev, dtype=torch.float32)
+        if isinstance(frames, Packed):
+            _lib.check(self.lib.sm_crop_resize_ragged(frames.data.data_ptr(), frames.desc.data_ptr(),
+                                                      frame_idx.data_ptr(), boxes.data_ptr(), N, size, out.data_ptr(),
+                                                      self._stream()))
+            return out
         H, W = self._hw(frames)
         stride = 0 if frames.dim() == 3 else H * W * 3
-        out = torch.empty(N, 3, size, size, device=self.dev, dtype=torch.float32)
         _lib.check(self.lib.sm_crop_resize_indexed(frames.data_ptr(), stride, H, W, frame_idx.data_ptr(),
                                                    boxes.data_ptr(), N, size, out.data_ptr(), self._stream()))
         return out
@@ -160,19 +290,27 @@ class BatchTracker:
         self.tsz = torch.zeros(N, 2, dtype=torch.float64, device=dev)
         self.aux = torch.zeros(N, 4, dtype=torch.float64, device=dev)
         self.maps = torch.zeros(N, 6, dtype=torch.float64, device=dev)
+        self.imsize = torch.tensor([[w, h] for h, w in self._size], dtype=torch.int32, device=dev).reshape(N, 2)
+        sizes = set(self._size)
+        self.im_h, self.im_w = next(iter(sizes)) if len(sizes) == 1 else (None, None)
+        self._mask_table = None                         # sm_image_desc of the rows' pasted masks, built on first use
 
     def _template(self, fr: torch.Tensor, src: list[int], state: torch.Tensor, slots: list[int]) -> torch.Tensor:
         """The template half of siamese_init (tools/test.py:142-155) for n streams: fr uint8 frames on the device, src
         [n] the frame of `fr` each stream reads, state f64 [n,4] (target_pos, target_sz) exactly as siamese_init
         receives them, slots [n] the engine slots to write.  Returns the streams' avg_chans, int32 [n,3]."""
         n = len(src)
-        H, W = self._hw(fr)
         src_dev = torch.tensor(src, dtype=torch.int32, device=self.dev)
         # avg_chans = np.mean(im, axis=(0, 1)); written into a uint8 image it truncates (:146, :89-100).
         # Sums of < 2^53 integers are exact in float64, so sum / n equals numpy's mean bit for bit.
-        f4 = fr if fr.dim() == 4 else fr.unsqueeze(0)
         uniq = sorted(set(src))
-        mean = f4[uniq].to(torch.float64).sum(dim=(1, 2)) / float(H * W)
+        if isinstance(fr, Packed):
+            mean = torch.stack([fr.view(i).to(torch.float64).sum(dim=(0, 1)) / float(fr.shapes[i][0] * fr.shapes[i][1])
+                                for i in uniq])
+        else:
+            H, W = self._hw(fr)
+            f4 = fr if fr.dim() == 4 else fr.unsqueeze(0)
+            mean = f4[uniq].to(torch.float64).sum(dim=(1, 2)) / float(H * W)
         where = torch.tensor([uniq.index(i) for i in src], device=self.dev)
         avg = mean[where].to(torch.uint8).to(torch.int32).contiguous()
         # template window (:149-155): s_z = round(sqrt(wc_z * hc_z)), crop around target_pos, resize to 127
@@ -221,16 +359,14 @@ class BatchTracker:
             return self._join(frames, self._state(target_pos, target_sz), frame_index, hp)
 
     def _join(self, frames, state: torch.Tensor, frame_index, hp) -> list[int]:
-        fr = self._frames(frames)
+        fr = self._input(frames)
         n = state.shape[0]
-        H, W = self._hw(fr)
-        if self.N and (H, W) != (self.im_h, self.im_w):
-            raise ValueError(f"all streams of a tracker share one frame size ({self.im_h}x{self.im_w})")
         idx = list(range(n)) if frame_index is None else [int(i) for i in np.asarray(frame_index).reshape(-1)]
         if len(idx) != n:
             raise ValueError("one frame index per new stream expected")
-        F = 1 if fr.dim() == 3 else int(fr.shape[0])
-        if fr.dim() == 4 and any(i < 0 or i >= F for i in idx):
+        ragged = isinstance(fr, Packed)
+        F = len(fr.shapes) if ragged else (1 if fr.dim() == 3 else int(fr.shape[0]))
+        if (ragged or fr.dim() == 4) and any(i < 0 or i >= F for i in idx):
             raise ValueError(f"frame index out of range [0, {F})")
         if any(i < 0 for i in idx):
             raise ValueError("frame indices must be >= 0")
@@ -249,14 +385,14 @@ class BatchTracker:
             return []
         if self.N + n > self.net.max_batch or len(free) < n:
             raise ValueError("more streams than the engine was built for")
-        src = idx if fr.dim() == 4 else [0] * n          # frame each new stream reads in this call
+        src = idx if ragged or fr.dim() == 4 else [0] * n          # frame each new stream reads in this call
+        sizes = self._sizes_read(fr, src)                          # each new stream is bound to its frame's size
         avg = self._template(fr, src, state, free)
         ids = list(range(self._next_id, self._next_id + n))
         self._next_id += n
-        self.im_w, self.im_h = W, H
         self.state = torch.cat([self.state, state], 0).contiguous()
         self.avg = torch.cat([self.avg, avg], 0).contiguous()
-        self.imsize = torch.tensor([[W, H]] * (self.N + n), dtype=torch.int32, device=self.dev)
+        self._size += sizes
         self._ids += ids
         self._slots += free
         self._fidx += idx
@@ -280,13 +416,10 @@ class BatchTracker:
         if not ids:
             return
         with torch.cuda.device(self.dev):
-            fr = self._frames(frames)
-            if self._hw(fr) != (self.im_h, self.im_w):
-                raise ValueError(f"frames must be {self.im_h}x{self.im_w}")
+            fr = self._input(frames)
             rows = [self._ids.index(i) for i in ids]
-            src = [self._fidx[r] for r in rows] if fr.dim() == 4 else [0] * len(rows)
-            if fr.dim() == 4 and max(src) >= fr.shape[0]:
-                raise ValueError(f"a stream reads frame {max(src)}, but only {fr.shape[0]} frames were given")
+            src = [self._fidx[r] for r in rows] if isinstance(fr, Packed) or fr.dim() == 4 else [0] * len(rows)
+            self._check_sizes(fr, rows, src)
             state = self._state(target_pos, target_sz)
             if state.shape[0] != len(ids):
                 raise ValueError(f"target_pos and target_sz must be [{len(ids)}, 2]")
@@ -309,8 +442,8 @@ class BatchTracker:
             rows = torch.tensor(keep, dtype=torch.long, device=self.dev)
             self.state = self.state.index_select(0, rows).contiguous()
             self.avg = self.avg.index_select(0, rows).contiguous()
-            self.imsize = self.imsize.index_select(0, rows).contiguous()
             self._ids = [self._ids[r] for r in keep]
+            self._size = [self._size[r] for r in keep]
             self._slots = [self._slots[r] for r in keep]
             self._fidx = [self._fidx[r] for r in keep]
             self._hp = [self._hp[r] for r in keep]
@@ -320,8 +453,8 @@ class BatchTracker:
     # ------------------------------------------------------------------ siamese_init (tools/test.py:132-169)
     @torch.no_grad()
     def init(self, frames, boxes_xywh):
-        """Start over with N streams in slots slot0 .. slot0+N-1.  frames: uint8 [N,H,W,3] (or one shared [H,W,3]);
-        boxes_xywh: [N,4] top-left x, y, w, h of the targets.  Stream i reads frame i of later per-stream frame tensors."""
+        """Start over with N streams in slots slot0 .. slot0+N-1.  frames: uint8 [N,H,W,3] (or one shared [H,W,3], or a
+        list of N frames that may differ in size); boxes_xywh: [N,4] top-left x, y, w, h of the targets.  Stream i reads frame i of later per-stream frame tensors."""
         n = np.asarray(boxes_xywh).reshape(-1, 4).shape[0]
         if n > self.net.max_batch or self.slot0 + n > self.net.num_slots:
             raise ValueError("more streams than the engine was built for")
@@ -339,11 +472,15 @@ class BatchTracker:
             raise RuntimeError("no active streams: call init() or add() first")
         p, N = self.p, self.N
         with torch.cuda.device(self.dev):
-            fr = self._frames(frames)
-            if self._hw(fr) != (self.im_h, self.im_w):
-                raise ValueError(f"frames must be {self.im_h}x{self.im_w}")
-            if fr.dim() == 4 and self._max_fidx >= fr.shape[0]:
-                raise ValueError(f"a stream reads frame {self._max_fidx}, but only {fr.shape[0]} frames were given")
+            fr = self._input(frames)
+            if isinstance(fr, Packed):
+                self._check_sizes(fr, range(N), self._fidx)
+            else:
+                if self._hw(fr) != (self.im_h, self.im_w):
+                    raise ValueError(f"frames must be {self.im_h}x{self.im_w}" if self.im_h is not None else
+                                     "the streams track frames of different sizes: pass the frames as a list")
+                if fr.dim() == 4 and self._max_fidx >= fr.shape[0]:
+                    raise ValueError(f"a stream reads frame {self._max_fidx}, but only {fr.shape[0]} frames were given")
             st = self._stream()
             _lib.check(self.lib.sm_tracker_prepare(N, self.state.data_ptr(), self.avg.data_ptr(), C.byref(self.hp),
                                                    self.boxes.data_ptr(), self.tsz.data_ptr(), self.aux.data_ptr(), st))
@@ -367,10 +504,21 @@ class BatchTracker:
                     raise ValueError(f"out_size {p.out_size} does not match the mask source ({side})")
                 m = logits.sigmoid().view(N, side, side).contiguous()
                 extras["mask_prob"], extras["maps"] = m, self.maps
-                if paste:
+                if paste and self.im_h is not None:
                     W, H = self.im_w, self.im_h
                     pasted = torch.empty(N, H, W, device=self.dev, dtype=torch.float32)
                     _lib.check(self.lib.sm_warp_affine(m.data_ptr(), side, side, self.maps.data_ptr(), pasted.data_ptr(),
                                                        H, W, C.c_float(-1.0), N, st))
                     mask_out = pasted > p.seg_thr
+                elif paste:                                 # streams of different sizes: one packed buffer
+                    if self._mask_table is None:
+                        self._mask_table = self.packer.table(self._size, 1)
+                    desc, table = self._mask_table
+                    total = int(table["offset"][-1]) + self._size[-1][0] * self._size[-1][1]
+                    pasted = torch.empty(total, device=self.dev, dtype=torch.float32)
+                    _lib.check(self.lib.sm_warp_affine_ragged(m.data_ptr(), side, self.maps.data_ptr(), pasted.data_ptr(),
+                                                              desc.data_ptr(), N, max(h for h, _ in self._size),
+                                                              max(w for _, w in self._size), C.c_float(-1.0), st))
+                    flat = pasted > p.seg_thr
+                    mask_out = [flat[int(o):int(o) + h * w].view(h, w) for o, (h, w) in zip(table["offset"], self._size)]
             return TrackResult(state=res, mask=mask_out, extras=extras)

@@ -1,5 +1,6 @@
 """Multi-object video object segmentation on the device: the `track_vos` loop of tools/test.py:459-542 (also driven by
-tools/tune_vos.py) for G videos of one frame size at once.
+tools/tune_vos.py) for G videos at once, which may differ in frame size (pass the frames and annotations as lists:
+the label maps then come back as a list, and the label map, scores and init boxes run through the *_ragged kernels).
 
 In the reference every object of a video is a separate tracker run with its own lifetime: it is initialised from the
 annotation label map at its `start_frame` with `cv2.boundingRect(anno == id)` (:483-498), tracked while
@@ -176,12 +177,21 @@ class VideoSegmenter:
     def frame(self, frames, annos=None) -> torch.Tensor:
         """Advance every video by one frame.  frames: uint8 [G,H,W,3] (BGR); annos: uint8 [G,H,W] annotation label maps
         of this frame, needed when some object starts here or, when scoring, when the frame lies in some object's
-        scored window.  Returns labels uint8 [G,H,W] on the device."""
+        scored window.  Returns labels uint8 [G,H,W] on the device.  frames may instead be a list of G frames
+        [H_g,W_g,3] of different sizes, with annos a list of G maps [H_g,W_g]; labels are then a list of G uint8
+        [H_g,W_g] views of one packed buffer."""
         f = self.f
-        fr = self.tracker._frames(frames)
-        if fr.dim() != 4 or fr.shape[0] != self.G:
-            raise ValueError(f"frames must be [{self.G},H,W,3]")
-        G, H, W = int(fr.shape[0]), int(fr.shape[1]), int(fr.shape[2])
+        ragged = isinstance(frames, (list, tuple))
+        fr = self.tracker._input(frames) if ragged else self.tracker._frames(frames)
+        if ragged:
+            if len(fr.shapes) != self.G or any(s is None for s in fr.shapes):
+                raise ValueError(f"frames must be a list of {self.G} frames")
+            G = self.G
+            H, W = max(s[0] for s in fr.shapes), max(s[1] for s in fr.shapes)      # the grid of the label kernels
+        else:
+            if fr.dim() != 4 or fr.shape[0] != self.G:
+                raise ValueError(f"frames must be [{self.G},H,W,3]")
+            G, H, W = int(fr.shape[0]), int(fr.shape[1]), int(fr.shape[2])
         kinds = schedule(self._start, self._end, f)
         starting = [k for k in range(len(self.objects)) if kinds[k] == OBJ_INIT]
         scored = None
@@ -193,16 +203,36 @@ class VideoSegmenter:
                 raise ValueError(f"frame {f} is scored: annotation label maps are required")
             if not scored.any():
                 scored = None
+        if ragged and annos is not None:                # host check from shapes alone, before any device work
+            if not isinstance(annos, (list, tuple)) or len(annos) != G:
+                raise ValueError(f"annos must be a list of {G} label maps, one per frame")
+            shp = [None if a is None else tuple(int(v) for v in a.shape) for a in annos]
+            if shp != [tuple(s) for s in fr.shapes]:
+                raise ValueError(f"each anno must be [H_g, W_g] of its frame: {shp} vs {fr.shapes}")
         anno = None
         if starting or scored is not None:
             if annos is None:
                 raise ValueError(f"frame {f}: objects start here, annotation label maps are required")
-            anno = torch.as_tensor(annos).to(self.dev).contiguous()
-            if anno.dtype != torch.uint8 or tuple(anno.shape) != (G, H, W):
-                raise ValueError(f"annos must be uint8 [{G},{H},{W}]")
+            if ragged:
+                if not isinstance(annos, (list, tuple)) or len(annos) != G:
+                    raise ValueError(f"annos must be a list of {G} label maps, one per frame")
+                pa = self.tracker.packer.pack(annos, 1)
+                if pa.shapes != fr.shapes:
+                    raise ValueError(f"each anno must match its frame's size: {pa.shapes} vs {fr.shapes}")
+                anno = pa.data
+            else:
+                anno = torch.as_tensor(annos).to(self.dev).contiguous()
+                if anno.dtype != torch.uint8 or tuple(anno.shape) != (G, H, W):
+                    raise ValueError(f"annos must be uint8 [{G},{H},{W}]")
+        plane = None
+        if ragged:                                      # sm_image_desc of the G label maps (and annotations)
+            desc, ptable = self.tracker.packer.table(fr.shapes, 1)
+            plane = (desc, int(ptable["offset"][-1]) + fr.shapes[-1][0] * fr.shapes[-1][1])
         if starting:
             # init boxes (:494-496): one D2H copy, at init frames only
-            boxes = ops.label_boxes(anno, [(self.objects[k][0], self.objects[k][1]) for k in starting]).cpu().numpy()
+            queries = [(self.objects[k][0], self.objects[k][1]) for k in starting]
+            boxes = (ops._label_boxes_ragged(anno, plane[0], G, queries) if ragged
+                     else ops.label_boxes(anno, queries)).cpu().numpy()
             missing = [self.objects[k][:2] for k, b in zip(starting, boxes) if b[2] == 0]
             if missing:
                 raise ValueError(f"frame {f}: (video, id) {missing} not in the annotation")
@@ -226,11 +256,13 @@ class VideoSegmenter:
             for k, sid in zip(starting, ids):
                 self._sid[k] = sid
         if scored is None:
-            labels = ops._paste_labels(masks, maps, anno, self._offsets, table, (H, W), self.p.seg_thr)
+            labels = ops._paste_labels(masks, maps, anno, self._offsets, table, (H, W), self.p.seg_thr, ragged=plane)
         else:
             labels, _ = ops._paste_labels_iou(masks, maps, anno, self._offsets, table, self._target_ids(scored), (H, W),
-                                              self.p.seg_thr, self._thrs_dev, counts=self._counts[f])
+                                              self.p.seg_thr, self._thrs_dev, counts=self._counts[f], ragged=plane)
         self.f += 1
+        if ragged:
+            return [labels[int(o):int(o) + h * w].view(h, w) for o, (h, w) in zip(ptable["offset"], fr.shapes)]
         return labels
 
     def state(self):

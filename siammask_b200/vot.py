@@ -9,7 +9,8 @@ prediction `cxy_wh_2_rect(target_pos, target_sz)` as the entry.
 
 Here every sequence (x every hyper-parameter combination) is one stream of a `BatchTracker`:
     1. `track(mask=False)` advances all active streams;
-    2. `sm_vot_overlap` scores each stream's clamped-state rectangle against its sequence's ground truth of the frame;
+    2. `sm_vot_overlap` scores each stream's clamped-state rectangle against its sequence's ground truth of the frame
+       (`sm_vot_overlap_sized` with each sequence's own (W, H) when the sequences differ in frame size);
     3. device tensors keep each stream's start frame, entry codes, float64 locations and lost_times, without a host
        sync;
     4. streams whose start frame is this frame are templated again in their own engine slots (`BatchTracker.reinit`);
@@ -20,6 +21,9 @@ pinned memory behind an event, and frame f + 5 reads frame f's flags, which are 
 queues its work without waiting for the device, unless it re-initialises streams or one of its sequences ends: those
 upload small tables (the template rows, the active set) once.
 
+Sequences of different frame sizes run in one batch: pass each frame as a list of G frames (`BatchTracker` packs them;
+the entry of a sequence that has ended may be None).
+
 Mask-mode VOT (the rotated box of tools/test.py:284-303), EAO / accuracy-robustness and the OTB branch are not here.
 """
 from __future__ import annotations
@@ -28,7 +32,7 @@ import numpy as np
 import torch
 
 from . import ops
-from .tracker import BatchTracker, TrackerParams
+from .tracker import BatchTracker, Packed, TrackerParams
 
 # tools/tune_vot.py's argparse defaults: a 9 x 14 x 3 grid of (penalty_k, window_influence, lr)
 DEFAULT_PENALTY_K = np.arange(0.05, 0.5, 0.05)
@@ -93,7 +97,7 @@ def write_result(path, regions) -> None:
 
 
 class VotRunner:
-    """track_vot for G sequences of one frame size on one engine (group a dataset by frame size).  With combos=None
+    """track_vot for G sequences on one engine; their frames may differ in size.  With combos=None
     each sequence is one stream with `params`' hyper-parameters; with combos float64 [K,3] = (penalty_k,
     window_influence, lr) rows (tune_vot's grid is `tune.grid(DEFAULT_PENALTY_K, DEFAULT_WINDOW_INFLUENCE,
     DEFAULT_LR)`, in its nested-loop order) each sequence runs every combination, and stream (g, k) is row g*K + k of
@@ -121,13 +125,19 @@ class VotRunner:
 
     @torch.no_grad()
     def open(self, frames0, gt):
-        """siamese_init of every stream on frame 0.  frames0: uint8 [G,H,W,3] (BGR) frame 0 of each sequence; gt: G
-        float64 arrays [T_g, 8], each sequence's ground-truth polygons (lengths may differ).  Every gt row is checked
-        and uploaded here, once."""
-        fr = self.tracker._frames(frames0)
-        if fr.dim() != 4:
-            raise ValueError("frames0 must be [G,H,W,3]")
-        G, K = int(fr.shape[0]), self.K
+        """siamese_init of every stream on frame 0.  frames0: uint8 [G,H,W,3] (BGR) frame 0 of each sequence, or a list
+        of G frames [H_g,W_g,3] whose sizes may differ; gt: G float64 arrays [T_g, 8], each sequence's ground-truth
+        polygons (lengths may differ).  Every gt row is checked and uploaded here, once."""
+        fr = self.tracker._input(frames0)
+        if isinstance(fr, Packed):
+            if any(s is None for s in fr.shapes):
+                raise ValueError("frames0 must hold frame 0 of every sequence")
+            G, self._hw = len(fr.shapes), list(fr.shapes)
+        else:
+            if fr.dim() != 4:
+                raise ValueError("frames0 must be [G,H,W,3]")
+            G, self._hw = int(fr.shape[0]), [self.tracker._hw(fr)] * int(fr.shape[0])
+        K = self.K
         gts = check_gt(gt)
         if len(gts) != G:
             raise ValueError(f"one gt array per sequence expected ({G})")
@@ -172,6 +182,9 @@ class VotRunner:
         self._row_streams = [self._stream_of[i] for i in self.tracker.ids]
         self._row_dev = torch.tensor(self._row_streams, dtype=torch.long, device=self.dev)
         self._row_video = torch.as_tensor(self._video[self._row_streams], dtype=torch.long, device=self.dev)
+        if len(set(self._hw)) > 1:                      # each row's own (W, H) for sm_vot_overlap_sized
+            wh = [self._hw[self._video[s]][::-1] for s in self._row_streams]
+            self._row_wh = torch.tensor(wh, dtype=torch.int32, device=self.dev).reshape(-1, 2)
 
     def _retire(self):
         """Step 5: streams whose sequence ends with frame self.f leave the batch."""
@@ -182,16 +195,19 @@ class VotRunner:
 
     @torch.no_grad()
     def frame(self, frames):
-        """Frame f (the next one) of every sequence: frames uint8 [G,H,W,3]; the slots of sequences that have ended are
-        not read (any frame of the right size will do).  Returns the tracker's `TrackResult` of the streams that were
-        active, whose rows are skipped or re-initialised streams too."""
+        """Frame f (the next one) of every sequence: frames uint8 [G,H,W,3], or a list of G frames [H_g,W_g,3] in which
+        the entry of a sequence that has ended may be None; the slots of sequences that have ended are not read (any
+        frame of the right size will do).  Returns the tracker's `TrackResult` of the streams that were active, whose
+        rows are skipped or re-initialised streams too."""
         f = self.f
         if self.G == 0 or self.tracker.N == 0:
             raise ValueError("call open() first; every sequence has ended")
-        fr = self.tracker._frames(frames)
-        if fr.dim() != 4 or fr.shape[0] != self.G:
+        fr = self.tracker._input(frames)
+        if isinstance(fr, Packed):
+            if len(fr.shapes) != self.G:
+                raise ValueError(f"frames must be a list of {self.G} frames")
+        elif fr.dim() != 4 or fr.shape[0] != self.G:
             raise ValueError(f"frames must be [{self.G},H,W,3]")
-        H, W = self.tracker.im_h, self.tracker.im_w
         rows = self._row_dev
         # 1. track every active stream (skipped ones too: their outputs are discarded below)
         r = self.tracker.track(fr, mask=False)
@@ -202,7 +218,10 @@ class VotRunner:
         x1, y1 = x0 + st[:, 2], y0 + st[:, 3]
         loc = torch.stack([x0, y0, st[:, 2], st[:, 3]], 1)
         pred = torch.stack([x0, y0, x1, y0, x1, y1, x0, y1], 1).float()
-        ov = ops._vot_overlap(self._gt[self._row_video, f], pred, (H, W))
+        if len(set(self._hw)) > 1:
+            ov = ops._vot_overlap_sized(self._gt[self._row_video, f], pred, self._row_wh)
+        else:
+            ov = ops._vot_overlap(self._gt[self._row_video, f], pred, self._hw[0])
         # 3. bookkeeping on the device: init / track / skip by the stream's start frame; only an overlap of exactly 0
         #    is a failure (NaN is truthy)
         start = self._start[rows]
