@@ -32,12 +32,13 @@ struct ConvGeom {
 enum OutMode : int { OUT_NHWC_SPLIT = 0, OUT_NHWC_F32 = 1, OUT_NCHW_F32 = 2 };
 
 // Epilogue common to the tensor-core GEMM conv and the SIMT reference conv:
-//   v = acc * alpha[c] + beta[c]  (+ residual[m][c])  (relu)  -> out
+//   v = acc * alpha[c] + beta[c]  (+ residual[m][c] * res_scale)  (relu)  -> out
 struct Epilogue {
   const float* alpha = nullptr;   // [Cout] (folded BN scale / pow2 weight de-scaling)
   const float* beta = nullptr;    // [Cout] (folded BN shift or conv bias)
-  const __half* res_hi = nullptr; // residual NHWC [M][Cout], split planes
+  const __half* res_hi = nullptr; // SIMT conv: residual NHWC [M][Cout], split planes (the GEMM takes it as an Act)
   const __half* res_lo = nullptr;
+  float res_scale = 1.f;          // GEMM: power of two that brings the residual to the output's scale, 2^(s_out - s_res)
   __half* out_hi = nullptr;       // OUT_NHWC_SPLIT
   __half* out_lo = nullptr;
   float* out_f32 = nullptr;       // OUT_NHWC_F32 / OUT_NCHW_F32
@@ -56,8 +57,7 @@ constexpr int kStatusBadSlot = 2;
 
 // One K-segment of the implicit GEMM (see conv_gemm_sm90.cu).
 struct GemmSegment {
-  CUtensorMap tmA[2];  // hi / lo plane.  kind 0, mode 0: 2D [M][Cin]; mode 1: im2col over NHWC; kind 1: residual [M][Cout]
-  int kind;            // 0: convolution segment, 1: identity (residual) segment
+  CUtensorMap tmA[2];  // hi / lo plane.  mode 0: 2D [M][Cin]; mode 1: im2col over NHWC
   int mode;
   int num_kb, cblks, KW;
   int stride, pad, dil;
@@ -69,6 +69,9 @@ struct GemmParams {
   GemmSegment seg[2];
   int nseg;
   CUtensorMap tmB[2];   // weights: hi / lo, 2D [Cout_pad][w_ld], K-major
+  CUtensorMap tmO[2];   // NHWC outputs [M][Cout] (TMA stores): hi / lo fp16 plane, or the fp32 tensor in tmO[0]
+  CUtensorMap tmR[2];   // residual [M][Cout] hi / lo fp16 plane (has_res)
+  int has_res;
   int M, Cout, Ho, Wo;
   int n_tiles, m_tiles;
   int reverse_m;        // 1: walk the M tiles from the last to the first (see Engine::conv_into: L2 reuse)
@@ -123,9 +126,9 @@ inline void ensure_dynamic_smem(K kernel, int bytes, unsigned long long& done_ma
 bool gemm_conv_supported(const ConvGeom& g);
 void launch_gemm_conv(const Act& in, const ConvGeom& g, const __half* w_hi, const __half* w_lo, int cout_pad,
                       const Epilogue& ep, int nsplit, int num_sms, cudaStream_t st);
-// General form: 1-2 conv segments accumulating into the same output, optional identity (residual) segment whose
-// diag(2^e) block starts at weight column res_col0 (< 0: none).  w_ld = row length of the weight matrix.
-void launch_gemm_multi(const GemmInput* convs, int nconv, const Act* residual, int res_col0, const __half* w_hi,
+// General form: 1-2 conv segments accumulating into the same output, plus an optional residual (NHWC split output
+// only) added in the epilogue as residual * ep.res_scale.  w_ld = row length of the weight matrix.
+void launch_gemm_multi(const GemmInput* convs, int nconv, const Act* residual, const __half* w_hi,
                        const __half* w_lo, int cout_pad, int w_ld, const Epilogue& ep, int nsplit, int num_sms,
                        cudaStream_t st, bool reverse_m = false);
 

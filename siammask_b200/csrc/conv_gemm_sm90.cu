@@ -6,21 +6,22 @@
 //   tiles (cp.async.bulk.tensor.4d...im2col) for everything else — padding, stride and dilation are resolved
 //   by the TMA unit, out-of-image taps arrive as zeros, and the 128-pixel M tile runs across row and image
 //   boundaries so batch absorbs the odd spatial sizes (31x31, 29x29, 25x25 ...).
-// * W (K-major fp16, [Cout_pad][KH*KW*Cin]) is staged by 2-D TMA tiles.  Both land in 128B-swizzled smem, in a ring
-//   of k-block stages guarded by full / empty mbarriers, and are consumed by wgmma.mma_async (M=64 per warpgroup,
-//   N=BLOCK_N, K=16) accumulating in fp32 registers.
+// * W (K-major fp16, [Cout_pad][KH*KW*Cin]) is staged by 2-D TMA tiles.  Both land in swizzled smem (128 B rows for
+//   64-wide k-blocks, 64 B rows for 32-wide ones, see Cfg), in a ring of k-block stages guarded by full / empty
+//   mbarriers, and are consumed by wgmma.mma_async (M=64 per warpgroup, N=BLOCK_N, K=16) accumulating in fp32
+//   registers.
 // * Precision: NSPLIT=1 multiplies the fp16 hi planes only.  NSPLIT=2 ("exact") keeps activations and
 //   weights as hi+lo fp16 pairs (22 significant bits) and issues three MMAs per k-step
 //   (hi*hi into one accumulator, hi*lo + lo*hi into a second one, summed in the epilogue: the tensor pipe truncates
 //   on every accumulate, so the small cross terms must not be fed into the large running sum) — fp32-class results
 //   from the fp16 tensor pipe.
-// * Epilogue straight from the accumulator registers: acc*alpha[c]+beta[c] (+ residual) (ReLU) -> NHWC split-fp16
-//   planes, NHWC fp32, or NCHW fp32 (the boundary layout of the reference's outputs, tools/test.py:205-206).
-//
-// * K may consist of up to two SEGMENTS that accumulate into the same tile: (conv over input 0) + (conv over
-//   input 1) fuses a bottleneck's downsample branch with its conv3, and an IDENTITY segment
-//   acc += residual * diag(2^e) streams the residual tensor through the same TMA/MMA pipeline (one extra
-//   k-block per 64 output columns) instead of stalling the epilogue on it.
+// * K may consist of up to two segments that accumulate into the same tile: (conv over input 0) + (conv over
+//   input 1) fuses a bottleneck's downsample branch with its conv3.
+// * Epilogue: acc*alpha[c]+beta[c] (+ residual*res_scale) (ReLU).  NHWC outputs (split fp16 planes or fp32) are
+//   written into a per-warpgroup staging buffer in the swizzled layout of 64-row TMA boxes and leave by TMA stores
+//   that overlap the warpgroup's next tile; a residual tile arrives in the same buffer by TMA, loaded by the producer
+//   while the tile's k-blocks run.  NCHW fp32 outputs (the reference's boundary layout, tools/test.py:205-206) are
+//   written straight from the accumulator registers: a 64-row box cannot follow an M tile across the image boundary.
 //
 // Warp roles (384 threads): warpgroup 0 = TMA producer (one elected lane of warp 0; the warpgroup hands most of its
 // registers to the consumers), warpgroups 1 and 2 = consumers, each computing 64 of the tile's 128 rows and writing
@@ -38,7 +39,7 @@ namespace smk {
 namespace {
 
 constexpr int BLOCK_M = 128;
-constexpr int BLOCK_K = 64;     // k-block width in fp16 elements: 128-byte swizzled rows
+constexpr int WG_ROWS = 64;     // tile rows per consumer warpgroup (one staging buffer, one store box row range)
 constexpr int CIN_GRAIN = 64;   // convs need Cin % 64 == 0
 constexpr int MMA_K = 16;
 constexpr int SMEM_LIMIT = 227 * 1024;
@@ -50,16 +51,29 @@ constexpr int CONSUMER_REGS = 232;
 
 template <int BLOCK_N, int NSPLIT>
 struct Cfg {
+  // epilogue staging per consumer warpgroup: 64 rows x BLOCK_N at 4 bytes (fp32, or hi + lo fp16 planes; a residual's
+  // planes arrive in the same bytes)
+  static constexpr int STAGING_BYTES = WG_ROWS * BLOCK_N * 4;
+  static constexpr int RING_BYTES = SMEM_LIMIT - 2048 - 2 * STAGING_BYTES;
+  static constexpr int stage_bytes(int bk) { return NSPLIT * (BLOCK_M + BLOCK_N) * bk * 2; }
+  // 64-wide k-blocks (128 B swizzle) unless fewer than three of them fit beside the staging buffers, which happens in
+  // exact mode at N = 128: there 32-wide k-blocks (64 B swizzle) keep five stages in flight
+  static constexpr int BLOCK_K = RING_BYTES / stage_bytes(64) >= 3 ? 64 : 32;
+  static constexpr int SW = BLOCK_K * 2;                 // operand swizzle span = k-block row in bytes
   static constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;
   static constexpr int B_TILE_BYTES = BLOCK_N * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = NSPLIT * (A_TILE_BYTES + B_TILE_BYTES);
-  static constexpr int RAW_STAGES = (SMEM_LIMIT - 2048) / STAGE_BYTES;
+  static constexpr int RAW_STAGES = RING_BYTES / STAGE_BYTES;
   static constexpr int STAGES = RAW_STAGES > 6 ? 6 : RAW_STAGES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * STAGING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
   static constexpr int ACC = BLOCK_N / 2;               // fp32 accumulator registers per thread and accumulator
-  static_assert(STAGES >= 2, "pipeline needs at least two stages");
+  // store / residual boxes: 64 rows of at most 128 bytes; the swizzle span equals the box row
+  static constexpr int H_BOX = BLOCK_N < 64 ? BLOCK_N : 64;   // fp16 columns per box
+  static constexpr int F_BOX = BLOCK_N < 32 ? BLOCK_N : 32;   // fp32 columns per box
+  static constexpr int H_PLANE = WG_ROWS * BLOCK_N * 2;       // one fp16 plane of a warpgroup's rows
+  static_assert(STAGES >= 3, "pipeline needs at least three stages");
   static_assert(BLOCK_N % 16 == 0 && BLOCK_N >= 16 && BLOCK_N <= 128, "N tile (register accumulators)");
-  static_assert(B_TILE_BYTES % 1024 == 0, "stage parts stay 1024-aligned (swizzle atoms)");
+  static_assert(STAGE_BYTES % 1024 == 0 && B_TILE_BYTES % 1024 == 0, "stage parts stay 1024-aligned (swizzle atoms)");
   static_assert(SMEM_BYTES <= SMEM_LIMIT, "shared memory budget");
 };
 
@@ -70,16 +84,32 @@ __device__ __forceinline__ int m_block(const GemmParams& p, int tile) {
   return p.reverse_m ? p.m_tiles - 1 - mb : mb;
 }
 
+// byte offset inside a TMA box of SPAN-byte rows -> its swizzled smem offset (the box starts 1024-aligned): the 16-byte
+// chunk index is XORed with the row's position in the 1024-byte swizzle atom
+template <int SPAN>
+__device__ __forceinline__ uint32_t swizzle(uint32_t o) {
+  return o ^ (((o >> 7) & (SPAN / 16 - 1)) << 4);
+}
+
+__device__ __forceinline__ void named_barrier_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
 template <int BLOCK_N, int NSPLIT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_gemm_kernel(const __grid_constant__ GemmParams p) {
   using C = Cfg<BLOCK_N, NSPLIT>;
   constexpr int STAGES = C::STAGES;
+  constexpr int BLOCK_K = C::BLOCK_K;
   constexpr int A_TILE_BYTES = C::A_TILE_BYTES;
 
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * C::STAGE_BYTES);
+  // 1024-aligned by pointer arithmetic on smem_raw, so the epilogue's staging accesses stay st/ld.shared
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* staging = smem + STAGES * C::STAGE_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + 2 * C::STAGING_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* free_bar = empty_bar + STAGES;   // [wg]: the warpgroup's previous TMA store has read its staging buffer
+  uint64_t* res_bar = free_bar + 2;          // [wg]: the residual tile has landed in the staging buffer
 
   // warp index through a shuffle: provably warp-uniform for the compiler, so the role branches below are convergent
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
@@ -95,6 +125,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_gemm_kernel(const __grid_
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], NUM_CONSUMER_WARPS);   // one arrival per consumer warp
     }
+    for (int w = 0; w < 2; ++w) {
+      mbar_init(&free_bar[w], 1);
+      mbar_init(&res_bar[w], 1);
+    }
     fence_barrier_init();
   }
   __syncthreads();
@@ -106,14 +140,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_gemm_kernel(const __grid_
     const bool leader = elect_one();
     int stage = 0;
     uint32_t phase = 0;
-    auto acquire = [&](uint32_t bytes) {
-      mbar_wait(&empty_bar[stage], phase ^ 1);
-      if (leader) mbar_arrive_expect_tx(&full_bar[stage], bytes);
-    };
-    auto load_2d = [&](void* dst, const CUtensorMap* map, int c0, int c1) {
-      if (leader) tma_load_2d(dst, map, &full_bar[stage], c0, c1);
-    };
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    uint32_t iter = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++iter) {
       const int m0 = m_block(p, tile) * BLOCK_M;
       const int n0 = (tile % p.n_tiles) * BLOCK_N;
       const int q = m0 % p.Wo;
@@ -122,46 +150,55 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_gemm_kernel(const __grid_
       const int nb = t / p.Ho;
       for (int sgi = 0; sgi < p.nseg; ++sgi) {
         const GemmSegment& sg = p.seg[sgi];
-        if (sg.kind == 1) {
-          // identity segment: A = residual tile [128 rows x 64 cols] (K-major), B = diag(2^e) block (its lo plane is
-          // zero; it is loaded anyway so that every k-block runs the same MMA sequence)
-#pragma unroll 1
-          for (int kb = 0; kb < BLOCK_N / BLOCK_K; ++kb) {
-            acquire(C::STAGE_BYTES);
-            uint8_t* st = smem + stage * C::STAGE_BYTES;
-#pragma unroll
-            for (int s = 0; s < NSPLIT; ++s) {
-              load_2d(st + s * A_TILE_BYTES, &sg.tmA[s], n0 + kb * BLOCK_K, m0);
-              load_2d(st + NSPLIT * A_TILE_BYTES + s * C::B_TILE_BYTES, &p.tmB[s], sg.b_col0 + n0 + kb * BLOCK_K, n0);
-            }
-            __syncwarp();
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-          continue;
-        }
         const int wb = q * sg.stride - sg.pad;
         const int hb = pq * sg.stride - sg.pad;
 #pragma unroll 1
         for (int kb = 0; kb < sg.num_kb; ++kb) {
-          acquire(C::STAGE_BYTES);
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          if (leader) mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
           uint8_t* st = smem + stage * C::STAGE_BYTES;
           const int tap = kb / sg.cblks;
           const int c0 = (kb - tap * sg.cblks) * BLOCK_K;
 #pragma unroll
           for (int s = 0; s < NSPLIT; ++s) {
             uint8_t* a_dst = st + s * A_TILE_BYTES;
-            if (sg.mode == 0) {
-              load_2d(a_dst, &sg.tmA[s], c0, m0);
-            } else if (leader) {
-              const int r = tap / sg.KW;
-              const int sx = tap - r * sg.KW;
-              tma_load_im2col_4d(a_dst, &sg.tmA[s], &full_bar[stage], c0, wb, hb, nb,
-                                 static_cast<uint16_t>(sx * sg.dil), static_cast<uint16_t>(r * sg.dil));
+            if (leader) {
+              if (sg.mode == 0) {
+                tma_load_2d(a_dst, &sg.tmA[s], &full_bar[stage], c0, m0);
+              } else {
+                const int r = tap / sg.KW;
+                const int sx = tap - r * sg.KW;
+                tma_load_im2col_4d(a_dst, &sg.tmA[s], &full_bar[stage], c0, wb, hb, nb,
+                                   static_cast<uint16_t>(sx * sg.dil), static_cast<uint16_t>(r * sg.dil));
+              }
+              tma_load_2d(st + NSPLIT * A_TILE_BYTES + s * C::B_TILE_BYTES, &p.tmB[s], &full_bar[stage],
+                          sg.b_col0 + kb * BLOCK_K, n0);
             }
-            load_2d(st + NSPLIT * A_TILE_BYTES + s * C::B_TILE_BYTES, &p.tmB[s], sg.b_col0 + kb * BLOCK_K, n0);
           }
           __syncwarp();
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+      if (p.has_res) {
+        // the residual tile of each warpgroup, into its staging buffer once the previous tile's store has read it
+        // (the consumers signal that after their first k-block of this tile, which is already in the ring)
+#pragma unroll 1
+        for (int w = 0; w < 2; ++w) {
+          mbar_wait(&free_bar[w], iter & 1);
+          const int r0 = m0 + w * WG_ROWS;
+          if (leader) {
+            mbar_arrive_expect_tx(&res_bar[w], r0 < p.M ? NSPLIT * C::H_PLANE : 0);
+            if (r0 < p.M) {
+              uint8_t* dst = staging + w * C::STAGING_BYTES;
+#pragma unroll
+              for (int s = 0; s < NSPLIT; ++s)
+#pragma unroll
+                for (int b = 0; b < BLOCK_N / C::H_BOX; ++b)
+                  tma_load_2d(dst + s * C::H_PLANE + b * (WG_ROWS * C::H_BOX * 2), &p.tmR[s], &res_bar[w],
+                              n0 + b * C::H_BOX, r0);
+            }
+          }
+          __syncwarp();
         }
       }
     }
@@ -172,29 +209,30 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_gemm_kernel(const __grid_
   setmaxnreg_inc<CONSUMER_REGS>();
   const int wg = (warp >> 2) - 1;
   const int wl = warp & 3;
+  const bool store_thread = wl == 0 && lane == 0;     // issues (and later waits for) the warpgroup's TMA stores
   const Epilogue& ep = p.ep;
   const int HoWo = p.Ho * p.Wo;
+  uint8_t* my_staging = staging + wg * C::STAGING_BYTES;
   float acc[C::ACC];
   float acc2[C::ACC];     // exact mode: the hi*lo + lo*hi cross terms
   int stage = 0;
   uint32_t phase = 0;
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+  uint32_t iter = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++iter) {
 #pragma unroll
     for (int i = 0; i < C::ACC; ++i) { acc[i] = 0.f; acc2[i] = 0.f; }
     int prev = -1;
     for (int sgi = 0; sgi < p.nseg; ++sgi) {
-      const GemmSegment& sg = p.seg[sgi];
-      const bool ident = sg.kind == 1;
-      const int nkb = ident ? BLOCK_N / BLOCK_K : sg.num_kb;
+      const int nkb = p.seg[sgi].num_kb;
 #pragma unroll 1
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        const uint32_t a_hi = smem_u32(smem + stage * C::STAGE_BYTES) + wg * (64 * BLOCK_K * 2);
+        const uint32_t a_hi = smem_u32(smem + stage * C::STAGE_BYTES) + wg * (WG_ROWS * BLOCK_K * 2);
         const uint32_t b_hi = smem_u32(smem + stage * C::STAGE_BYTES) + NSPLIT * A_TILE_BYTES;
-        const uint64_t da_hi0 = wgmma_desc_kmajor<128>(a_hi);
-        const uint64_t db_hi0 = wgmma_desc_kmajor<128>(b_hi);
-        const uint64_t da_lo0 = wgmma_desc_kmajor<128>(a_hi + A_TILE_BYTES);
-        const uint64_t db_lo0 = wgmma_desc_kmajor<128>(b_hi + C::B_TILE_BYTES);
+        const uint64_t da_hi0 = wgmma_desc_kmajor<C::SW>(a_hi);
+        const uint64_t db_hi0 = wgmma_desc_kmajor<C::SW>(b_hi);
+        const uint64_t da_lo0 = wgmma_desc_kmajor<C::SW>(a_hi + A_TILE_BYTES);
+        const uint64_t db_lo0 = wgmma_desc_kmajor<C::SW>(b_hi + C::B_TILE_BYTES);
         // one MMA sequence for every k-block: a data-dependent branch between in-flight wgmma groups makes ptxas
         // insert warpgroup.arrive serialisation around the accumulators
         wgmma_fence();
@@ -213,6 +251,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_gemm_kernel(const __grid_
         if (prev >= 0) {
           __syncwarp();
           if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        } else if (store_thread) {
+          // first k-block of the tile is in flight: by now the previous tile's store has long read the staging buffer
+          tma_store_wait_read<0>();
+          mbar_arrive(&free_bar[wg]);
         }
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -224,19 +266,59 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_gemm_kernel(const __grid_
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[prev]);
 
-    // ---- epilogue: thread holds rows row0, row0 + 8 and column pairs col0 + 8j (see wgmma_f16)
-    const int row0 = m_block(p, tile) * BLOCK_M + wg * 64 + wl * 16 + (lane >> 2);
-    const int col0 = (tile % p.n_tiles) * BLOCK_N + 2 * (lane & 3);
+    // ---- epilogue: thread holds tile rows rl, rl + 8 (of its warpgroup's 64) and column pairs 2 * (lane & 3) + 8j
+    // (see wgmma_f16)
+    const int m0 = m_block(p, tile) * BLOCK_M + wg * WG_ROWS;
+    const int n0 = (tile % p.n_tiles) * BLOCK_N;
+    const int rl = wl * 16 + (lane >> 2);
+    const int cl = 2 * (lane & 3);
+    if (ep.out_mode == OUT_NCHW_F32) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = m0 + rl + 8 * h;
+        if (m >= p.M) continue;
+        const int b = m / HoWo;
+        const int hw = m - b * HoWo;
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int n = n0 + cl + 8 * j;
+          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if constexpr (NSPLIT == 2) {
+            v0 += acc2[4 * j + 2 * h];
+            v1 += acc2[4 * j + 2 * h + 1];
+          }
+          const float2 al = __ldg(reinterpret_cast<const float2*>(ep.alpha + n));
+          const float2 be = __ldg(reinterpret_cast<const float2*>(ep.beta + n));
+          v0 = fmaf(v0, al.x, be.x);
+          v1 = fmaf(v1, al.y, be.y);
+          if (ep.relu) {
+            v0 = fmaxf(v0, 0.f);
+            v1 = fmaxf(v1, 0.f);
+          }
+          if (n < p.Cout) {  // write-once output: stream past L2; the last N tile may be ragged
+            float* dst = ep.out_f32 + (static_cast<size_t>(b) * p.Cout + n) * HoWo + hw;
+            __stcs(dst, v0);
+            if (n + 1 < p.Cout) __stcs(dst + HoWo, v1);
+          }
+        }
+      }
+      continue;
+    }
+
+    // staged NHWC epilogue.  The residual's arrival implies the previous store has read the buffer (the producer
+    // waited for that before loading it); without a residual, wait for that directly.
+    mbar_wait(p.has_res ? &res_bar[wg] : &free_bar[wg], iter & 1);
+    const bool split = ep.out_mode == OUT_NHWC_SPLIT;
+    const bool two_planes = ep.out_lo != nullptr;
     float amax = 0.f;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int m = row0 + 8 * h;
-      if (m >= p.M) continue;
-      const int b = m / HoWo;
-      const int hw = m - b * HoWo;
+      const int r = rl + 8 * h;
+      const bool row_in = m0 + r < p.M;    // rows past M are clipped by the store; they carry beta, keep them out of amax
 #pragma unroll
       for (int j = 0; j < BLOCK_N / 8; ++j) {
-        const int n = col0 + 8 * j;
+        const int c = cl + 8 * j;
+        const int n = n0 + c;
         float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
         if constexpr (NSPLIT == 2) {
           v0 += acc2[4 * j + 2 * h];
@@ -246,39 +328,56 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_gemm_kernel(const __grid_
         const float2 be = __ldg(reinterpret_cast<const float2*>(ep.beta + n));
         v0 = fmaf(v0, al.x, be.x);
         v1 = fmaf(v1, al.y, be.y);
-        const size_t off = static_cast<size_t>(m) * p.Cout + n;
-        if (ep.res_hi != nullptr) {
-          const float2 f = __half22float2(*reinterpret_cast<const __half2*>(ep.res_hi + off));
-          v0 += f.x;
-          v1 += f.y;
-          if (ep.res_lo != nullptr) {
-            const float2 l = __half22float2(*reinterpret_cast<const __half2*>(ep.res_lo + off));
-            v0 += l.x;
-            v1 += l.y;
+        // fp16 planes: box c / H_BOX, 2-byte columns
+        const uint32_t oh = (c / C::H_BOX) * (WG_ROWS * C::H_BOX * 2) +
+                            swizzle<C::H_BOX * 2>(r * (C::H_BOX * 2) + (c % C::H_BOX) * 2);
+        if (p.has_res) {
+          float2 f = __half22float2(*reinterpret_cast<const __half2*>(my_staging + oh));
+          if constexpr (NSPLIT == 2) {
+            const float2 l = __half22float2(*reinterpret_cast<const __half2*>(my_staging + C::H_PLANE + oh));
+            f.x += l.x;
+            f.y += l.y;
           }
+          v0 += f.x * ep.res_scale;
+          v1 += f.y * ep.res_scale;
         }
         if (ep.relu) {
           v0 = fmaxf(v0, 0.f);
           v1 = fmaxf(v1, 0.f);
         }
-        if (ep.out_mode == OUT_NHWC_SPLIT) {
-          amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
+        if (split) {
+          if (row_in) amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
           const __half2 hv = __floats2half2_rn(v0, v1);
           const float2 hf = __half22float2(hv);
-          *reinterpret_cast<__half2*>(ep.out_hi + off) = hv;
-          if (ep.out_lo != nullptr)
-            *reinterpret_cast<__half2*>(ep.out_lo + off) = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
-        } else if (ep.out_mode == OUT_NHWC_F32) {
-          *reinterpret_cast<float2*>(ep.out_f32 + off) = make_float2(v0, v1);
-        } else if (n < p.Cout) {  // OUT_NCHW_F32 (write-once output: stream past L2); the last N tile may be ragged
-          float* dst = ep.out_f32 + (static_cast<size_t>(b) * p.Cout + n) * HoWo + hw;
-          __stcs(dst, v0);
-          if (n + 1 < p.Cout) __stcs(dst + HoWo, v1);
+          *reinterpret_cast<__half2*>(my_staging + oh) = hv;
+          if (two_planes)
+            *reinterpret_cast<__half2*>(my_staging + C::H_PLANE + oh) = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
+        } else {
+          const uint32_t of = (c / C::F_BOX) * (WG_ROWS * C::F_BOX * 4) +
+                              swizzle<C::F_BOX * 4>(r * (C::F_BOX * 4) + (c % C::F_BOX) * 4);
+          *reinterpret_cast<float2*>(my_staging + of) = make_float2(v0, v1);
         }
       }
     }
-    if (ep.out_mode == OUT_NHWC_SPLIT) flag_if_out_of_range(amax, ep.ovf);
+    // generic-proxy writes -> visible to the TMA unit, then one thread stores the warpgroup's boxes
+    fence_proxy_async();
+    named_barrier_sync(1 + wg, 128);
+    if (store_thread && m0 < p.M) {
+      if (split) {
+        for (int s = 0; s < (two_planes ? 2 : 1); ++s)
+#pragma unroll
+          for (int b = 0; b < BLOCK_N / C::H_BOX; ++b)
+            tma_store_2d(&p.tmO[s], my_staging + s * C::H_PLANE + b * (WG_ROWS * C::H_BOX * 2), n0 + b * C::H_BOX, m0);
+      } else {
+#pragma unroll
+        for (int b = 0; b < BLOCK_N / C::F_BOX; ++b)
+          tma_store_2d(&p.tmO[0], my_staging + b * (WG_ROWS * C::F_BOX * 4), n0 + b * C::F_BOX, m0);
+      }
+      tma_store_commit();
+    }
+    if (split) flag_if_out_of_range(amax, ep.ovf);
   }
+  if (store_thread) tma_store_wait_all();
 }
 
 // ------------------------------------------------------------------ host side: tensor maps
@@ -399,18 +498,6 @@ CUtensorMap make_map_im2col(const __half* base, const Act& in, const ConvGeom& g
   return cached_map(k, [&] { return make_map_im2col_raw(base, in, g, bk); });
 }
 
-template <int BLOCK_N, int NSPLIT>
-void launch_cfg(const GemmParams& p, int num_sms, cudaStream_t st) {
-  using C = Cfg<BLOCK_N, NSPLIT>;
-  auto kern = conv_gemm_kernel<BLOCK_N, NSPLIT>;
-  static unsigned long long attr_done = 0;
-  ensure_dynamic_smem(kern, C::SMEM_BYTES, attr_done);
-  const int tiles = p.m_tiles * p.n_tiles;
-  const int grid = tiles < num_sms ? tiles : num_sms;     // one CTA per SM
-  kern<<<grid, NUM_THREADS, C::SMEM_BYTES, st>>>(p);
-  SMK_CUDA(cudaGetLastError());
-}
-
 }  // namespace
 
 // 2-D fp16 tensor map with a chosen swizzle span (32 / 64 / 128 bytes); shared with stem_sm90.cu
@@ -479,22 +566,75 @@ int gemm_cout_pad(int cout) {
   return (cout + 255) / 256 * 256;
 }
 
+// 2-D fp32 tensor map for the epilogue's TMA stores of NHWC fp32 outputs
+static CUtensorMap make_map_2d_f32(const float* base, uint64_t inner, uint64_t outer, uint32_t box_inner,
+                                   uint32_t box_outer, int swizzle_bytes) {
+  MapKey k{};
+  k.v[0] = 6; k.v[1] = (uint64_t)base; k.v[2] = inner; k.v[3] = outer; k.v[4] = box_inner; k.v[5] = box_outer;
+  k.v[6] = (uint64_t)swizzle_bytes;
+  return cached_map(k, [&] {
+    CUtensorMap m;
+    cuuint64_t dims[2] = {inner, outer};
+    cuuint64_t strides[1] = {inner * sizeof(float)};
+    cuuint32_t box[2] = {box_inner, box_outer};
+    cuuint32_t estr[2] = {1, 1};
+    const CUtensorMapSwizzle sw = swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                  : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
+    CUresult r = driver_api().tiled(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides,
+                                    box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    SMK_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (f32) failed, code " + std::to_string((int)r));
+    return m;
+  });
+}
+
+// The k-block width depends on the tile configuration (Cfg::BLOCK_K), so the operand maps and k-block counts are
+// built here, per instantiation.
+template <int BLOCK_N, int NSPLIT>
+static void launch_cfg(GemmParams& p, const GemmInput* convs, const __half* w_hi, const __half* w_lo, int cout_pad,
+                       int w_ld, int num_sms, cudaStream_t st) {
+  using C = Cfg<BLOCK_N, NSPLIT>;
+  constexpr int bk = C::BLOCK_K;
+  for (int i = 0; i < p.nseg; ++i) {
+    const ConvGeom& g = convs[i].g;
+    const Act& in = convs[i].in;
+    GemmSegment& sg = p.seg[i];
+    sg.cblks = g.Cin / bk;
+    sg.num_kb = g.KH * g.KW * sg.cblks;
+    for (int s = 0; s < NSPLIT; ++s) {
+      const __half* a = s == 0 ? in.hi : in.lo;
+      sg.tmA[s] = sg.mode == 0 ? make_map_2d(a, g.Cin, (uint64_t)in.M(), bk, BLOCK_M) : make_map_im2col(a, in, g, bk);
+    }
+    if (NSPLIT == 1) sg.tmA[1] = sg.tmA[0];
+  }
+  if (p.nseg == 1) p.seg[1] = p.seg[0];
+  for (int s = 0; s < NSPLIT; ++s) p.tmB[s] = make_map_2d(s == 0 ? w_hi : w_lo, (uint64_t)w_ld, cout_pad, bk, BLOCK_N);
+  if (NSPLIT == 1) p.tmB[1] = p.tmB[0];
+
+  auto kern = conv_gemm_kernel<BLOCK_N, NSPLIT>;
+  static unsigned long long attr_done = 0;
+  ensure_dynamic_smem(kern, C::SMEM_BYTES, attr_done);
+  const int tiles = p.m_tiles * p.n_tiles;
+  const int grid = tiles < num_sms ? tiles : num_sms;     // one CTA per SM
+  kern<<<grid, NUM_THREADS, C::SMEM_BYTES, st>>>(p);
+  SMK_CUDA(cudaGetLastError());
+}
+
 void launch_gemm_conv(const Act& in, const ConvGeom& g, const __half* w_hi, const __half* w_lo, int cout_pad,
                       const Epilogue& ep, int nsplit, int num_sms, cudaStream_t st) {
   GemmInput gi{in, g, 0};
-  launch_gemm_multi(&gi, 1, nullptr, -1, w_hi, w_lo, cout_pad, g.KH * g.KW * g.Cin, ep, nsplit, num_sms, st);
+  launch_gemm_multi(&gi, 1, nullptr, w_hi, w_lo, cout_pad, g.KH * g.KW * g.Cin, ep, nsplit, num_sms, st);
 }
 
-void launch_gemm_multi(const GemmInput* convs, int nconv, const Act* residual, int res_col0, const __half* w_hi,
-                       const __half* w_lo, int cout_pad, int w_ld, const Epilogue& ep_in, int nsplit, int num_sms,
+void launch_gemm_multi(const GemmInput* convs, int nconv, const Act* residual, const __half* w_hi,
+                       const __half* w_lo, int cout_pad, int w_ld, const Epilogue& ep, int nsplit, int num_sms,
                        cudaStream_t st, bool reverse_m) {
   SMK_CHECK(nconv >= 1 && nconv <= 2, "1 or 2 convolution segments");
-  SMK_CHECK(nconv + (residual != nullptr ? 1 : 0) <= 2, "at most two K segments");
-  Epilogue ep = ep_in;
   const ConvGeom& g0 = convs[0].g;
   const Act& in0 = convs[0].in;
   const int Ho = g0.out_size(in0.H), Wo = g0.out_size(in0.W);
   GemmParams p;
+  std::memset(&p, 0, sizeof p);
   p.M = in0.B * Ho * Wo;
   p.Cout = g0.Cout;
   p.Ho = Ho;
@@ -502,13 +642,12 @@ void launch_gemm_multi(const GemmInput* convs, int nconv, const Act* residual, i
   // Tile: 128 x min(Cout_pad, 128).  The accumulators live in registers (exact mode: two of them, 2 x 64 fp32 per
   // consumer thread at N = 128), which caps the N tile at 128 columns.
   const int block_n = cout_pad < 128 ? cout_pad : 128;
-  const int bk = BLOCK_K;
   SMK_CHECK(cout_pad % block_n == 0, "cout_pad must be a multiple of the N tile");
   if (ep.out_mode != OUT_NCHW_F32) SMK_CHECK(g0.Cout == cout_pad, "NHWC outputs need Cout to match the padded tile width");
   p.n_tiles = cout_pad / block_n;
   p.m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
   p.reverse_m = reverse_m ? 1 : 0;
-  p.nseg = 0;
+  p.nseg = nconv;
   for (int i = 0; i < nconv; ++i) {
     const ConvGeom& g = convs[i].g;
     const Act& in = convs[i].in;
@@ -516,10 +655,7 @@ void launch_gemm_multi(const GemmInput* convs, int nconv, const Act* residual, i
     SMK_CHECK(in.C == g.Cin && g.Cout == g0.Cout && in.B == in0.B, "segment channels/batch mismatch");
     SMK_CHECK(g.out_size(in.H) == Ho && g.out_size(in.W) == Wo, "segments must produce the same output size");
     SMK_CHECK(nsplit == 1 || (in.lo != nullptr && w_lo != nullptr), "exact mode needs lo planes");
-    GemmSegment& sg = p.seg[p.nseg++];
-    sg.kind = 0;
-    sg.cblks = g.Cin / bk;
-    sg.num_kb = g.KH * g.KW * sg.cblks;
+    GemmSegment& sg = p.seg[i];
     sg.KW = g.KW;
     sg.stride = g.stride;
     sg.pad = g.pad;
@@ -527,40 +663,34 @@ void launch_gemm_multi(const GemmInput* convs, int nconv, const Act* residual, i
     sg.mode = (g.KH == 1 && g.KW == 1 && g.stride == 1 && g.pad == 0) ? 0 : 1;
     sg.b_col0 = convs[i].w_col0;
     SMK_CHECK(sg.b_col0 % 64 == 0 && sg.b_col0 + g.KH * g.KW * g.Cin <= w_ld, "weight column range");
-    for (int s = 0; s < nsplit; ++s) {
-      const __half* a = s == 0 ? in.hi : in.lo;
-      sg.tmA[s] = sg.mode == 0 ? make_map_2d(a, g.Cin, (uint64_t)in.M(), bk, BLOCK_M) : make_map_im2col(a, in, g, bk);
-    }
-    if (nsplit == 1) sg.tmA[1] = sg.tmA[0];
+  }
+  // epilogue TMA boxes: 64 rows of min(block_n, 64) fp16 / min(block_n, 32) fp32 columns, swizzle span = box row
+  const uint32_t hbox = block_n < 64 ? block_n : 64, fbox = block_n < 32 ? block_n : 32;
+  auto aligned = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  if (ep.out_mode == OUT_NHWC_SPLIT) {
+    SMK_CHECK(aligned(ep.out_hi) && (ep.out_lo == nullptr || aligned(ep.out_lo)), "NHWC output planes 16-byte aligned");
+    for (int s = 0; s < (ep.out_lo != nullptr ? 2 : 1); ++s)
+      p.tmO[s] = make_map_2d_any(s == 0 ? ep.out_hi : ep.out_lo, (uint64_t)p.Cout, (uint64_t)p.M, hbox, 64, hbox * 2);
+  } else if (ep.out_mode == OUT_NHWC_F32) {
+    SMK_CHECK(aligned(ep.out_f32), "NHWC fp32 output 16-byte aligned");
+    p.tmO[0] = make_map_2d_f32(ep.out_f32, (uint64_t)p.Cout, (uint64_t)p.M, fbox, 64, fbox * 4);
   }
   if (residual != nullptr) {
-    // the residual rides the tensor pipe: needs the diag(2^e) block in the weights and 64-wide column blocks
-    SMK_CHECK(res_col0 >= 0 && res_col0 % 64 == 0 && res_col0 + g0.Cout <= w_ld && block_n % 64 == 0,
-              "identity segment needs a diagonal block in the packed weights");
+    SMK_CHECK(ep.out_mode == OUT_NHWC_SPLIT, "a residual needs an NHWC split-plane output");
     SMK_CHECK(residual->C == g0.Cout && residual->M() == p.M, "residual shape");
     SMK_CHECK(nsplit == 1 || residual->lo != nullptr, "exact mode residual needs both planes");
-    GemmSegment& sg = p.seg[p.nseg++];
-    sg.kind = 1;
-    sg.mode = 0;
-    sg.num_kb = block_n / bk;
-    sg.cblks = sg.KW = sg.stride = sg.dil = 1;
-    sg.pad = 0;
-    sg.b_col0 = res_col0;
+    SMK_CHECK(aligned(residual->hi) && (nsplit == 1 || aligned(residual->lo)), "residual planes 16-byte aligned");
+    p.has_res = 1;
     for (int s = 0; s < nsplit; ++s)
-      sg.tmA[s] = make_map_2d(s == 0 ? residual->hi : residual->lo, g0.Cout, (uint64_t)p.M, bk, BLOCK_M);
-    if (nsplit == 1) sg.tmA[1] = sg.tmA[0];
-    ep.res_hi = ep.res_lo = nullptr;       // accumulated by the MMA, not by the epilogue
+      p.tmR[s] = make_map_2d_any(s == 0 ? residual->hi : residual->lo, (uint64_t)p.Cout, (uint64_t)p.M, hbox, 64,
+                                 hbox * 2);
   }
-  if (p.nseg == 1) p.seg[1] = p.seg[0];
-  for (int s = 0; s < nsplit; ++s)
-    p.tmB[s] = make_map_2d(s == 0 ? w_hi : w_lo, (uint64_t)w_ld, cout_pad, bk, block_n);
-  if (nsplit == 1) p.tmB[1] = p.tmB[0];
   p.ep = ep;
 
-#define SMK_DISPATCH(BN)                                             \
-  case BN:                                                           \
-    if (nsplit == 2) launch_cfg<BN, 2>(p, num_sms, st);              \
-    else launch_cfg<BN, 1>(p, num_sms, st);                          \
+#define SMK_DISPATCH(BN)                                                                         \
+  case BN:                                                                                       \
+    if (nsplit == 2) launch_cfg<BN, 2>(p, convs, w_hi, w_lo, cout_pad, w_ld, num_sms, st);       \
+    else launch_cfg<BN, 1>(p, convs, w_hi, w_lo, cout_pad, w_ld, num_sms, st);                   \
     break;
   switch (block_n) {
     SMK_DISPATCH(16)

@@ -33,12 +33,11 @@ struct ConvW {
   bool gemm_ok = false;
   std::string conv_key, bn_key;       // bn_key empty -> conv has a bias instead
   // tensor-core weight matrix [cout_pad][w_ld]: columns [0,K) this conv, then optionally a second conv whose
-  // output is accumulated into the same tile (the bottleneck's downsample branch, fused with conv3) or a
-  // diag(2^e) block that lets the residual tensor ride the MMA pipeline (identity segment).
+  // output is accumulated into the same tile (the bottleneck's downsample branch, fused with conv3).
   ConvGeom g2{};
   std::string conv_key2, bn_key2;
-  bool fused2 = false, has_diag = false;
-  int w_ld = 0, col2 = 0, col_diag = -1;
+  bool fused2 = false;
+  int w_ld = 0, col2 = 0;
   size_t off_beta2 = 0;
   float* beta2 = nullptr;             // beta of the fused form (sum of both branches' shifts)
   size_t off_whi = 0, off_wlo = 0, off_wref = 0, off_alpha = 0, off_beta = 0;
@@ -446,9 +445,7 @@ void Engine::build_layer_table() {
         c3.g2 = ds.g;
         c3.conv_key2 = ds.conv_key;
         c3.bn_key2 = ds.bn_key;
-      } else {                            // out = relu(bn3(conv3(t)) + x): residual via the identity segment
-        c3.has_diag = true;
-      }
+      }                                   // else out = relu(bn3(conv3(t)) + x): residual added in the GEMM epilogue
       inplanes = sp.planes * 4;
     }
   }
@@ -489,7 +486,6 @@ void Engine::assign_blob_layout() {
     const size_t K = (size_t)w.g.KH * w.g.KW * w.g.Cin;
     w.w_ld = (int)K;
     if (w.fused2) { w.col2 = w.w_ld; w.w_ld += w.g2.KH * w.g2.KW * w.g2.Cin; }
-    if (w.has_diag) { w.col_diag = w.w_ld; w.w_ld += w.g.Cout; }
     if (w.gemm_ok) {
       w.off_whi = off; off = align_up(off + (size_t)w.cout_pad * w.w_ld * sizeof(__half));
       w.off_wlo = off; off = align_up(off + (size_t)w.cout_pad * w.w_ld * sizeof(__half));
@@ -752,12 +748,12 @@ int weight_exp(float amax) {
 }
 }  // namespace
 
-// Step 2: tensor-core operands for the layer's current activation scales.  With inputs stored as a * 2^s_in (a2 * 2^s_in2,
-// r * 2^s_res) the accumulator of output channel n is 2^(e_n + s_in) * sum(w a) when
+// Step 2: tensor-core operands for the layer's current activation scales.  With inputs stored as a * 2^s_in (a2 * 2^s_in2)
+// the accumulator of output channel n is 2^(e_n + s_in) * sum(w a) when
 //   * the first conv's weights are scaled by 2^e_n (per-channel, keeps hi AND lo fp16 parts normal),
-//   * the fused second conv's by 2^(e_n + s_in - s_in2),
-//   * the residual's diag entry is 2^(e_n + s_in - s_res);
-// the epilogue's alpha = 2^(s_out - s_in - e_n) and beta = shift * 2^s_out then store the output at 2^s_out.
+//   * the fused second conv's by 2^(e_n + s_in - s_in2);
+// the epilogue's alpha = 2^(s_out - s_in - e_n) and beta = shift * 2^s_out then store the output at 2^s_out, and a
+// residual stored at 2^s_res is added times res_scale = 2^(s_out - s_res) (conv_into).
 void Engine::quantize_layer(ConvW& L, uint8_t* host) {
   const ConvGeom& g = L.g;
   const size_t K = (size_t)g.KH * g.KW * g.Cin;
@@ -782,15 +778,8 @@ void Engine::quantize_layer(ConvW& L, uint8_t* host) {
     alpha[n] = std::ldexp(1.f, L.s_out - L.s_in);
     if (!L.gemm_ok) continue;
     // per-output-channel power-of-two scaling keeps hi AND lo fp16 parts in the normal range for max |w| down to
-    // ~2^-24 (a clamp at 14 left the planes of a channel whose weights are all below ~2^-14 subnormal).  With a
-    // residual the diag entry 2^(e + s_in - s_res) must itself be a normal fp16, so there e stays within 14 - d and
-    // a channel of such tiny weights keeps subnormal planes.
-    int e = weight_exp(amax);
-    if (L.has_diag) {
-      const int d = L.s_in - L.s_res;
-      e = std::max(-14 - d, std::min(14 - d, e));
-      SMK_CHECK(e >= -24 && e <= 24, "activation scales of a residual block are too far apart");
-    }
+    // ~2^-24 (a clamp at 14 left the planes of a channel whose weights are all below ~2^-14 subnormal)
+    const int e = weight_exp(amax);
     alpha[n] = std::ldexp(1.f, L.s_out - L.s_in - e);
     __half* rh = w_hi + (size_t)n * ld;
     __half* rl = w_lo + (size_t)n * ld;
@@ -806,7 +795,6 @@ void Engine::quantize_layer(ConvW& L, uint8_t* host) {
       rh[L.col2 + k] = h;
       rl[L.col2 + k] = __float2half_rn(fw - __half2float(h));
     }
-    if (L.has_diag) rh[L.col_diag + n] = __float2half_rn(std::ldexp(1.f, e + L.s_in - L.s_res));   // rest stays 0
   }
 }
 
@@ -1091,15 +1079,12 @@ void Engine::conv_into(const Act& in, const ConvW& Lw, Epilogue ep, cudaStream_t
   const bool reverse = !use_patch && end_of(*big) > 0;
   GemmInput gi[2] = {{in, Lw.g, 0}, {in, Lw.g, 0}};
   int nconv = 1;
-  const Act* ident = nullptr;
   if (in2 != nullptr) {
     gi[1] = {*in2, Lw.g2, Lw.col2};
     nconv = 2;
     ep.beta = Lw.beta2;
-  } else if (res != nullptr) {
-    if (Lw.has_diag) ident = res;                                  // residual through the MMA pipeline
-    else { ep.res_hi = res->hi; ep.res_lo = res->lo; }             // epilogue-side add
   }
+  if (res != nullptr) ep.res_scale = std::ldexp(1.f, Lw.s_out - Lw.s_res);   // stored at 2^s_res, output at 2^s_out
   launch(st, 1, Lw.conv_key, "conv_gemm", flops, bytes, [&] {
     const int now_end = reverse ? -1 : +1;
     last_end_[in.hi] = now_end;
@@ -1109,7 +1094,7 @@ void Engine::conv_into(const Act& in, const ConvW& Lw, Epilogue ep, cudaStream_t
     if (use_patch)
       launch_conv3x3_patch(in, Lw.g, Lw.w_hi, Lw.w_lo, Lw.w_ld, ep, exact_ ? 2 : 1, num_sms_, st);
     else
-      launch_gemm_multi(gi, nconv, ident, Lw.col_diag, Lw.w_hi, Lw.w_lo, Lw.cout_pad, Lw.w_ld, ep, exact_ ? 2 : 1,
+      launch_gemm_multi(gi, nconv, res, Lw.w_hi, Lw.w_lo, Lw.cout_pad, Lw.w_ld, ep, exact_ ? 2 : 1,
                         num_sms_, st, reverse);
   });
 }

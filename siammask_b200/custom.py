@@ -170,7 +170,8 @@ class Custom:
 
     # packed-weight file (SURVEY §8f row 4): BN-folded, repacked, fp16-split arena exactly as it sits in HBM, so a
     # fleet of ranks loads (or receives by broadcast) the blob instead of re-folding the 21 M-parameter checkpoint
-    _PACK_MAGIC = b"SMB200PK1"
+    # the version digit moves with the arena layout, so a file of another layout is rejected by name, not by size
+    _PACK_MAGIC = b"SMB200PK2"
 
     def _pack_tag(self) -> bytes:
         return ("%d,%d,%d,%d" % (self.search_size, self.precision, self.anchor_num, int(self.with_mask))).encode()
@@ -187,7 +188,11 @@ class Custom:
         if not self._engine.value:
             raise RuntimeError("call .to(cuda device) first")
         with open(path, "rb") as f:
-            if f.read(len(self._PACK_MAGIC)) != self._PACK_MAGIC:
+            magic = f.read(len(self._PACK_MAGIC))
+            if magic != self._PACK_MAGIC:
+                if magic.startswith(self._PACK_MAGIC[:-1]):
+                    raise ValueError(f"packed-weight file of another arena layout ({magic!r}; this engine reads "
+                                     f"{self._PACK_MAGIC!r}): pack the weights again")
                 raise ValueError("not a siammask_b200 packed-weight file")
             tag = f.read(int.from_bytes(f.read(4), "little"))
             n = int.from_bytes(f.read(8), "little")
