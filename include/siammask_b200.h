@@ -228,6 +228,46 @@ int sm_vot_overlap(const float* poly_a, const float* poly_b, int32_t B, int32_t 
 int sm_vot_overlap_sized(const float* poly_a, const float* poly_b, int32_t B, const int32_t* wh, float* overlap,
                          void* stream);
 
+/* Per-frame overlaps of VOT results as pysot's calculate_accuracy computes them (utils/pysot/utils/statistics.py) for
+ * a result file written by track_vot and read back by load_tracker.  rec: device f64 [>= T][S][5], frame f of stream s
+ * at rec[(f * S + s) * 5] = (entry code, x, y, w, h) with code 1 init, 2 lost, 0 skipped, 3 a location.  gt: device
+ * f32 [G][gt_frames][8] gt polygons; seq: device int32 [S] the sequence g of each stream; wh: device int32 [S][2] the
+ * stream's (W, H); lengths: device int32 [S] the stream's T.
+ * Outputs device f32 [T][S]: acc with bounds (W, H) and burn-in 10 (NaN on the init entry and the 9 frames after it),
+ * eao with bounds (W - 1, H - 1) and no burn-in.  An entry other than a location is NaN (0x7FC00000) in both, as is
+ * every frame f >= lengths[s].  A location passes through the result file first: each value v becomes
+ * rint((double)(float)v * 1e4) / 1e4 (the "%.4f" print and strtod read-back), and the rectangle's vertices x + w, y + h
+ * are summed in double and stored as floats, as pyvotkit's vot_overlap does.  The overlap itself is sm_vot_overlap's
+ * rasteriser, bit for bit, with the location's rectangle as poly_a.
+ * Preconditions (not checked on the device): lengths[s] <= T; 0 <= seq[s] < G; 2 <= W, H and (W+1)*(H+1) fits in
+ * int32; the gt rows and the rounded rectangles inside sm_vot_overlap's coordinate precondition.  2 * T * S <= INT32_MAX. */
+int sm_vot_trajectory_overlap(const double* rec, int32_t T, int32_t S, const float* gt, int32_t gt_frames,
+                              const int32_t* seq, const int32_t* wh, const int32_t* lengths, float* acc, float* eao,
+                              void* stream);
+
+/* Bytes of device workspace sm_vot_eao_accumulate needs for T frames and S streams (0 for bad sizes). */
+size_t sm_vot_eao_workspace_size(int32_t T, int32_t S);
+
+/* Adds S streams' VOT scores (the 'all' tag of pysot's AccuracyRobustnessBenchmark and EAOBenchmark) into R score rows.
+ * eao / acc: the planes of sm_vot_trajectory_overlap, f32 [T][S]; rec: the same record (its entry codes are read);
+ * lengths: device int32 [S]; combo: device int32 [S], the score row of each stream (a row outside [0, R) takes no
+ * stream).  Score state, device f64: num / den [R][cap], tail_in / tail_out [R][2], stats [R][4].
+ *   num[r][i] += sum of fweight * mean(fragment[1..i]) and den[r][i] += sum of fweight over the fragments of row r's
+ *   streams alive at column i (1 <= i < cap), with EAOBenchmark's fragments: for a stream with no lost entry the
+ *   overlaps with their NaNs; otherwise one fragment per start point (0 and f + 5 <= T for every lost entry f), NaN
+ *   read as 0, zero-padded unless it is the last one.  The expected-overlap curve is num / den (0 where den is 0).
+ *   Columns i >= tail_from also receive the non-last fragments of earlier calls: tail_in[r] = (sum of fweight *
+ *   fragment sum, sum of fweight); tail_out = tail_in plus this call's.  Grow cap between calls by copying num / den
+ *   into a wider zeroed buffer and passing the old cap as tail_from; pass tail_from = cap otherwise.
+ *   stats[r] += (sum and count of the non-NaN acc overlaps, number of lost entries, frames) of row r's streams.
+ * Streams are visited in ascending order and every output has one writer, so equal inputs give equal bits.
+ * Preconditions: lengths[s] <= T <= cap; R <= 65535; tail_in and tail_out do not alias; workspace is device memory of
+ * at least sm_vot_eao_workspace_size(T, S) bytes, 8-byte aligned. */
+int sm_vot_eao_accumulate(const float* eao, const float* acc, const double* rec, int32_t T, int32_t S,
+                          const int32_t* lengths, const int32_t* combo, int32_t R, int32_t cap, int32_t tail_from,
+                          const double* tail_in, double* tail_out, double* num, double* den, double* stats,
+                          void* workspace, size_t workspace_bytes, void* stream);
+
 /* Score / box post-processing + argmax of siamese_track — tools/test.py:205-254 — on the device, so that
  * sm_track -> sm_select -> sm_refine needs no host round trip.  All pointers are device pointers:
  * cls/loc as returned by sm_track; anchors f32 [A*R*R][4] = (cx,cy,w,h) in generate_anchor order (tools/test.py:113-129);

@@ -85,6 +85,11 @@ SIGNATURES = {
     "sm_label_boxes": (C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "sm_vot_overlap": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_void_p]),
     "sm_vot_overlap_sized": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sm_vot_trajectory_overlap": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32] +
+                                  [C.c_void_p] * 6),
+    "sm_vot_eao_workspace_size": (C.c_size_t, [C.c_int32, C.c_int32]),
+    "sm_vot_eao_accumulate": (C.c_int, [C.c_void_p] * 3 + [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p] +
+                              [C.c_int32] * 3 + [C.c_void_p] * 6 + [C.c_size_t, C.c_void_p]),
     "sm_crop_resize_ragged": (C.c_int, [C.c_void_p] * 4 + [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "sm_warp_affine_ragged": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 3 + [C.c_int32] * 3 +
                               [C.c_float, C.c_void_p]),

@@ -173,6 +173,15 @@ void launch_label_boxes(const uint8_t* anno, int G, int H, int W, const int32_t*
 // or, with wh (device int32 [B][2]), pair b's own (W, H) = wh[b]
 void launch_vot_overlap(const float* poly_a, const float* poly_b, int B, int W, int H, float* overlap, cudaStream_t st,
                         const int32_t* wh = nullptr);
+// sm_vot_trajectory_overlap / sm_vot_eao_accumulate (include/siammask_b200.h); the workspace of the latter holds
+// vot_eao_workspace_size(T, S) bytes, 8-byte aligned
+void launch_vot_trajectory_overlap(const double* rec, int T, int S, const float* gt, int gt_frames, const int32_t* seq,
+                                   const int32_t* wh, const int32_t* lengths, float* acc, float* eao, cudaStream_t st);
+size_t vot_eao_workspace_size(int T, int S);
+void launch_vot_eao_accumulate(const float* eao, const float* acc, const double* rec, int T, int S,
+                               const int32_t* lengths, const int32_t* combo, int R, int cap, int tail_from,
+                               const double* tail_in, double* tail_out, double* num, double* den, double* stats,
+                               void* workspace, cudaStream_t st);
 void launch_absmax(const Act& a, float* slot, cudaStream_t st);
 void launch_xcorr_nchw_f32(const float* x, const float* k, float* out, int planes, int H, int W, int kh, int kw,
                            cudaStream_t st);

@@ -2104,6 +2104,41 @@ int sm_vot_overlap_sized(const float* poly_a, const float* poly_b, int32_t B, co
   SM_API_END
 }
 
+int sm_vot_trajectory_overlap(const double* rec, int32_t T, int32_t S, const float* gt, int32_t gt_frames,
+                              const int32_t* seq, const int32_t* wh, const int32_t* lengths, float* acc, float* eao,
+                              void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(T >= 1 && S >= 1 && gt_frames >= T, "bad argument");
+  SMK_CHECK(2 * (int64_t)T * S <= INT32_MAX, "2 * T * S must fit in int32 (two blocks per frame and stream)");
+  SMK_CHECK(rec && gt && seq && wh && lengths && acc && eao, "null argument");
+  require_device();
+  smk::launch_vot_trajectory_overlap(rec, T, S, gt, gt_frames, seq, wh, lengths, acc, eao,
+                                     static_cast<cudaStream_t>(stream));
+  SM_API_END
+}
+
+size_t sm_vot_eao_workspace_size(int32_t T, int32_t S) {
+  return T >= 1 && S >= 1 ? smk::vot_eao_workspace_size(T, S) : 0;
+}
+
+int sm_vot_eao_accumulate(const float* eao, const float* acc, const double* rec, int32_t T, int32_t S,
+                          const int32_t* lengths, const int32_t* combo, int32_t R, int32_t cap, int32_t tail_from,
+                          const double* tail_in, double* tail_out, double* num, double* den, double* stats,
+                          void* workspace, size_t workspace_bytes, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(T >= 1 && S >= 1 && R >= 1 && R <= 65535 && cap >= T && tail_from >= 0 && tail_from <= cap,
+            "bad argument");
+  SMK_CHECK(eao && acc && rec && lengths && combo && tail_in && tail_out && num && den && stats && workspace,
+            "null argument");
+  SMK_CHECK(tail_in != tail_out, "tail_in and tail_out must not alias");
+  SMK_CHECK(workspace_bytes >= smk::vot_eao_workspace_size(T, S) && reinterpret_cast<uintptr_t>(workspace) % 8 == 0,
+            "workspace too small or not 8-byte aligned (sm_vot_eao_workspace_size)");
+  require_device();
+  smk::launch_vot_eao_accumulate(eao, acc, rec, T, S, lengths, combo, R, cap, tail_from, tail_in, tail_out, num, den,
+                                 stats, workspace, static_cast<cudaStream_t>(stream));
+  SM_API_END
+}
+
 int sm_warp_affine_ragged(const float* src, int32_t side, const double* maps, float* dst, const sm_image_desc* dst_desc,
                           int32_t B, int32_t max_h, int32_t max_w, float border_value, void* stream) {
   SM_API_BEGIN

@@ -1409,19 +1409,12 @@ __device__ __forceinline__ int vot_row(const float* poly, int pixelY, int width,
   return n;
 }
 
-__global__ void __launch_bounds__(VO_THREADS) vot_overlap_kernel(const float* __restrict__ poly_a,
-                                                                 const float* __restrict__ poly_b, int W, int H,
-                                                                 float* __restrict__ overlap,
-                                                                 const int32_t* __restrict__ wh) {
+// compute_polygon_overlap(pa, pb, bounds (0, 0, W, H)) by the whole block (VO_THREADS threads, all of them call it
+// with the same arguments); the result is valid in thread 0.  The shared arrays are reused by a later call in the same
+// block: every thread has passed this call's last barrier before any thread writes them again.
+__device__ __forceinline__ float vot_polygon_overlap(const float* pa, const float* pb, int W, int H) {
   __shared__ int red[3][VO_THREADS / 32];
   __shared__ float s_poly[2][8];
-  const int p = blockIdx.x;
-  if (wh != nullptr) {                                 // sm_vot_overlap_sized: pair p's own bounds
-    W = wh[2 * p];
-    H = wh[2 * p + 1];
-  }
-  const float* pa = poly_a + 8 * (size_t)p;
-  const float* pb = poly_b + 8 * (size_t)p;
   const VotBounds b1 = vot_bounds(pa, (float)W, (float)H), b2 = vot_bounds(pb, (float)W, (float)H);
   // The two early exits of the C code both return 0 and have no side effect, so they are tested together.  Ratio
   // test: a1 / a2 or a2 / a1 < 1e-10 (float areas, double quotients).  bounds_overlap(b1, b2) == 0: MAX(0, q) is 0
@@ -1435,10 +1428,7 @@ __global__ void __launch_bounds__(VO_THREADS) vot_overlap_kernel(const float* __
   const float x0 = c_min(b1.left, b2.left), y0 = c_min(b1.top, b2.top);
   const int width = (int)__fsub_rn(c_max(b1.right, b2.right), x0) + 1;
   const int height = (int)__fsub_rn(c_max(b1.bottom, b2.bottom), y0) + 1;
-  if (empty || width < 1 || height < 1) {
-    if (threadIdx.x == 0) overlap[p] = 0.f;
-    return;
-  }
+  if (empty || width < 1 || height < 1) return 0.f;
   if (threadIdx.x < 16) {                              // offset_polygon(-x, -y), then round_polygon
     const int k = threadIdx.x & 7;
     s_poly[threadIdx.x >> 3][k] = c_roundf(__fadd_rn((threadIdx.x < 8 ? pa : pb)[k], (k & 1) ? -y0 : -x0));
@@ -1463,11 +1453,206 @@ __global__ void __launch_bounds__(VO_THREADS) vot_overlap_kernel(const float* __
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (lane == 0) { red[0][warp] = n_and; red[1][warp] = n_a; red[2][warp] = n_b; }
   __syncthreads();
+  if (threadIdx.x != 0) return 0.f;
+  int c = 0, ca = 0, cb = 0;
+  for (int w = 0; w < VO_THREADS / 32; ++w) { c += red[0][w]; ca += red[1][w]; cb += red[2][w]; }
+  const int uni = ca + cb - c;                           // mask_1 + mask_2 + mask_intersect
+  return uni == 0 ? __int_as_float(0xFFC00000) : __fdiv_rn(__int2float_rn(c), __int2float_rn(uni));
+}
+
+__global__ void __launch_bounds__(VO_THREADS) vot_overlap_kernel(const float* __restrict__ poly_a,
+                                                                 const float* __restrict__ poly_b, int W, int H,
+                                                                 float* __restrict__ overlap,
+                                                                 const int32_t* __restrict__ wh) {
+  const int p = blockIdx.x;
+  if (wh != nullptr) {                                 // sm_vot_overlap_sized: pair p's own bounds
+    W = wh[2 * p];
+    H = wh[2 * p + 1];
+  }
+  const float v = vot_polygon_overlap(poly_a + 8 * (size_t)p, poly_b + 8 * (size_t)p, W, H);
+  if (threadIdx.x == 0) overlap[p] = v;
+}
+
+// sm_vot_trajectory_overlap: the per-frame overlaps pysot's calculate_accuracy gives for a VOT result file read back by
+// load_tracker.  One block per (frame f, stream s) of the record rec f64 [T][S][5] = (code, x, y, w, h).  A location
+// goes through the result file as float("%.4f" % float32(v)): float32(v) * 1e4 is exact in double (24 + 10 significant
+// bits), printf rounds that exact decimal half to even like rint, and strtod's correctly rounded n / 10^4 is the IEEE
+// quotient.  vot_overlap then builds the rectangle's vertices x + w, y + h in double and stores them as C floats.
+// acc (bounds (W, H)) is NaN on entries other than a location and on the 10 burn-in frames from every init entry;
+// eao (bounds (W-1, H-1)) is NaN on entries other than a location.  Frames f >= lengths[s] are NaN in both.
+__device__ __forceinline__ float entry_nan() { return __int_as_float(0x7FC00000); }   // float("nan") as a C float
+
+__device__ __forceinline__ double vot_result_value(double v) {
+  return __ddiv_rn(rint(__dmul_rn((double)__double2float_rn(v), 1e4)), 1e4);
+}
+
+__global__ void __launch_bounds__(VO_THREADS) vot_trajectory_overlap_kernel(
+    const double* __restrict__ rec, int S, const float* __restrict__ gt, int gt_frames, const int32_t* __restrict__ seq,
+    const int32_t* __restrict__ wh, const int32_t* __restrict__ lengths, float* __restrict__ acc,
+    float* __restrict__ eao) {
+  __shared__ float s_pred[8];
+  const int eao_pass = blockIdx.x & 1;                   // block 2q computes acc[q], block 2q + 1 eao[q]
+  const unsigned q = blockIdx.x >> 1;
+  const int s = (int)(q % (unsigned)S), f = (int)(q / (unsigned)S);
+  const size_t o = (size_t)f * S + s;
+  float* out = eao_pass ? eao : acc;
+  const double* r = rec + 5 * o;
+  bool skip = f >= lengths[s] || (int)r[0] != 3;         // past the end, or an integer entry (init, lost, skip)
+  for (int j = 1; j < 10 && j <= f && !eao_pass; ++j)    // calculate_accuracy's burnin=10 after every init entry
+    skip |= (int)rec[5 * ((size_t)(f - j) * S + s)] == 1;
+  if (skip) {
+    if (threadIdx.x == 0) out[o] = entry_nan();
+    return;
+  }
   if (threadIdx.x == 0) {
-    int c = 0, ca = 0, cb = 0;
-    for (int w = 0; w < VO_THREADS / 32; ++w) { c += red[0][w]; ca += red[1][w]; cb += red[2][w]; }
-    const int uni = ca + cb - c;                         // mask_1 + mask_2 + mask_intersect
-    overlap[p] = uni == 0 ? __int_as_float(0xFFC00000) : __fdiv_rn(__int2float_rn(c), __int2float_rn(uni));
+    const double x = vot_result_value(r[1]), y = vot_result_value(r[2]);
+    const double x1 = __dadd_rn(x, vot_result_value(r[3])), y1 = __dadd_rn(y, vot_result_value(r[4]));
+    s_pred[0] = (float)x;  s_pred[1] = (float)y;  s_pred[2] = (float)x1; s_pred[3] = (float)y;
+    s_pred[4] = (float)x1; s_pred[5] = (float)y1; s_pred[6] = (float)x;  s_pred[7] = (float)y1;
+  }
+  __syncthreads();
+  const float* g = gt + ((size_t)seq[s] * gt_frames + f) * 8;
+  const int W = wh[2 * s], H = wh[2 * s + 1];
+  const float v = vot_polygon_overlap(s_pred, g, W - eao_pass, H - eao_pass);
+  if (threadIdx.x == 0) out[o] = v;
+}
+
+// sm_vot_eao_accumulate, pass 1: one warp per stream.  Its EAO overlaps with NaN as 0 become the prefix sums
+// pre[s][j] = sum of frames < j (double), nanc[s][j] counts the NaN frames < j, and points[s] lists pysot's fragment
+// start points: 0, then f + 5 for every lost entry f with f + 5 <= T.  stat[s] = (sum and count of the non-NaN accuracy
+// overlaps, lost entries, frames).  Warp scans and reductions in a fixed order: the result does not depend on timing.
+constexpr int EP_WARPS = 4;
+
+__global__ void __launch_bounds__(EP_WARPS * 32) vot_eao_prep_kernel(
+    const float* __restrict__ eao, const float* __restrict__ acc, const double* __restrict__ rec, int S, int T,
+    const int32_t* __restrict__ lengths, double* __restrict__ pre, int32_t* __restrict__ nanc,
+    int32_t* __restrict__ points, int32_t* __restrict__ npoints, double* __restrict__ stat) {
+  const int lane = threadIdx.x & 31, s = blockIdx.x * EP_WARPS + (threadIdx.x >> 5);
+  if (s >= S) return;
+  const int Ts = lengths[s];
+  double* P = pre + (size_t)s * (T + 1);
+  int32_t* N = nanc + (size_t)s * (T + 1);
+  int32_t* pts = points + (size_t)s * (T + 1);
+  if (lane == 0) { P[0] = 0.0; N[0] = 0; pts[0] = 0; }
+  double carry = 0.0, asum = 0.0;
+  int ncarry = 0, np = 1, acnt = 0, lost = 0;
+  for (int f0 = 0; f0 < Ts; f0 += 32) {
+    const int f = f0 + lane;
+    const bool in = f < Ts;
+    const float v = in ? eao[(size_t)f * S + s] : 0.f;
+    const bool vn = in && isnan(v);
+    double x = vn ? 0.0 : (double)v;
+    int c = vn;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {                   // inclusive scans
+      const double xo = __shfl_up_sync(0xffffffffu, x, o);
+      const int co = __shfl_up_sync(0xffffffffu, c, o);
+      if (lane >= o) { x = __dadd_rn(x, xo); c += co; }
+    }
+    if (in) { P[f + 1] = __dadd_rn(carry, x); N[f + 1] = ncarry + c; }
+    carry = __dadd_rn(carry, __shfl_sync(0xffffffffu, x, 31));
+    ncarry += __shfl_sync(0xffffffffu, c, 31);
+    const bool is_lost = in && (int)rec[5 * ((size_t)f * S + s)] == 2;
+    lost += is_lost;
+    const unsigned pb = __ballot_sync(0xffffffffu, is_lost && f + 5 <= Ts);
+    if (pb & (1u << lane)) pts[np + __popc(pb & ((1u << lane) - 1u))] = f + 5;
+    np += __popc(pb);
+    const float a = in ? acc[(size_t)f * S + s] : entry_nan();
+    if (!isnan(a)) { asum = __dadd_rn(asum, (double)a); ++acnt; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    asum = __dadd_rn(asum, __shfl_xor_sync(0xffffffffu, asum, o));
+    acnt += __shfl_xor_sync(0xffffffffu, acnt, o);
+    lost += __shfl_xor_sync(0xffffffffu, lost, o);
+  }
+  if (lane == 0) {
+    npoints[s] = np;
+    stat[4 * s] = asum; stat[4 * s + 1] = acnt; stat[4 * s + 2] = lost; stat[4 * s + 3] = Ts;
+  }
+}
+
+// sm_vot_eao_accumulate, pass 2: one block per (column tile, score row r).  Each thread owns column i of row r and
+// adds, over the streams of row r in ascending order and over each stream's fragments in order, pysot's
+// fweight * mean(fragment[1..i]) to num[r][i] and fweight to den[r][i] for every fragment alive at column i:
+//   no lost entry : overlaps[0:T] with its NaNs, alive where overlap i is not NaN; a NaN in 1..i makes the mean NaN;
+//   non-last      : overlaps[p:q+1] with NaN as 0, zero-padded, so alive at every column; weight
+//                   (min(q+1, T) - p) / (q - p + 1), which is below 1 when q == T;
+//   last          : overlaps[p:] with NaN as 0, alive for i < T - p; weight 1.
+// A non-last fragment's value at columns past its end is sum / i, so columns added by a later call that grows cap get
+// sum(w * sum) / i and sum(w) from tail_in (tail_from: the first such column).  tail_out = tail_in plus this call's
+// non-last fragments, and stats[r] += the row's stream stats; both are written by the block of tile 0.  Every value has
+// one writer: the result is the same bits for the same inputs.
+constexpr int EA_THREADS = 128;
+
+__global__ void __launch_bounds__(EA_THREADS) vot_eao_accumulate_kernel(
+    const int32_t* __restrict__ combo, int S, int T, const int32_t* __restrict__ lengths,
+    const double* __restrict__ pre, const int32_t* __restrict__ nanc, const int32_t* __restrict__ points,
+    const int32_t* __restrict__ npoints, const double* __restrict__ stat, int cap, int tail_from,
+    const double* __restrict__ tail_in, double* __restrict__ tail_out, double* __restrict__ num,
+    double* __restrict__ den, double* __restrict__ stats) {
+  __shared__ int s_list[EA_THREADS];
+  __shared__ int s_count[EA_THREADS / 32];
+  const int r = blockIdx.y, i = blockIdx.x * EA_THREADS + threadIdx.x;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const bool col = i >= 1 && i < cap;
+  const bool owner = blockIdx.x == 0 && threadIdx.x == 0;
+  const double di = (double)i;
+  double n = 0.0, d = 0.0, tn = 0.0, tw = 0.0, st[4] = {0.0, 0.0, 0.0, 0.0};
+  if (col && i >= tail_from) { n = __ddiv_rn(tail_in[2 * r], di); d = tail_in[2 * r + 1]; }
+  for (int c0 = 0; c0 < S; c0 += EA_THREADS) {          // this row's streams, compacted in ascending order
+    const bool mine = c0 + threadIdx.x < S && combo[c0 + threadIdx.x] == r;
+    const unsigned b = __ballot_sync(0xffffffffu, mine);
+    if (lane == 0) s_count[warp] = __popc(b);
+    __syncthreads();
+    int base = 0, cnt = 0;
+    for (int w = 0; w < EA_THREADS / 32; ++w) { base += w < warp ? s_count[w] : 0; cnt += s_count[w]; }
+    if (mine) s_list[base + __popc(b & ((1u << lane) - 1u))] = c0 + threadIdx.x;
+    __syncthreads();
+    for (int k = 0; k < cnt; ++k) {
+      const int s = s_list[k], Ts = lengths[s];
+      const double* P = pre + (size_t)s * (T + 1);
+      if (owner)
+        for (int j = 0; j < 4; ++j) st[j] = __dadd_rn(st[j], stat[4 * s + j]);
+      if (stat[4 * s + 2] == 0.0) {                      // no lost entry: the overlaps with their NaNs
+        const int32_t* N = nanc + (size_t)s * (T + 1);
+        if (col && i < Ts && N[i + 1] == N[i]) {
+          n = __dadd_rn(n, N[i] != N[1] ? __longlong_as_double(0x7ff8000000000000LL)
+                                         : __ddiv_rn(__dsub_rn(P[i + 1], P[1]), di));
+          d = __dadd_rn(d, 1.0);
+        }
+        continue;
+      }
+      const int32_t* pts = points + (size_t)s * (T + 1);
+      const int np = npoints[s];
+      for (int j = 0; j < np; ++j) {
+        const int p = pts[j];
+        if (j + 1 < np) {
+          const int q = pts[j + 1], end = min(q, Ts - 1);
+          const double w = __ddiv_rn((double)(min(q + 1, Ts) - p), (double)(q - p + 1));
+          if (col) {
+            const int m = min(i, end - p);
+            n = __dadd_rn(n, __dmul_rn(__ddiv_rn(__dsub_rn(P[p + m + 1], P[p + 1]), di), w));
+            d = __dadd_rn(d, w);
+          }
+          tn = __dadd_rn(tn, __dmul_rn(w, __dsub_rn(P[end + 1], P[p + 1])));
+          tw = __dadd_rn(tw, w);
+        } else if (col && i < Ts - p) {
+          n = __dadd_rn(n, __ddiv_rn(__dsub_rn(P[p + i + 1], P[p + 1]), di));
+          d = __dadd_rn(d, 1.0);
+        }
+      }
+    }
+    __syncthreads();
+  }
+  if (col) {
+    num[(size_t)r * cap + i] = __dadd_rn(num[(size_t)r * cap + i], n);
+    den[(size_t)r * cap + i] = __dadd_rn(den[(size_t)r * cap + i], d);
+  }
+  if (owner) {
+    tail_out[2 * r] = __dadd_rn(tail_in[2 * r], tn);
+    tail_out[2 * r + 1] = __dadd_rn(tail_in[2 * r + 1], tw);
+    for (int j = 0; j < 4; ++j) stats[4 * r + j] = __dadd_rn(stats[4 * r + j], st[j]);
   }
 }
 
@@ -1891,6 +2076,35 @@ void launch_label_boxes(const uint8_t* anno, int G, int H, int W, const int32_t*
 void launch_vot_overlap(const float* poly_a, const float* poly_b, int B, int W, int H, float* overlap, cudaStream_t st,
                         const int32_t* wh) {
   vot_overlap_kernel<<<B, VO_THREADS, 0, st>>>(poly_a, poly_b, W, H, overlap, wh);
+  SMK_CUDA(cudaGetLastError());
+}
+
+void launch_vot_trajectory_overlap(const double* rec, int T, int S, const float* gt, int gt_frames, const int32_t* seq,
+                                   const int32_t* wh, const int32_t* lengths, float* acc, float* eao, cudaStream_t st) {
+  vot_trajectory_overlap_kernel<<<2u * (unsigned)T * (unsigned)S, VO_THREADS, 0, st>>>(rec, S, gt, gt_frames, seq, wh,
+                                                                                  lengths, acc, eao);
+  SMK_CUDA(cudaGetLastError());
+}
+
+size_t vot_eao_workspace_size(int T, int S) {
+  return (size_t)S * (T + 1) * (sizeof(double) + 2 * sizeof(int32_t)) + (size_t)S * (4 * sizeof(double) + sizeof(int32_t));
+}
+
+void launch_vot_eao_accumulate(const float* eao, const float* acc, const double* rec, int T, int S,
+                               const int32_t* lengths, const int32_t* combo, int R, int cap, int tail_from,
+                               const double* tail_in, double* tail_out, double* num, double* den, double* stats,
+                               void* workspace, cudaStream_t st) {
+  double* pre = static_cast<double*>(workspace);                         // [S][T+1]
+  double* stat = pre + (size_t)S * (T + 1);                               // [S][4]
+  int32_t* nanc = reinterpret_cast<int32_t*>(stat + (size_t)S * 4);       // [S][T+1]
+  int32_t* points = nanc + (size_t)S * (T + 1);                           // [S][T+1]
+  int32_t* npoints = points + (size_t)S * (T + 1);                        // [S]
+  vot_eao_prep_kernel<<<(S + EP_WARPS - 1) / EP_WARPS, EP_WARPS * 32, 0, st>>>(eao, acc, rec, S, T, lengths, pre, nanc,
+                                                                                points, npoints, stat);
+  SMK_CUDA(cudaGetLastError());
+  const dim3 grid((cap + EA_THREADS - 1) / EA_THREADS, R);
+  vot_eao_accumulate_kernel<<<grid, EA_THREADS, 0, st>>>(combo, S, T, lengths, pre, nanc, points, npoints, stat, cap,
+                                                         tail_from, tail_in, tail_out, num, den, stats);
   SMK_CUDA(cudaGetLastError());
 }
 

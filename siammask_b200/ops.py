@@ -436,3 +436,36 @@ def _vot_overlap_sized(poly_a, poly_b, wh, out=None) -> torch.Tensor:
         _lib.check(lib.sm_vot_overlap_sized(poly_a.data_ptr(), poly_b.data_ptr(), B, wh.contiguous().data_ptr(),
                                             out.data_ptr(), _stream(dev)))
     return out
+
+
+def _vot_trajectory_overlap(rec, T: int, S: int, gt, seq, wh, lengths):
+    """C ABI `sm_vot_trajectory_overlap` without host-side checks: rec float64 CUDA [>= T, S, 5] (a `VotRunner` record),
+    gt float32 CUDA [G, >= T, 8], seq / lengths int32 CUDA [S], wh int32 CUDA [S, 2] = (W, H), all inside the
+    precondition.  Returns (acc, eao) float32 [T, S]: pysot's per-frame overlaps with bounds (W, H) and burn-in 10, and
+    with bounds (W-1, H-1)."""
+    lib = _lib.load()
+    dev = rec.device
+    acc = torch.empty(T, S, dtype=torch.float32, device=dev)
+    eao = torch.empty(T, S, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.sm_vot_trajectory_overlap(rec.data_ptr(), T, S, gt.data_ptr(), int(gt.shape[1]), seq.data_ptr(),
+                                                 wh.data_ptr(), lengths.data_ptr(), acc.data_ptr(), eao.data_ptr(),
+                                                 _stream(dev)))
+    return acc, eao
+
+
+def _vot_eao_accumulate(eao, acc, rec, lengths, combo, tail_from, tail_in, tail_out, num, den, stats):
+    """C ABI `sm_vot_eao_accumulate` without host-side checks: adds the streams of the planes eao / acc float32 CUDA
+    [T, S] into the score rows combo[s] of num / den float64 [R, cap], tail_out float64 [R, 2] (from tail_in) and stats
+    float64 [R, 4].  The workspace comes from torch's caching allocator."""
+    lib = _lib.load()
+    dev = eao.device
+    T, S = int(eao.shape[0]), int(eao.shape[1])
+    R, cap = int(num.shape[0]), int(num.shape[1])
+    nbytes = int(lib.sm_vot_eao_workspace_size(T, S))
+    ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.sm_vot_eao_accumulate(eao.data_ptr(), acc.data_ptr(), rec.data_ptr(), T, S, lengths.data_ptr(),
+                                             combo.data_ptr(), R, cap, int(tail_from), tail_in.data_ptr(),
+                                             tail_out.data_ptr(), num.data_ptr(), den.data_ptr(), stats.data_ptr(),
+                                             ws.data_ptr(), ws.numel() * 8, _stream(dev)))

@@ -24,7 +24,18 @@ upload small tables (the template rows, the active set) once.
 Sequences of different frame sizes run in one batch: pass each frame as a list of G frames (`BatchTracker` packs them;
 the entry of a sequence that has ended may be None).
 
-Mask-mode VOT (the rotated box of tools/test.py:284-303), EAO / accuracy-robustness and the OTB branch are not here.
+`VotScore` scores finished runs the way tools/eval.py does for VOT2016/2017/2018/2019 ('all' tag): pysot's
+AccuracyRobustnessBenchmark (accuracy, robustness, lost number) and EAOBenchmark (expected-overlap curve and EAO), for
+every hyper-parameter combination at once, from the runner's device record and without result files:
+    1. `sm_vot_trajectory_overlap` reads each frame's entry as load_tracker would read it back from the result file
+       ("%.4f" of the float32 value) and computes both per-frame overlaps: bounds (W, H) with burn-in 10 for accuracy,
+       bounds (W-1, H-1) for EAO;
+    2. `sm_vot_eao_accumulate` turns them into per-combination float64 sums: accuracy sum and count, lost entries and
+       frames, and the numerator / denominator of every column of the expected-overlap curve over the fragments pysot
+       cuts at each failure.  A column's sums depend only on its index, so runs of any split of the dataset (by
+       sequence or by combination) add up; the curve is read out up to the longest sequence added.
+
+Mask-mode VOT (the rotated box of tools/test.py:284-303), per-attribute EAO tags and the OTB branch are not here.
 """
 from __future__ import annotations
 
@@ -264,3 +275,149 @@ class VotRunner:
         regions = [[regions_from_record(rec[:, g * K + k], int(n[g])) for k in range(K)] for g in range(G)]
         return regions, rec[-1, :, 0].astype(np.int64).reshape(G, K)
 
+
+
+# EAOBenchmark's (low, high) per dataset (utils/pysot/evaluation/eao_benchmark.py): EAO averages curve[low-1 .. high-1]
+EAO_BOUNDS = {"VOT2016": (100, 356), "VOT2017": (100, 356), "VOT2018": (100, 356), "VOT2019": (46, 291)}
+
+
+class VotScore:
+    """tools/eval.py's VOT numbers ('all' tag) for `num_combos` hyper-parameter combinations, accumulated on the device.
+
+        score = VotScore(K, dataset="VOT2018")          # or low=, high= for other EAO bounds
+        score.add(runner)                                # a finished VotRunner; combo_index maps its k to score rows
+        r = score.result()                               # accuracy, robustness, lost_number, eao, expected_overlaps
+
+    Every combination's row gathers all sequences added to it; add() may be called per batch of sequences or per chunk
+    of the grid.  Sequences must be at least 2 x 2 pixels (EAO scores them with bounds (W-1, H-1))."""
+
+    def __init__(self, num_combos: int, dataset: str | None = "VOT2018", low: int | None = None,
+                 high: int | None = None, device=None):
+        K = int(num_combos)
+        if not 1 <= K <= 65535:
+            raise ValueError(f"num_combos must be in [1, 65535], got {num_combos}")
+        if low is None and high is None:
+            if dataset not in EAO_BOUNDS:
+                raise ValueError(f"unknown dataset {dataset!r}: pass low= and high= (known: {sorted(EAO_BOUNDS)})")
+            low, high = EAO_BOUNDS[dataset]
+        elif low is None or high is None or not 1 <= int(low) <= int(high):
+            raise ValueError(f"EAO bounds need 1 <= low <= high, got low={low}, high={high}")
+        self.K, self.low, self.high = K, int(low), int(high)
+        self.dev = torch.device(device if device is not None else "cuda")
+        z = lambda *shape: torch.zeros(*shape, dtype=torch.float64, device=self.dev)      # noqa: E731
+        self._num, self._den = z(K, 0), z(K, 0)
+        self._tail, self._tail_next = z(K, 2), z(K, 2)
+        self._stats = z(K, 4)                       # accuracy sum, accuracy count, lost entries, frames
+        self._sequences = np.zeros(K, np.int64)
+
+    @property
+    def cap(self) -> int:
+        return int(self._num.shape[1])
+
+    def _rows(self, combo_index, K: int) -> np.ndarray:
+        ci = np.arange(K) if combo_index is None else np.asarray(combo_index)
+        if ci.shape != (K,) or not np.issubdtype(ci.dtype, np.integer):
+            raise ValueError(f"combo_index must be {K} integers (one score row per combination of the run)")
+        if (ci < 0).any() or (ci >= self.K).any():
+            raise ValueError(f"combo_index entries must lie in [0, {self.K})")
+        if len(set(ci.tolist())) != K:
+            raise ValueError("combo_index entries must be distinct")
+        return ci.astype(np.int64)
+
+    @torch.no_grad()
+    def add(self, runner: VotRunner, combo_index=None):
+        """Adds every stream of a VotRunner whose sequences have all ended: stream (g, k) goes to score row
+        combo_index[k] (default k).  Reads the runner's device record in place; no host sync."""
+        if runner.G == 0:
+            raise ValueError("the runner has not been opened")
+        if (runner.T > runner.f).any():
+            raise ValueError(f"every sequence must have ended: frame {runner.f} of lengths {runner.T.tolist()}")
+        sizes = [(int(h), int(w)) for h, w in runner._hw]
+        self._add(runner._rec, runner._gt, runner.T, sizes, runner.K, combo_index)
+        return self
+
+    @torch.no_grad()
+    def add_regions(self, regions, gt, sizes, combo_index=None):
+        """Adds trajectories in the form `VotRunner.result()` returns: regions[g][k] is the list of sequence g under
+        combination k (1 init, 2 lost, 0 skipped, or a location x, y, w, h), gt[g] its float64 [T_g, 8] polygons and
+        sizes[g] its frame (H, W).  Every list must have T_g entries."""
+        gts = check_gt(gt)
+        G = len(gts)
+        if len(regions) != G or len(sizes) != G or G == 0:
+            raise ValueError("regions, gt and sizes need one entry per sequence")
+        K = len(regions[0])
+        if K == 0 or any(len(r) != K for r in regions):
+            raise ValueError("every sequence needs the same number of combinations")
+        T = np.array([len(a) for a in gts])
+        Tmax = int(T.max())
+        rec = np.zeros((Tmax, G * K, 5))
+        for g in range(G):
+            for k in range(K):
+                traj = regions[g][k]
+                if len(traj) != T[g]:
+                    raise ValueError(f"regions[{g}][{k}] has {len(traj)} entries, the sequence {T[g]} frames")
+                for f, x in enumerate(traj):
+                    if isinstance(x, (int, np.integer)):
+                        if x not in (CODE_SKIP, CODE_INIT, CODE_LOST):
+                            raise ValueError(f"regions[{g}][{k}][{f}]: integer entries are 0, 1 or 2")
+                        rec[f, g * K + k, 0] = x
+                    else:
+                        loc = np.asarray(x, np.float64).reshape(-1)
+                        if loc.size != 4 or not np.isfinite(loc).all():
+                            raise ValueError(f"regions[{g}][{k}][{f}]: a location is 4 finite values")
+                        rec[f, g * K + k] = (CODE_LOCATION, *loc)
+        locs = rec[..., 1:]
+        if (np.abs(locs[..., :2]) + np.abs(locs[..., 2:]) > ops.VOT_COORD_LIMIT / 2).any():
+            raise ValueError("locations must lie within +-2^19 px")
+        polys = np.zeros((G, Tmax, 8), np.float32)
+        for g, a in enumerate(gts):
+            polys[g, :len(a)] = a
+        self._add(torch.from_numpy(rec).to(self.dev), torch.from_numpy(polys).to(self.dev), T,
+                  [(int(h), int(w)) for h, w in sizes], K, combo_index)
+        return self
+
+    def _add(self, rec, gt, T, sizes, K, combo_index):
+        rows = self._rows(combo_index, K)
+        G = len(T)
+        wh = np.array([(w, h) for h, w in sizes], np.int64)
+        if (wh < 2).any() or ((wh[:, 0] + 1) * (wh[:, 1] + 1) > 2 ** 31 - 1).any():
+            raise ValueError("frames must be at least 2 x 2 px (EAO uses bounds (W-1, H-1)) and (W+1)*(H+1) < 2^31")
+        Tmax, S = int(np.max(T)), G * K
+        if 2 * Tmax * S > 2 ** 31 - 1:
+            raise ValueError(f"{S} streams x {Tmax} frames is too large for one add(); add the run in parts")
+        if self.dev.type != "cuda":
+            raise RuntimeError("VotScore runs on a CUDA device only; there is no CPU path")
+        seq = np.repeat(np.arange(G), K)
+        table = np.concatenate([seq, np.asarray(T)[seq], np.tile(rows, G), wh[seq].ravel()]).astype(np.int32)
+        t = torch.from_numpy(table).to(self.dev)                       # one upload: seq, lengths, combo, (W, H)
+        seq_d, len_d, combo_d, wh_d = t[:S], t[S:2 * S], t[2 * S:3 * S], t[3 * S:]
+        with torch.cuda.device(self.dev):
+            acc, eao = ops._vot_trajectory_overlap(rec, Tmax, S, gt, seq_d, wh_d, len_d)
+            old = self.cap
+            if Tmax > old:                                             # grow: earlier fragments reach the new columns
+                num = torch.zeros(self.K, Tmax, dtype=torch.float64, device=self.dev)
+                den = torch.zeros_like(num)
+                num[:, :old], den[:, :old] = self._num, self._den
+                self._num, self._den = num, den
+            ops._vot_eao_accumulate(eao, acc, rec, len_d, combo_d, old, self._tail, self._tail_next, self._num,
+                                    self._den, self._stats)
+        self._tail, self._tail_next = self._tail_next, self._tail
+        self._sequences[rows] += G
+
+    def result(self) -> dict:
+        """One D2H copy.  Per combination (arrays [K]): accuracy (nan-mean of the burn-in overlaps), robustness (lost
+        entries per 100 frames), lost_number, eao, and expected_overlaps float32 [K, max_T] (the curve, entry 0 = 1);
+        sequences: how many sequences each row has gathered.  Rows without sequences are NaN."""
+        cap = self.cap
+        h = torch.cat([self._num, self._den, self._stats], 1).cpu().numpy()
+        num, den, st = h[:, :cap], h[:, cap:2 * cap], h[:, 2 * cap:]
+        with np.errstate(divide="ignore", invalid="ignore"):
+            curve = np.where(den > 0, num / np.where(den > 0, den, 1), 0.0).astype(np.float32)
+            if cap:
+                curve[:, 0] = 1
+            seg = curve[:, self.low - 1:min(self.high, cap)].astype(np.float64)
+            valid = ~np.isnan(seg)
+            eao = np.where(valid, seg, 0.0).sum(1) / valid.sum(1)
+            return {"accuracy": st[:, 0] / st[:, 1], "robustness": st[:, 2] / st[:, 3] * 100,
+                    "lost_number": st[:, 2].astype(np.int64), "eao": eao, "expected_overlaps": curve,
+                    "sequences": self._sequences.copy()}
