@@ -287,21 +287,19 @@ def _label_boxes_ragged(anno: torch.Tensor, desc: torch.Tensor, G: int, queries)
     return out
 
 
-def _crop_resize_ragged(frames: torch.Tensor, desc: torch.Tensor, frame_idx, boxes, model_size: int) -> torch.Tensor:
+def _crop_resize_ragged(frames: torch.Tensor, desc: torch.Tensor, frame_idx: torch.Tensor, boxes: torch.Tensor,
+                        model_size: int) -> torch.Tensor:
     """`crop_resize` over a packed uint8 CUDA frame buffer (C ABI `sm_crop_resize_ragged`): stream b crops frame
-    desc[frame_idx[b]]; boxes int [B,6] as in `crop_resize`.  No host-side checks."""
+    desc[frame_idx[b]]; frame_idx int32 CUDA [B]; boxes int32 CUDA [B,8] whose first 6 columns are `crop_resize`'s
+    boxes.  No host-side checks and no host staging."""
     lib = _lib.load()
     dev = frames.device
-    bx = torch.as_tensor(boxes, dtype=torch.int32).reshape(-1, 6)
-    B = bx.shape[0]
-    full = torch.zeros(B, 8, dtype=torch.int32)
-    full[:, :6] = bx
-    full = full.to(dev)
-    idx = torch.as_tensor(frame_idx, dtype=torch.int32).reshape(-1).to(dev).contiguous()
+    B = int(boxes.shape[0])
     out = torch.empty(B, 3, model_size, model_size, device=dev, dtype=torch.float32)
     with torch.cuda.device(dev):
-        _lib.check(lib.sm_crop_resize_ragged(frames.contiguous().data_ptr(), desc.data_ptr(), idx.data_ptr(),
-                                             full.data_ptr(), B, model_size, out.data_ptr(), _stream(dev)))
+        _lib.check(lib.sm_crop_resize_ragged(frames.contiguous().data_ptr(), desc.data_ptr(),
+                                             frame_idx.contiguous().data_ptr(), boxes.contiguous().data_ptr(), B,
+                                             model_size, out.data_ptr(), _stream(dev)))
     return out
 
 

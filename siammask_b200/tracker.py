@@ -6,10 +6,10 @@ arithmetic, crop + resize, score/box post-processing + argmax, learning-rate upd
 mask paste-back — runs here as a fixed sequence of kernels over all streams (C ABI in include/siammask_b200.h):
 
     sm_tracker_prepare      state -> crop boxes, target size in the crop, scale          (tools/test.py:180-198, 71-76)
-    sm_crop_resize_indexed  uint8 frames -> f32 [N,3,S,S] search crops (cv2-exact)        (:67-110)
+    sm_crop_resize_ragged   uint8 frames -> f32 [N,3,S,S] search crops (cv2-exact)        (:67-110)
     sm_step_slots_hp        track_mask -> select -> track_refine                          (:201-261)
     sm_tracker_update_hp    winner box + score -> new state (lr, clamps), paste-back map  (:239-249, 263-282, 305-315)
-    sm_warp_affine          127x127 sigmoid mask -> frame, threshold                      (:263-284)
+    sm_warp_affine_ragged   127x127 sigmoid mask -> frame, threshold                      (:263-284)
 
 The state (target_pos, target_sz, float64) lives on the device; a frame costs one small D2H copy only if the caller
 asks for the numbers (`TrackResult.cpu()`).  Contour extraction / minAreaRect (:285-303) is not part of this module.
@@ -17,17 +17,19 @@ asks for the numbers (`TrackResult.cpu()`).  Contour extraction / minAreaRect (:
 Streams join and leave a running tracker: `add` templates new streams into free engine slots, `remove` frees them.  The
 active streams are kept as compact rows (state, slot, frame index, hyper-parameters), and every frame runs exactly those
 rows as one batch through the slot table and the per-stream (penalty_k, window_influence, lr) table
-(`sm_step_slots_hp`, `sm_tracker_update_hp`) and the frame-index table (`sm_crop_resize_indexed`); the tables are
+(`sm_step_slots_hp`, `sm_tracker_update_hp`) and the frame-index table (`sm_crop_resize_ragged`); the tables are
 uploaded only when the set changes.  A stream's hyper-parameters default to the tracker's `TrackerParams`.  Each stream
-reads one frame of the tensor passed to `track`: its frame index, set by `add` (for `init`, stream i reads frame i; a
+reads one frame of the frames passed to `track`: its frame index, set by `add` (for `init`, stream i reads frame i; a
 single [H,W,3] frame is shared by all streams).  `add_state` starts streams from the centre form siamese_init receives
 (target_pos, target_sz), and `reinit` runs siamese_init again for running streams in their own slots (the VOT
 protocol's restart after a failure) without changing the active set; all three template through `_template`.
 
-Frames of different sizes run in one batch: a list of frames (numpy arrays or CUDA tensors, any mix of sizes) is packed
-by `FramePacker` into one device buffer plus an `sm_image_desc` table (offset, h, w per frame), and the crop and the
-paste-back read each stream's own frame from it (`sm_crop_resize_ragged`, `sm_warp_affine_ragged`).  A stream is bound
-to the size of the frame it was added from; the per-stream (W, H) table that the state update clamps against holds it.
+The frames of a call always reach the kernels as a `Packed`: one device buffer plus an `sm_image_desc` table (offset,
+h, w per frame), from which the crop and the paste-back read each stream's own frame.  A list of frames (numpy arrays
+or CUDA tensors, any mix of sizes) is packed by `FramePacker.pack`; a [F,H,W,3] array or tensor (and a shared [H,W,3]
+frame) is wrapped by `FramePacker.wrap` without a copy, under a table that is uploaded only when the shape changes.
+Frames of different sizes therefore run in one batch.  A stream is bound to the size of the frame it was added from;
+the per-stream (W, H) table that the state update clamps against holds it.
 
 The arithmetic is pinned by `tests/test_batch_tracker.py` to the reference loop's golden trajectory and to
 single-stream runs of the host restatement in `oracle/ref_loop.py`.
@@ -40,7 +42,7 @@ from dataclasses import dataclass, field
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, ops
 from .anchors import cosine_window, generate_anchor
 
 
@@ -105,21 +107,28 @@ class Packed:
 
 class FramePacker:
     """Packs lists of images that differ in size (uint8 numpy arrays or CUDA tensors, [h,w,3] frames or [h,w] label
-    maps) into one device buffer plus an sm_image_desc table.  The table depends only on the sequence of shapes and is
-    uploaded only when that changes, asynchronously from pinned memory, so packing never waits for the device.  Host
-    arrays are concatenated on the host and copied in one transfer; CUDA tensors are concatenated on the device."""
+    maps) into one device buffer plus an sm_image_desc table, and wraps same-size batches in place.  The table depends
+    only on the sequence of shapes and is uploaded only when that changes, asynchronously from pinned memory, so packing
+    never waits for the device.  Host arrays are concatenated on the host and copied in one transfer; CUDA tensors are
+    concatenated on the device."""
 
     def __init__(self, dev):
         self.dev = dev
-        self._tables: dict = {}                     # channels -> (shapes key, device table, host table)
+        self._tables: dict = {}                     # channels -> ((shapes, shared) key, device table, host table)
 
-    def table(self, shapes, channels: int):
-        """(device sm_image_desc table, host table) of `shapes` at `channels` elements per pixel."""
-        key = tuple(None if s is None else (int(s[0]), int(s[1])) for s in shapes)
+    def table(self, shapes, channels: int, shared: bool = False):
+        """(device sm_image_desc table, host table) of `shapes` at `channels` elements per pixel; shared: every entry
+        at offset 0 (one image that all entries read)."""
+        return self._table(tuple(None if s is None else (int(s[0]), int(s[1])) for s in shapes), channels, shared)
+
+    def _table(self, shapes: tuple, channels: int, shared: bool):
+        key = (shapes, shared)
         hit = self._tables.get(channels)
         if hit is not None and hit[0] == key:
             return hit[1], hit[2]
-        t = image_table(key, channels)
+        t = image_table(shapes, channels)
+        if shared:
+            t["offset"] = 0
         host = torch.from_numpy(t.view(np.uint8).reshape(-1).copy())
         if torch.device(self.dev).type == "cuda":
             host = host.pin_memory()                # the copy below then queues without waiting for the device
@@ -155,6 +164,19 @@ class FramePacker:
         else:
             data = torch.zeros(1, dtype=torch.uint8, device=self.dev)
         return Packed(data, desc, shapes, channels, table)
+
+    def wrap(self, images, channels: int = 3, shared: int | None = None) -> Packed:
+        """A batch of same-size images as a `Packed` without a copy: images uint8 [F,h,w,3] (channels 3) or [F,h,w]
+        (channels 1), a tensor or a numpy array (moved to the device once), whose flat storage becomes `data` under the
+        table of F images back to back.  With shared=n, images is one [h,w,3] (or [h,w]) image that all n entries read
+        (every offset 0).  No checks: the callers validate dtype and rank."""
+        t = torch.as_tensor(images).to(self.dev).contiguous()
+        if shared is None:
+            n, h, w = (int(v) for v in t.shape[:3])
+        else:
+            n, (h, w) = int(shared), (int(v) for v in t.shape[:2])
+        desc, table = self._table(((h, w),) * n, channels, shared is not None)      # no per-entry key building
+        return Packed(t.reshape(-1), desc, [(h, w)] * n, channels, table)
 
 
 @dataclass
@@ -201,7 +223,6 @@ class BatchTracker:
         self._fidx: list[int] = []
         self._hp: list[tuple[float, float, float]] = []
         self._size: list[tuple[int, int]] = []         # (H, W) of the frames each stream reads
-        self.im_w = self.im_h = None                   # the streams' common frame size (None when they differ)
         dev = self.dev
         self.state = torch.zeros(0, 4, dtype=torch.float64, device=dev)
         self.avg = torch.zeros(0, 3, dtype=torch.int32, device=dev)
@@ -220,63 +241,37 @@ class BatchTracker:
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
 
-    def _frames(self, frames) -> torch.Tensor:
-        """uint8 [F,H,W,3] on the device (a single [H,W,3] frame is shared by all streams)."""
+    def _input(self, frames, shared: int = 1) -> Packed:
+        """The frames of a call as a `Packed`: a list (or tuple) of frames, which may differ in size, is packed (None
+        entries skipped); a uint8 [F,H,W,3] array or tensor is moved to the device once and wrapped without a copy; a
+        single [H,W,3] frame is wrapped as `shared` entries that all read it."""
+        if isinstance(frames, Packed):
+            return frames
         if isinstance(frames, (list, tuple)):
-            frames = np.stack([np.asarray(f) for f in frames], 0)
+            return self.packer.pack(frames, 3)
         t = torch.as_tensor(frames)
         if t.dtype != torch.uint8:
             raise ValueError("frames must be uint8 HWC (BGR as cv2.imread returns them)")
         if t.dim() not in (3, 4) or t.shape[-1] != 3:
             raise ValueError(f"frames must be [H,W,3] or [F,H,W,3], got {tuple(t.shape)}")
-        return t.to(self.dev).contiguous()
+        return self.packer.wrap(t, 3, shared if t.dim() == 3 else None)
 
-    def _input(self, frames):
-        """The frames of a call: a list (or tuple) of frames, which may differ in size, is packed (`Packed`, None
-        entries skipped); anything else goes through `_frames`."""
-        if isinstance(frames, Packed):
-            return frames
-        if isinstance(frames, (list, tuple)):
-            return self.packer.pack(frames, 3)
-        return self._frames(frames)
-
-    @staticmethod
-    def _hw(fr: torch.Tensor):
-        return (int(fr.shape[0]), int(fr.shape[1])) if fr.dim() == 3 else (int(fr.shape[1]), int(fr.shape[2]))
-
-    def _sizes_read(self, fr, src: list[int]) -> list:
+    def _sizes_read(self, fr: Packed, src: list[int]) -> list:
         """(H, W) of the frame each of the streams reading frames `src` of `fr` gets; ValueError for a missing one."""
-        if isinstance(fr, Packed):
-            bad = [i for i in src if not 0 <= i < len(fr.shapes) or fr.shapes[i] is None]
-            if bad:
-                raise ValueError(f"a stream reads frame {bad[0]}, but {len(fr.shapes)} frames were given "
-                                 "(or that entry is None)")
-            return [fr.shapes[i] for i in src]
-        if fr.dim() == 4 and any(i >= fr.shape[0] for i in src):
-            raise ValueError(f"a stream reads frame {max(src)}, but only {fr.shape[0]} frames were given")
-        return [self._hw(fr)] * len(src)
+        n = len(fr.shapes)
+        got = [fr.shapes[i] if 0 <= i < n else None for i in src]
+        if None in got:
+            raise ValueError(f"a stream reads frame {src[got.index(None)]}, but {n} frames were given "
+                             "(or that entry is None)")
+        return got
 
-    def _check_sizes(self, fr, rows: list[int], src: list[int]):
+    def _check_sizes(self, fr: Packed, rows, src: list[int]):
         """A stream is bound to the frame size it was added with: ValueError when rows read frames of another size."""
-        got = self._sizes_read(fr, src)
-        for r, hw in zip(rows, got):
-            if hw != self._size[r]:
-                raise ValueError(f"stream {self._ids[r]} tracks {self._size[r][0]}x{self._size[r][1]} frames, "
-                                 f"got {hw[0]}x{hw[1]}")
-
-    def _crop(self, frames, frame_idx: torch.Tensor, boxes: torch.Tensor, size: int) -> torch.Tensor:
-        N = boxes.shape[0]
-        out = torch.empty(N, 3, size, size, device=self.dev, dtype=torch.float32)
-        if isinstance(frames, Packed):
-            _lib.check(self.lib.sm_crop_resize_ragged(frames.data.data_ptr(), frames.desc.data_ptr(),
-                                                      frame_idx.data_ptr(), boxes.data_ptr(), N, size, out.data_ptr(),
-                                                      self._stream()))
-            return out
-        H, W = self._hw(frames)
-        stride = 0 if frames.dim() == 3 else H * W * 3
-        _lib.check(self.lib.sm_crop_resize_indexed(frames.data_ptr(), stride, H, W, frame_idx.data_ptr(),
-                                                   boxes.data_ptr(), N, size, out.data_ptr(), self._stream()))
-        return out
+        got, want = self._sizes_read(fr, src), [self._size[r] for r in rows]
+        if got != want:                             # one comparison on the hot path; the loop only finds the culprit
+            r, hw = next((r, hw) for r, hw, s in zip(rows, got, want) if hw != s)
+            raise ValueError(f"frames must be {self._size[r][0]}x{self._size[r][1]} for stream {self._ids[r]}, "
+                             f"got {hw[0]}x{hw[1]}")
 
     def _upload_tables(self):
         """Device copies of the active set (slot table, frame-index table) and per-frame work buffers; runs only when the
@@ -291,27 +286,23 @@ class BatchTracker:
         self.aux = torch.zeros(N, 4, dtype=torch.float64, device=dev)
         self.maps = torch.zeros(N, 6, dtype=torch.float64, device=dev)
         self.imsize = torch.tensor([[w, h] for h, w in self._size], dtype=torch.int32, device=dev).reshape(N, 2)
-        sizes = set(self._size)
-        self.im_h, self.im_w = next(iter(sizes)) if len(sizes) == 1 else (None, None)
-        self._mask_table = None                         # sm_image_desc of the rows' pasted masks, built on first use
+        self._mask_table = None                         # paste-back table, buffer length, grid; built on first use
 
-    def _template(self, fr: torch.Tensor, src: list[int], state: torch.Tensor, slots: list[int]) -> torch.Tensor:
-        """The template half of siamese_init (tools/test.py:142-155) for n streams: fr uint8 frames on the device, src
+    def _template(self, fr: Packed, src: list[int], state: torch.Tensor, slots: list[int]) -> torch.Tensor:
+        """The template half of siamese_init (tools/test.py:142-155) for n streams: fr the frames on the device, src
         [n] the frame of `fr` each stream reads, state f64 [n,4] (target_pos, target_sz) exactly as siamese_init
         receives them, slots [n] the engine slots to write.  Returns the streams' avg_chans, int32 [n,3]."""
         n = len(src)
         src_dev = torch.tensor(src, dtype=torch.int32, device=self.dev)
         # avg_chans = np.mean(im, axis=(0, 1)); written into a uint8 image it truncates (:146, :89-100).
-        # Sums of < 2^53 integers are exact in float64, so sum / n equals numpy's mean bit for bit.
-        uniq = sorted(set(src))
-        if isinstance(fr, Packed):
-            mean = torch.stack([fr.view(i).to(torch.float64).sum(dim=(0, 1)) / float(fr.shapes[i][0] * fr.shapes[i][1])
-                                for i in uniq])
-        else:
-            H, W = self._hw(fr)
-            f4 = fr if fr.dim() == 4 else fr.unsqueeze(0)
-            mean = f4[uniq].to(torch.float64).sum(dim=(1, 2)) / float(H * W)
-        where = torch.tensor([uniq.index(i) for i in src], device=self.dev)
+        # Sums of < 2^53 integers are exact in float64, so sum / n equals numpy's mean bit for bit.  Each frame is
+        # reduced once: the entries of a shared frame have one offset.
+        offset = [int(fr.table["offset"][i]) for i in src]
+        uniq = sorted(set(offset))
+        entry = dict(zip(offset, src))
+        mean = torch.stack([fr.view(entry[o]).to(torch.float64).sum(dim=(0, 1))
+                            / float(fr.shapes[entry[o]][0] * fr.shapes[entry[o]][1]) for o in uniq])
+        where = torch.tensor([uniq.index(o) for o in offset], device=self.dev)
         avg = mean[where].to(torch.uint8).to(torch.int32).contiguous()
         # template window (:149-155): s_z = round(sqrt(wc_z * hc_z)), crop around target_pos, resize to 127
         sw, sh = state[:, 2], state[:, 3]
@@ -324,7 +315,7 @@ class BatchTracker:
         zb[:, 1] = torch.round(state[:, 1] - c).to(torch.int32)
         zb[:, 2] = s_z.to(torch.int32)
         zb[:, 3:6] = avg
-        z = self._crop(fr, src_dev, zb, self.p.exemplar_size)
+        z = ops._crop_resize_ragged(fr.data, fr.desc, src_dev, zb, self.p.exemplar_size)
         self.net.template(z, slots=torch.tensor(slots, dtype=torch.int32, device=self.dev))
         return avg
 
@@ -359,17 +350,15 @@ class BatchTracker:
             return self._join(frames, self._state(target_pos, target_sz), frame_index, hp)
 
     def _join(self, frames, state: torch.Tensor, frame_index, hp) -> list[int]:
-        fr = self._input(frames)
         n = state.shape[0]
         idx = list(range(n)) if frame_index is None else [int(i) for i in np.asarray(frame_index).reshape(-1)]
         if len(idx) != n:
             raise ValueError("one frame index per new stream expected")
-        ragged = isinstance(fr, Packed)
-        F = len(fr.shapes) if ragged else (1 if fr.dim() == 3 else int(fr.shape[0]))
-        if (ragged or fr.dim() == 4) and any(i < 0 or i >= F for i in idx):
-            raise ValueError(f"frame index out of range [0, {F})")
+        fr = self._input(frames, max(idx, default=0) + 1)
         if any(i < 0 for i in idx):
             raise ValueError("frame indices must be >= 0")
+        if any(i >= len(fr.shapes) for i in idx):
+            raise ValueError(f"frame index out of range [0, {len(fr.shapes)})")
         if hp is None:
             rows = [(float(self.p.penalty_k), float(self.p.window_influence), float(self.p.lr))] * n
         else:
@@ -385,9 +374,8 @@ class BatchTracker:
             return []
         if self.N + n > self.net.max_batch or len(free) < n:
             raise ValueError("more streams than the engine was built for")
-        src = idx if ragged or fr.dim() == 4 else [0] * n          # frame each new stream reads in this call
-        sizes = self._sizes_read(fr, src)                          # each new stream is bound to its frame's size
-        avg = self._template(fr, src, state, free)
+        sizes = self._sizes_read(fr, idx)                          # each new stream is bound to its frame's size
+        avg = self._template(fr, idx, state, free)
         ids = list(range(self._next_id, self._next_id + n))
         self._next_id += n
         self.state = torch.cat([self.state, state], 0).contiguous()
@@ -416,9 +404,9 @@ class BatchTracker:
         if not ids:
             return
         with torch.cuda.device(self.dev):
-            fr = self._input(frames)
             rows = [self._ids.index(i) for i in ids]
-            src = [self._fidx[r] for r in rows] if isinstance(fr, Packed) or fr.dim() == 4 else [0] * len(rows)
+            src = [self._fidx[r] for r in rows]
+            fr = self._input(frames, max(src) + 1)
             self._check_sizes(fr, rows, src)
             state = self._state(target_pos, target_sz)
             if state.shape[0] != len(ids):
@@ -472,19 +460,12 @@ class BatchTracker:
             raise RuntimeError("no active streams: call init() or add() first")
         p, N = self.p, self.N
         with torch.cuda.device(self.dev):
-            fr = self._input(frames)
-            if isinstance(fr, Packed):
-                self._check_sizes(fr, range(N), self._fidx)
-            else:
-                if self._hw(fr) != (self.im_h, self.im_w):
-                    raise ValueError(f"frames must be {self.im_h}x{self.im_w}" if self.im_h is not None else
-                                     "the streams track frames of different sizes: pass the frames as a list")
-                if fr.dim() == 4 and self._max_fidx >= fr.shape[0]:
-                    raise ValueError(f"a stream reads frame {self._max_fidx}, but only {fr.shape[0]} frames were given")
+            fr = self._input(frames, self._max_fidx + 1)
+            self._check_sizes(fr, range(N), self._fidx)
             st = self._stream()
             _lib.check(self.lib.sm_tracker_prepare(N, self.state.data_ptr(), self.avg.data_ptr(), C.byref(self.hp),
                                                    self.boxes.data_ptr(), self.tsz.data_ptr(), self.aux.data_ptr(), st))
-            x = self._crop(fr, self._fidx_dev, self.boxes, p.instance_size)
+            x = ops._crop_resize_ragged(fr.data, fr.desc, self._fidx_dev, self.boxes, p.instance_size)
             use_refine = mask and refine
             use_head = mask and not refine
             out = self.net._step(x, self.anchors, self.window, self.tsz, p.penalty_k, p.window_influence,
@@ -504,21 +485,16 @@ class BatchTracker:
                     raise ValueError(f"out_size {p.out_size} does not match the mask source ({side})")
                 m = logits.sigmoid().view(N, side, side).contiguous()
                 extras["mask_prob"], extras["maps"] = m, self.maps
-                if paste and self.im_h is not None:
-                    W, H = self.im_w, self.im_h
-                    pasted = torch.empty(N, H, W, device=self.dev, dtype=torch.float32)
-                    _lib.check(self.lib.sm_warp_affine(m.data_ptr(), side, side, self.maps.data_ptr(), pasted.data_ptr(),
-                                                       H, W, C.c_float(-1.0), N, st))
-                    mask_out = pasted > p.seg_thr
-                elif paste:                                 # streams of different sizes: one packed buffer
+                if paste:                                   # every row's mask in one packed buffer
                     if self._mask_table is None:
-                        self._mask_table = self.packer.table(self._size, 1)
-                    desc, table = self._mask_table
-                    total = int(table["offset"][-1]) + self._size[-1][0] * self._size[-1][1]
-                    pasted = torch.empty(total, device=self.dev, dtype=torch.float32)
-                    _lib.check(self.lib.sm_warp_affine_ragged(m.data_ptr(), side, self.maps.data_ptr(), pasted.data_ptr(),
-                                                              desc.data_ptr(), N, max(h for h, _ in self._size),
-                                                              max(w for _, w in self._size), C.c_float(-1.0), st))
-                    flat = pasted > p.seg_thr
-                    mask_out = [flat[int(o):int(o) + h * w].view(h, w) for o, (h, w) in zip(table["offset"], self._size)]
+                        desc, table = self.packer.table(self._size, 1)
+                        hs, ws = zip(*self._size)
+                        self._mask_table = desc, table, int(table["offset"][-1]) + hs[-1] * ws[-1], (max(hs), max(ws))
+                    desc, table, total, max_hw = self._mask_table
+                    flat = ops._warp_affine_ragged(m, self.maps, desc, max_hw, total) > p.seg_thr
+                    if len(set(self._size)) == 1:                  # one frame size: rows back to back, [N,H,W]
+                        mask_out = flat.view(N, *max_hw)
+                    else:
+                        mask_out = [flat[int(o):int(o) + h * w].view(h, w)
+                                    for o, (h, w) in zip(table["offset"], self._size)]
             return TrackResult(state=res, mask=mask_out, extras=extras)

@@ -52,6 +52,14 @@ def _check_thresholds(thrs) -> np.ndarray:
     return t
 
 
+def _one_size(frames, fr) -> bool:
+    """Whether `frames` (fr: the tracker's `Packed` of them) is a [G,H,W,3] batch or a list of frames of one size:
+    `sm_mask_iou` scores same-size videos only."""
+    if isinstance(frames, (list, tuple)):
+        return None not in fr.shapes and len(set(fr.shapes)) == 1
+    return np.ndim(frames) == 4
+
+
 class ParamSweep:
     """tune_vos's grid search over `combos` (float64 [K,3] = penalty_k, window_influence, lr; default `grid()`) for G
     videos on one engine.  `net` is a `siammask_b200.Custom` whose max_batch and num_slots cover G*K streams; `params`
@@ -82,10 +90,10 @@ class ParamSweep:
         """siamese_init of every (video, combination) stream on frame 0.  frames0: uint8 [G,H,W,3] (BGR); boxes_xywh:
         [G,4] top-left x, y, w, h of each video's target; num_frames: T, the videos' length.  Frames 1 .. T-2 are scored
         (tune_vos's start_frame < f < end_frame).  Stream (g, k) is row g*K + k of every per-frame output."""
-        fr = self.tracker._frames(frames0)
-        if fr.dim() != 4:
+        fr = self.tracker._input(frames0)
+        if not _one_size(frames0, fr):
             raise ValueError("frames0 must be [G,H,W,3]")
-        G, K, T = int(fr.shape[0]), self.K, int(num_frames)
+        G, K, T = len(fr.shapes), self.K, int(num_frames)
         boxes = np.asarray(boxes_xywh, dtype=np.float64)
         if boxes.shape != (G, 4):
             raise ValueError(f"boxes_xywh must be [{G}, 4]")
@@ -111,17 +119,18 @@ class ParamSweep:
         f = self.f
         if not 1 <= f < self.T:
             raise ValueError("call open() first; at most num_frames - 1 frames follow it")
-        fr = self.tracker._frames(frames)
-        if fr.dim() != 4 or fr.shape[0] != self.G:
+        fr = self.tracker._input(frames)
+        if not _one_size(frames, fr) or len(fr.shapes) != self.G:
             raise ValueError(f"frames must be [{self.G},H,W,3]")
+        H, W = fr.shapes[0]
         scored = f < self.T - 1
         anno = None
         if scored:
             if annos is None:
                 raise ValueError(f"frame {f} is scored: annotations are required")
             anno = torch.as_tensor(annos).to(self.dev).contiguous()
-            if anno.dtype != torch.uint8 or tuple(anno.shape) != (self.G, int(fr.shape[1]), int(fr.shape[2])):
-                raise ValueError(f"annos must be uint8 [{self.G},{int(fr.shape[1])},{int(fr.shape[2])}]")
+            if anno.dtype != torch.uint8 or tuple(anno.shape) != (self.G, H, W):
+                raise ValueError(f"annos must be uint8 [{self.G},{H},{W}]")
         r = self.tracker.track(fr, mask=True, refine=self.p.out_size == 127, paste=False)
         if scored:
             cnt = ops._mask_iou(r.extras["mask_prob"], r.extras["maps"], anno, self._video, self._thrs_dev)

@@ -1,6 +1,7 @@
 """Multi-object video object segmentation on the device: the `track_vos` loop of tools/test.py:459-542 (also driven by
 tools/tune_vos.py) for G videos at once, which may differ in frame size (pass the frames and annotations as lists:
-the label maps then come back as a list, and the label map, scores and init boxes run through the *_ragged kernels).
+the label maps then come back as a list).  Frames and annotations reach the kernels as `tracker.Packed` buffers with
+an sm_image_desc table, so the label map, its scores and the init boxes always run through the *_ragged kernels.
 
 In the reference every object of a video is a separate tracker run with its own lifetime: it is initialised from the
 annotation label map at its `start_frame` with `cv2.boundingRect(anno == id)` (:483-498), tracked while
@@ -10,13 +11,14 @@ one label map, `(argmax_k + 1) * (max_k > seg_thr)` (:480, :504, :521-523).
 
 `VideoSegmenter` restates that over a `BatchTracker`: all objects of all videos that are tracked at a frame advance
 as one batch (each stream crops its own video's frame in place), objects join at their start frame (`add`, init boxes
-from `sm_label_boxes`) and leave after their end frame (`remove`), and the label maps of all videos come from one fused
-paste-back + argmax kernel (`sm_paste_labels`): the per-object float frames are never materialised.
+from `sm_label_boxes_ragged`) and leave after their end frame (`remove`), and the label maps of all videos come from one
+fused paste-back + argmax kernel (`sm_paste_labels_ragged`): the per-object float frames are never materialised.
 
 With `open(..., score=...)` it also computes the score `track_vos` returns for a video, `MultiBatchIouMeter`
 (tools/test.py:421-456): per object and threshold of `VOS_THRESHOLDS`, the mean over the object's scored frames of the IoU
-between the fused label `== k+1` and the object's annotation.  Scored frames go through `sm_paste_labels_iou`, the same
-kernel pass with (intersection, union) counts per object and threshold; the counts stay on the device until `result`.
+between the fused label `== k+1` and the object's annotation.  Scored frames go through `sm_paste_labels_iou_ragged`,
+the same kernel pass with (intersection, union) counts per object and threshold; the counts stay on the device until
+`result`.
 The reference has two branches, both restated as they are:
   score="whole": no start_frame dict (DAVIS 2016/2017).  The k-th object of a video is scored against annotation id
                  k+1 (by position, whatever id it was tracked with) on frames 1 .. num_frames-2;
@@ -180,18 +182,8 @@ class VideoSegmenter:
         scored window.  Returns labels uint8 [G,H,W] on the device.  frames may instead be a list of G frames
         [H_g,W_g,3] of different sizes, with annos a list of G maps [H_g,W_g]; labels are then a list of G uint8
         [H_g,W_g] views of one packed buffer."""
-        f = self.f
-        ragged = isinstance(frames, (list, tuple))
-        fr = self.tracker._input(frames) if ragged else self.tracker._frames(frames)
-        if ragged:
-            if len(fr.shapes) != self.G or any(s is None for s in fr.shapes):
-                raise ValueError(f"frames must be a list of {self.G} frames")
-            G = self.G
-            H, W = max(s[0] for s in fr.shapes), max(s[1] for s in fr.shapes)      # the grid of the label kernels
-        else:
-            if fr.dim() != 4 or fr.shape[0] != self.G:
-                raise ValueError(f"frames must be [{self.G},H,W,3]")
-            G, H, W = int(fr.shape[0]), int(fr.shape[1]), int(fr.shape[2])
+        f, G = self.f, self.G
+        # the schedule and scoring checks need no frames: they fail before any frame reaches the device
         kinds = schedule(self._start, self._end, f)
         starting = [k for k in range(len(self.objects)) if kinds[k] == OBJ_INIT]
         scored = None
@@ -203,7 +195,14 @@ class VideoSegmenter:
                 raise ValueError(f"frame {f} is scored: annotation label maps are required")
             if not scored.any():
                 scored = None
-        if ragged and annos is not None:                # host check from shapes alone, before any device work
+        listed = isinstance(frames, (list, tuple))
+        fr = self.tracker._input(frames)
+        if listed and (len(fr.shapes) != G or any(s is None for s in fr.shapes)):
+            raise ValueError(f"frames must be a list of {G} frames")
+        if not listed and (np.ndim(frames) != 4 or len(fr.shapes) != G):
+            raise ValueError(f"frames must be [{G},H,W,3]")
+        H, W = max(s[0] for s in fr.shapes), max(s[1] for s in fr.shapes)      # the grid of the label kernels
+        if listed and annos is not None:                # host check from shapes alone, before any device work
             if not isinstance(annos, (list, tuple)) or len(annos) != G:
                 raise ValueError(f"annos must be a list of {G} label maps, one per frame")
             shp = [None if a is None else tuple(int(v) for v in a.shape) for a in annos]
@@ -213,26 +212,23 @@ class VideoSegmenter:
         if starting or scored is not None:
             if annos is None:
                 raise ValueError(f"frame {f}: objects start here, annotation label maps are required")
-            if ragged:
-                if not isinstance(annos, (list, tuple)) or len(annos) != G:
-                    raise ValueError(f"annos must be a list of {G} label maps, one per frame")
+            if listed:
                 pa = self.tracker.packer.pack(annos, 1)
                 if pa.shapes != fr.shapes:
                     raise ValueError(f"each anno must match its frame's size: {pa.shapes} vs {fr.shapes}")
-                anno = pa.data
             else:
-                anno = torch.as_tensor(annos).to(self.dev).contiguous()
-                if anno.dtype != torch.uint8 or tuple(anno.shape) != (G, H, W):
+                a = torch.as_tensor(annos)
+                if a.dtype != torch.uint8 or tuple(a.shape) != (G, H, W):
                     raise ValueError(f"annos must be uint8 [{G},{H},{W}]")
-        plane = None
-        if ragged:                                      # sm_image_desc of the G label maps (and annotations)
-            desc, ptable = self.tracker.packer.table(fr.shapes, 1)
-            plane = (desc, int(ptable["offset"][-1]) + fr.shapes[-1][0] * fr.shapes[-1][1])
+                pa = self.tracker.packer.wrap(a, 1)
+            anno = pa.data
+        # sm_image_desc of the G label maps (and annotations)
+        desc, ptable = self.tracker.packer.table(fr.shapes, 1)
+        plane = (desc, int(ptable["offset"][-1]) + fr.shapes[-1][0] * fr.shapes[-1][1])
         if starting:
             # init boxes (:494-496): one D2H copy, at init frames only
             queries = [(self.objects[k][0], self.objects[k][1]) for k in starting]
-            boxes = (ops._label_boxes_ragged(anno, plane[0], G, queries) if ragged
-                     else ops.label_boxes(anno, queries)).cpu().numpy()
+            boxes = ops._label_boxes_ragged(anno, desc, G, queries).cpu().numpy()
             missing = [self.objects[k][:2] for k, b in zip(starting, boxes) if b[2] == 0]
             if missing:
                 raise ValueError(f"frame {f}: (video, id) {missing} not in the annotation")
@@ -261,9 +257,9 @@ class VideoSegmenter:
             labels, _ = ops._paste_labels_iou(masks, maps, anno, self._offsets, table, self._target_ids(scored), (H, W),
                                               self.p.seg_thr, self._thrs_dev, counts=self._counts[f], ragged=plane)
         self.f += 1
-        if ragged:
+        if listed:
             return [labels[int(o):int(o) + h * w].view(h, w) for o, (h, w) in zip(ptable["offset"], fr.shapes)]
-        return labels
+        return labels.view(G, H, W)
 
     def state(self):
         """Per-object tracker state after the last frame: target_pos f64 [n,2], target_sz f64 [n,2] (NaN for objects

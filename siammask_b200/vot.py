@@ -9,8 +9,8 @@ prediction `cxy_wh_2_rect(target_pos, target_sz)` as the entry.
 
 Here every sequence (x every hyper-parameter combination) is one stream of a `BatchTracker`:
     1. `track(mask=False)` advances all active streams;
-    2. `sm_vot_overlap` scores each stream's clamped-state rectangle against its sequence's ground truth of the frame
-       (`sm_vot_overlap_sized` with each sequence's own (W, H) when the sequences differ in frame size);
+    2. `sm_vot_overlap_sized` scores each stream's clamped-state rectangle against its sequence's ground truth of the
+       frame, within its sequence's own (W, H);
     3. device tensors keep each stream's start frame, entry codes, float64 locations and lost_times, without a host
        sync;
     4. streams whose start frame is this frame are templated again in their own engine slots (`BatchTracker.reinit`);
@@ -43,7 +43,7 @@ import numpy as np
 import torch
 
 from . import ops
-from .tracker import BatchTracker, Packed, TrackerParams
+from .tracker import BatchTracker, TrackerParams
 
 # tools/tune_vot.py's argparse defaults: a 9 x 14 x 3 grid of (penalty_k, window_influence, lr)
 DEFAULT_PENALTY_K = np.arange(0.05, 0.5, 0.05)
@@ -140,14 +140,11 @@ class VotRunner:
         of G frames [H_g,W_g,3] whose sizes may differ; gt: G float64 arrays [T_g, 8], each sequence's ground-truth
         polygons (lengths may differ).  Every gt row is checked and uploaded here, once."""
         fr = self.tracker._input(frames0)
-        if isinstance(fr, Packed):
-            if any(s is None for s in fr.shapes):
-                raise ValueError("frames0 must hold frame 0 of every sequence")
-            G, self._hw = len(fr.shapes), list(fr.shapes)
-        else:
-            if fr.dim() != 4:
-                raise ValueError("frames0 must be [G,H,W,3]")
-            G, self._hw = int(fr.shape[0]), [self.tracker._hw(fr)] * int(fr.shape[0])
+        if not isinstance(frames0, (list, tuple)) and np.ndim(frames0) != 4:
+            raise ValueError("frames0 must be [G,H,W,3]")
+        if any(s is None for s in fr.shapes):
+            raise ValueError("frames0 must hold frame 0 of every sequence")
+        G, self._hw = len(fr.shapes), list(fr.shapes)
         K = self.K
         gts = check_gt(gt)
         if len(gts) != G:
@@ -193,9 +190,8 @@ class VotRunner:
         self._row_streams = [self._stream_of[i] for i in self.tracker.ids]
         self._row_dev = torch.tensor(self._row_streams, dtype=torch.long, device=self.dev)
         self._row_video = torch.as_tensor(self._video[self._row_streams], dtype=torch.long, device=self.dev)
-        if len(set(self._hw)) > 1:                      # each row's own (W, H) for sm_vot_overlap_sized
-            wh = [self._hw[self._video[s]][::-1] for s in self._row_streams]
-            self._row_wh = torch.tensor(wh, dtype=torch.int32, device=self.dev).reshape(-1, 2)
+        wh = [self._hw[self._video[s]][::-1] for s in self._row_streams]     # each row's own (W, H)
+        self._row_wh = torch.tensor(wh, dtype=torch.int32, device=self.dev).reshape(-1, 2)
 
     def _retire(self):
         """Step 5: streams whose sequence ends with frame self.f leave the batch."""
@@ -214,10 +210,10 @@ class VotRunner:
         if self.G == 0 or self.tracker.N == 0:
             raise ValueError("call open() first; every sequence has ended")
         fr = self.tracker._input(frames)
-        if isinstance(fr, Packed):
+        if isinstance(frames, (list, tuple)):
             if len(fr.shapes) != self.G:
                 raise ValueError(f"frames must be a list of {self.G} frames")
-        elif fr.dim() != 4 or fr.shape[0] != self.G:
+        elif np.ndim(frames) != 4 or len(fr.shapes) != self.G:
             raise ValueError(f"frames must be [{self.G},H,W,3]")
         rows = self._row_dev
         # 1. track every active stream (skipped ones too: their outputs are discarded below)
@@ -229,10 +225,7 @@ class VotRunner:
         x1, y1 = x0 + st[:, 2], y0 + st[:, 3]
         loc = torch.stack([x0, y0, st[:, 2], st[:, 3]], 1)
         pred = torch.stack([x0, y0, x1, y0, x1, y1, x0, y1], 1).float()
-        if len(set(self._hw)) > 1:
-            ov = ops._vot_overlap_sized(self._gt[self._row_video, f], pred, self._row_wh)
-        else:
-            ov = ops._vot_overlap(self._gt[self._row_video, f], pred, self._hw[0])
+        ov = ops._vot_overlap_sized(self._gt[self._row_video, f], pred, self._row_wh)
         # 3. bookkeeping on the device: init / track / skip by the stream's start frame; only an overlap of exactly 0
         #    is a failure (NaN is truthy)
         start = self._start[rows]

@@ -65,7 +65,9 @@ def test_crop_ragged_equals_indexed_crop_per_size_group():
     order = rng.permutation(len(boxes))                             # sizes interleaved in the batch
     boxes, fidx = np.array(boxes)[order], np.array(fidx)[order]
     pk = FramePacker("cuda").pack(frames, 3)
-    got = ops._crop_resize_ragged(pk.data, pk.desc, fidx, boxes, 255)
+    table = torch.zeros(len(boxes), 8, dtype=torch.int32)                # the tracker's [B,8] box table
+    table[:, :6] = torch.from_numpy(boxes)
+    got = ops._crop_resize_ragged(pk.data, pk.desc, torch.from_numpy(fidx).int().cuda(), table.cuda(), 255)
     dev = [torch.from_numpy(f).cuda() for f in frames]
     for g in range(len(SIZES)):
         sel = np.nonzero(fidx == g)[0]

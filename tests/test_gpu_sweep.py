@@ -9,7 +9,7 @@ import pytest
 import torch
 
 import siammask_b200 as smb
-from siammask_b200 import _lib
+from siammask_b200 import _lib, ops
 from siammask_b200.ops import mask_iou, warp_affine
 from siammask_b200.tracker import BatchTracker, TrackerParams
 from siammask_b200.tune import grid
@@ -202,11 +202,11 @@ def _scalar_track(bt, frames):
     """One frame of BatchTracker.track through the scalar entry points (sm_step_slots, sm_tracker_update): the path the
     tracker took before it carried a per-stream table."""
     p, N, lib = bt.p, bt.N, bt.lib
-    fr = bt._frames(frames)
+    fr = bt._input(frames)
     st = bt._stream()
     _lib.check(lib.sm_tracker_prepare(N, bt.state.data_ptr(), bt.avg.data_ptr(), C.byref(bt.hp), bt.boxes.data_ptr(),
                                       bt.tsz.data_ptr(), bt.aux.data_ptr(), st))
-    x = bt._crop(fr, bt._fidx_dev, bt.boxes, p.instance_size)
+    x = ops._crop_resize_ragged(fr.data, fr.desc, bt._fidx_dev, bt.boxes, p.instance_size)
     out = bt.net._step(x, bt.anchors, bt.window, bt.tsz, p.penalty_k, p.window_influence, refine=True,
                        slots=bt._slots_dev)
     res = torch.empty(N, 8, dtype=torch.float64, device="cuda")

@@ -70,6 +70,37 @@ def test_descriptor_table_is_reused_while_shapes_repeat():
     assert pk.table([f.shape[:2] for f in fr[::-1]], 3)[0] is changed
 
 
+def test_wrap_a_batch_in_place_under_the_uniform_table():
+    pk = FramePacker("cpu")
+    t = torch.from_numpy(np.random.RandomState(1).randint(0, 256, (4, 6, 5, 3)).astype(np.uint8))
+    p = pk.wrap(t, 3)
+    assert p.data.data_ptr() == t.data_ptr() and p.data.numel() == t.numel()       # no copy
+    assert p.table.tobytes() == image_table([(6, 5)] * 4, 3).tobytes()
+    assert bytes(p.desc.numpy()) == p.table.tobytes()
+    assert p.shapes == [(6, 5)] * 4 and p.channels == 3
+    for i in range(4):
+        assert torch.equal(p.view(i), t[i])
+    assert pk.wrap(t.clone(), 3).desc is p.desc                                      # same shape: no new table
+    assert pk.table([(6, 5)] * 4, 3)[0] is p.desc
+
+
+def test_wrap_a_shared_frame_and_label_maps():
+    pk = FramePacker("cpu")
+    frame = torch.from_numpy(np.random.RandomState(2).randint(0, 256, (6, 5, 3)).astype(np.uint8))
+    p = pk.wrap(frame, 3, shared=3)                                                  # 3 entries read one frame
+    assert p.data.data_ptr() == frame.data_ptr() and p.data.numel() == frame.numel()
+    assert list(p.table["offset"]) == [0, 0, 0] and list(p.table["h"]) == [6] * 3 and list(p.table["w"]) == [5] * 3
+    assert bytes(p.desc.numpy()) == p.table.tobytes()
+    assert all(torch.equal(p.view(i), frame) for i in range(3))
+    assert pk.wrap(frame, 3).desc is not p.desc                                      # [3 back to back] is another table
+    maps = np.random.RandomState(3).randint(0, 4, (3, 6, 5)).astype(np.uint8)         # [G,H,W] label maps, from numpy
+    m = pk.wrap(maps, 1)
+    assert m.table.tobytes() == image_table([(6, 5)] * 3, 1).tobytes() and m.channels == 1
+    for g in range(3):
+        np.testing.assert_array_equal(m.view(g).numpy(), maps[g])
+    assert pk.wrap(maps, 1).desc is m.desc
+
+
 def test_image_table_of_empty_and_single_entries():
     assert image_table([], 3).size == 0
     t = image_table([None, (2, 3)], 1)
