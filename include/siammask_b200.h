@@ -211,6 +211,15 @@ int sm_paste_labels_iou_ragged(const float* masks, int32_t side, const double* m
 int sm_label_boxes_ragged(const uint8_t* anno, const sm_image_desc* video_desc, int32_t G, const int32_t* queries,
                           int32_t Q, int32_t* boxes, void* stream);
 
+/* sm_mask_iou for annotations of different sizes: stream b is scored against the annotation image video[b] of the
+ * packed uint8 buffer anno, at anno + anno_desc[video[b]].offset (h x w bytes; anno_desc is a device table, video a
+ * device int32 [B] of entries that exist and are not empty).  Its pasted mask is clipped to that image's own bounds,
+ * and each distinct image's target count is counted once.  max_h / max_w bound every h / w (they size the grid).  Each
+ * stream's counts equal those of sm_mask_iou run on its image's size alone, bit for bit.  B == 0 is a no-op. */
+int sm_mask_iou_ragged(const float* masks, int32_t side, const double* maps, const uint8_t* anno,
+                       const sm_image_desc* anno_desc, const int32_t* video, int32_t B, int32_t max_h, int32_t max_w,
+                       const double* thrs, int32_t T, int32_t* counts, void* stream);
+
 /* Region overlap of the VOT supervised protocol (tools/test.py:341-354): for each of B pairs, overlap[b] (device f32
  * [B]) = the VOT toolkit's compute_polygon_overlap(poly_a[b], poly_b[b], bounds left 0, top 0, right W, bottom H) as
  * pyvotkit's vot_overlap calls it (flags 0: the non-legacy rasteriser), bit for bit.  poly_a / poly_b are device f32

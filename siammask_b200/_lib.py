@@ -99,6 +99,8 @@ SIGNATURES = {
                                    [C.c_double, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "sm_label_boxes_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
                                         C.c_void_p]),
+    "sm_mask_iou_ragged": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 4 + [C.c_int32] * 3 +
+                           [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "sm_step_host_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(SmStepIO), C.c_void_p,
                                      C.POINTER(C.c_int32)]),
     "sm_xcorr_depthwise": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int32] * 6 + [C.c_void_p]),

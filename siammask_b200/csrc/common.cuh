@@ -215,9 +215,11 @@ void launch_crop_resize(const uint8_t* frames, size_t frame_stride, int H, int W
 void launch_select(const float* cls, const float* loc, const float* anchors, const float* window, const double* tsz,
                    int B, int A, int R, double penalty_k, double window_influence, int32_t* best_idx, int32_t* pos,
                    float* rec, cudaStream_t st, const double* hp = nullptr);
-// sm_mask_iou (include/siammask_b200.h): fused paste-back + IouMeter counts; counts must hold B*T*2 int32
+// sm_mask_iou (include/siammask_b200.h): fused paste-back + IouMeter counts; counts must hold B*T*2 int32.  desc
+// (optional, sm_mask_iou_ragged): annotation g is desc[g] of a packed buffer, and H, W bound every image
 void launch_mask_iou(const float* masks, int side, const double* maps, const uint8_t* anno, const int32_t* video, int B,
-                     int H, int W, const double* thrs, int T, int32_t* counts, cudaStream_t st);
+                     int H, int W, const double* thrs, int T, int32_t* counts, cudaStream_t st,
+                     const sm_image_desc* desc = nullptr);
 // small-channel fp32 NHWC 3x3 pad-1 conv: in = up(a (+ b)); ymap/xmap: device nearest-upsample source indices
 void launch_small_conv3x3_maps(const float* a, const float* b, int B, int Hi, int Wi, int Ho, int Wo, int Cin, int Cout,
                                const int* ymap, const int* xmap, const float* w, const float* bias, int relu,

@@ -2190,6 +2190,21 @@ int sm_mask_iou(const float* masks, int32_t side, const double* maps, const uint
   SM_API_END
 }
 
+int sm_mask_iou_ragged(const float* masks, int32_t side, const double* maps, const uint8_t* anno,
+                       const sm_image_desc* anno_desc, const int32_t* video, int32_t B, int32_t max_h, int32_t max_w,
+                       const double* thrs, int32_t T, int32_t* counts, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(B >= 0 && max_h >= 1 && max_w >= 1 && side > 0, "bad argument");
+  SMK_CHECK((int64_t)max_h * max_w <= INT32_MAX, "frame too large for int32 counts");
+  SMK_CHECK(T >= 1 && T <= 32, "1 <= T <= 32 thresholds");
+  if (B == 0) return 0;
+  SMK_CHECK(masks && maps && anno && anno_desc && video && thrs && counts, "null argument");
+  require_device();
+  smk::launch_mask_iou(masks, side, maps, anno, video, B, max_h, max_w, thrs, T, counts,
+                       static_cast<cudaStream_t>(stream), anno_desc);
+  SM_API_END
+}
+
 int sm_label_boxes(const uint8_t* anno, int32_t G, int32_t H, int32_t W, const int32_t* queries, int32_t Q, int32_t* boxes,
                    void* stream) {
   SM_API_BEGIN

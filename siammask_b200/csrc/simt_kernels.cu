@@ -1177,6 +1177,9 @@ __global__ void __launch_bounds__(256) paste_labels_iou_kernel(const float* __re
 // nothing, which is exact too): a threshold below -1 gets no counts but the marker (-1, -1), stored by block 0 of the
 // rectangle kernel.  Inside the rectangle one warp covers 32 consecutive pixels and counts
 // every threshold with two ballots; lane t keeps threshold t's counts, so T <= 32.
+// desc (optional, sm_mask_iou_ragged): annotation g is desc[g] of a packed buffer.  H, W then bound every image (they
+// size the grids); the rectangle is clipped to the stream's own image and the target kernel's blocks past a smaller
+// image exit.
 constexpr int MI_THREADS = 256;
 constexpr int MI_MAX_T = 32;
 constexpr int MI_TARGET_BYTES = 16384;      // annotation bytes per block of mask_iou_target_kernel
@@ -1184,7 +1187,8 @@ constexpr int MI_TARGET_BYTES = 16384;      // annotation bytes per block of mas
 __global__ void __launch_bounds__(MI_THREADS) mask_iou_target_kernel(const uint8_t* __restrict__ anno,
                                                                      const int32_t* __restrict__ video, int B,
                                                                      size_t HW, const double* __restrict__ thrs, int T,
-                                                                     int32_t* __restrict__ counts) {
+                                                                     int32_t* __restrict__ counts,
+                                                                     const sm_image_desc* __restrict__ desc) {
   __shared__ int s_red[MI_THREADS / 32];
   const int b = blockIdx.y;
   const int g = video[b];
@@ -1192,9 +1196,15 @@ __global__ void __launch_bounds__(MI_THREADS) mask_iou_target_kernel(const uint8
   for (int j = threadIdx.x; j < b; j += MI_THREADS) dup |= video[j] == g;
   if (__syncthreads_or(dup)) return;                   // an earlier stream reads the same video and counts it
   const uint8_t* a = anno + (size_t)g * HW;
+  if (desc != nullptr) {                               // image g of a packed buffer; HW (the grid's) becomes its own
+    a = anno + desc[g].offset;
+    HW = (size_t)desc[g].h * desc[g].w;
+  }
   const size_t c0 = (size_t)blockIdx.x * MI_TARGET_BYTES, c1 = min(c0 + (size_t)MI_TARGET_BYTES, HW);
+  if (c0 >= HW) return;                                // block-uniform: past a smaller image (no barrier follows
+                                                       // before the reduction's, which every thread then skips)
   int cnt = 0;
-  if (((HW | reinterpret_cast<uintptr_t>(anno)) & 3) == 0) {
+  if (((HW | reinterpret_cast<uintptr_t>(a)) & 3) == 0) {
     const uint32_t* w = reinterpret_cast<const uint32_t*>(a);
     for (size_t i = c0 / 4 + threadIdx.x; i < c1 / 4; i += MI_THREADS) cnt += __popc(__vcmpne4(w[i], 0u)) >> 3;
   } else {
@@ -1217,12 +1227,14 @@ __global__ void __launch_bounds__(MI_THREADS) mask_iou_rect_kernel(const float* 
                                                                    const uint8_t* __restrict__ anno,
                                                                    const int32_t* __restrict__ video, int H, int W,
                                                                    const double* __restrict__ thrs, int T,
-                                                                   int32_t* __restrict__ counts) {
+                                                                   int32_t* __restrict__ counts,
+                                                                   const sm_image_desc* __restrict__ desc) {
   __shared__ double s_inv[6];
   __shared__ double s_thr[MI_MAX_T];
   __shared__ int s_rect[4];
   __shared__ int s_cnt[MI_MAX_T][2];
   const int b = blockIdx.y;
+  video_size(desc, video[b], H, W);                    // the rectangle is clipped to the stream's own image
   if (threadIdx.x < T) {
     s_thr[threadIdx.x] = thrs[threadIdx.x];
     s_cnt[threadIdx.x][0] = 0;
@@ -1258,7 +1270,7 @@ __global__ void __launch_bounds__(MI_THREADS) mask_iou_rect_kernel(const float* 
   const int x0 = s_rect[0], y0 = s_rect[1], rw = s_rect[2] - x0, rh = s_rect[3] - y0;
   const int n = rw > 0 && rh > 0 ? rw * rh : 0;
   const float* src = masks + (size_t)b * side * side;
-  const uint8_t* a = anno + (size_t)video[b] * H * W;
+  const uint8_t* a = anno + video_pixel(desc, video[b], 0, 0, H, W);
   const int lane = threadIdx.x & 31;
   int ci = 0, cu = 0;                                  // lane t < T: intersection / union-outside-target of threshold t
   // warp-uniform loop: each warp takes 32 consecutive pixels of the rectangle per iteration
@@ -2054,16 +2066,18 @@ void launch_paste_labels_iou(const float* masks, int side, const double* maps, c
 }
 
 void launch_mask_iou(const float* masks, int side, const double* maps, const uint8_t* anno, const int32_t* video, int B,
-                     int H, int W, const double* thrs, int T, int32_t* counts, cudaStream_t st) {
+                     int H, int W, const double* thrs, int T, int32_t* counts, cudaStream_t st,
+                     const sm_image_desc* desc) {
   SMK_CHECK(T >= 1 && T <= MI_MAX_T, "1 <= T <= 32 thresholds");
   SMK_CUDA(cudaMemsetAsync(counts, 0, (size_t)B * T * 2 * sizeof(int32_t), st));
   const size_t HW = (size_t)H * W;
   mask_iou_target_kernel<<<dim3((unsigned)((HW + MI_TARGET_BYTES - 1) / MI_TARGET_BYTES), B), MI_THREADS, 0, st>>>(
-      anno, video, B, HW, thrs, T, counts);
+      anno, video, B, HW, thrs, T, counts, desc);
   SMK_CUDA(cudaGetLastError());
   // a pasted 127x127 mask spans some 10^4..10^5 pixels: 16 blocks per stream keep every SM busy at a few streams
   const int per_stream = (int)std::min<size_t>(16, (HW + MI_THREADS * 8 - 1) / (MI_THREADS * 8));
-  mask_iou_rect_kernel<<<dim3(per_stream, B), MI_THREADS, 0, st>>>(masks, side, maps, anno, video, H, W, thrs, T, counts);
+  mask_iou_rect_kernel<<<dim3(per_stream, B), MI_THREADS, 0, st>>>(masks, side, maps, anno, video, H, W, thrs, T, counts,
+                                                                 desc);
   SMK_CUDA(cudaGetLastError());
 }
 

@@ -371,6 +371,66 @@ def _mask_iou(masks, maps, anno, video, thrs) -> torch.Tensor:
     return out
 
 
+def mask_iou_ragged(masks, maps, anno, table, video, thrs) -> torch.Tensor:
+    """`mask_iou` against annotations of different sizes (C ABI `sm_mask_iou_ragged`): anno a flat uint8 CUDA buffer
+    holding the annotation images back to back, table their host sm_image_desc rows (`tracker.IMAGE_DESC`: offset, h,
+    w per image), video int [B]: the image stream b is scored against.  Each stream's counts equal `mask_iou` on its
+    image alone.  The checks read `table`, `video` and `thrs` on the host: every image inside the buffer, every image
+    a stream reads at least 1 x 1."""
+    from .tracker import IMAGE_DESC
+    if not (torch.is_tensor(masks) and masks.is_cuda and masks.dtype == torch.float32 and masks.dim() == 3
+            and masks.shape[1] == masks.shape[2]):
+        raise ValueError("masks must be a float32 CUDA tensor [B, side, side]")
+    if not (torch.is_tensor(anno) and anno.is_cuda and anno.dtype == torch.uint8 and anno.dim() == 1):
+        raise ValueError("anno must be a flat uint8 CUDA tensor (the packed annotation images)")
+    B = int(masks.shape[0])
+    m = torch.as_tensor(maps)
+    if m.dtype != torch.float64 or tuple(m.shape) != (B, 6):
+        raise ValueError(f"maps must be float64 [{B}, 6]")
+    tb = np.asarray(table)
+    if tb.dtype != IMAGE_DESC or tb.ndim != 1 or tb.size == 0:
+        raise ValueError("table must be a non-empty 1-D array of sm_image_desc rows (tracker.IMAGE_DESC)")
+    off, h, w = tb["offset"].astype(np.int64), tb["h"].astype(np.int64), tb["w"].astype(np.int64)
+    if (off < 0).any() or (h < 0).any() or (w < 0).any() or (off + h * w > anno.numel()).any():
+        raise ValueError(f"every image must lie inside the {anno.numel()}-byte buffer with h, w >= 0")
+    if (h * w > 2 ** 31 - 1).any():
+        raise ValueError("image too large for int32 counts")
+    v = np.asarray(video.cpu() if torch.is_tensor(video) else video)
+    if v.shape != (B,) or not np.issubdtype(v.dtype, np.integer):
+        raise ValueError(f"video must be an integer array [{B}]")
+    if B and ((v < 0) | (v >= tb.size)).any():
+        raise ValueError(f"video entries must lie in [0, {tb.size})")
+    if B and ((h[v] < 1) | (w[v] < 1)).any():
+        raise ValueError("a stream reads an empty image")
+    t = np.asarray(thrs.cpu() if torch.is_tensor(thrs) else thrs, dtype=np.float64).reshape(-1)
+    if not 1 <= t.size <= 32:
+        raise ValueError("1 to 32 thresholds expected")
+    if not (t >= -1.0).all():
+        raise ValueError("thresholds must be >= -1 (pixels the mask misses have the value -1)")
+    dev = masks.device
+    if B == 0:
+        return torch.zeros(0, t.size, 2, dtype=torch.int32, device=dev)
+    desc = torch.from_numpy(tb.view(np.uint8).copy()).to(dev)
+    return _mask_iou_ragged(masks, m.to(dev), anno, desc, torch.as_tensor(v.astype(np.int32), device=dev),
+                            (int(h.max()), int(w.max())), torch.as_tensor(t, device=dev))
+
+
+def _mask_iou_ragged(masks, maps, anno, desc, video, max_hw, thrs) -> torch.Tensor:
+    """`mask_iou_ragged` without the host-side checks: anno the packed uint8 CUDA buffer, desc its device sm_image_desc
+    table, video int32 CUDA [B], max_hw = (max_h, max_w) bounding every image a stream reads, thrs float64 CUDA."""
+    lib = _lib.load()
+    dev = masks.device
+    masks, maps, video, thrs = (t.contiguous() for t in (masks, maps, video, thrs))
+    B, side = int(masks.shape[0]), int(masks.shape[-1])
+    T = int(thrs.numel())
+    out = torch.empty(B, T, 2, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.sm_mask_iou_ragged(masks.data_ptr(), side, maps.data_ptr(), anno.contiguous().data_ptr(),
+                                          desc.data_ptr(), video.data_ptr(), B, int(max_hw[0]), int(max_hw[1]),
+                                          thrs.data_ptr(), T, out.data_ptr(), _stream(dev)))
+    return out
+
+
 VOT_COORD_LIMIT = 2.0 ** 20       # |coordinate| bound of sm_vot_overlap's precondition
 
 

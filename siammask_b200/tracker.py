@@ -417,6 +417,37 @@ class BatchTracker:
             self.avg.index_copy_(0, r_dev, avg)
 
     @torch.no_grad()
+    def set_frame_index(self, ids, frame_index) -> None:
+        """Point running streams at other entries of the frame lists of later calls: stream ids[i] reads frame
+        frame_index[i] from now on (a queue whose frame list changes as sequences come and go).  The frame-index table
+        is uploaded only when an index changes, asynchronously from pinned memory, so the call never waits for the
+        device; the active set and every other table stay as they are.  The size check of `track` still binds each
+        stream to the size it was added with."""
+        ids = [int(i) for i in np.asarray(ids).reshape(-1)]
+        idx = [int(i) for i in np.asarray(frame_index).reshape(-1)]
+        if len(idx) != len(ids):
+            raise ValueError("one frame index per stream id expected")
+        unknown = set(ids) - set(self._ids)
+        if unknown:
+            raise ValueError(f"unknown stream ids {sorted(unknown)}")
+        if len(set(ids)) != len(ids):
+            raise ValueError("stream ids must be unique")
+        if any(i < 0 for i in idx):
+            raise ValueError("frame indices must be >= 0")
+        row = {i: r for r, i in enumerate(self._ids)}
+        fidx = list(self._fidx)
+        for i, v in zip(ids, idx):
+            fidx[row[i]] = v
+        if fidx == self._fidx:
+            return
+        self._fidx = fidx
+        self._max_fidx = max(fidx)
+        host = torch.tensor(fidx, dtype=torch.int32)
+        if torch.device(self.dev).type == "cuda":
+            host = host.pin_memory()                # the copy queues without waiting for the device
+        self._fidx_dev = host.to(self.dev, non_blocking=True)
+
+    @torch.no_grad()
     def remove(self, ids) -> None:
         """Stop tracking the given streams and free their engine slots (a later `add` may reuse them)."""
         drop = {int(i) for i in np.asarray(ids).reshape(-1)}

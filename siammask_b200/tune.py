@@ -8,6 +8,10 @@ frames in place and carries combination k in the tracker's per-stream hyper-para
 `sm_tracker_update_hp`).  Each frame is scored by one fused paste-back + count kernel (`sm_mask_iou`) without
 materialising a frame-sized mask per stream, and the IoU rows stay on the device until `ParamSweep.result`.
 
+`open_queue` / `needed` / `step` run a sweep of any size, with videos of different lengths and frame sizes, through a
+queue of streams (`schedule.Scheduler`); each step is scored by `sm_mask_iou_ragged` over the step's packed
+annotations.
+
 The rotated box of `siamese_track` (contours / minAreaRect) is not computed: tune_vos never scores it.
 """
 from __future__ import annotations
@@ -16,7 +20,8 @@ import numpy as np
 import torch
 
 from . import ops
-from .tracker import BatchTracker, TrackerParams
+from .schedule import Scheduler
+from .tracker import BatchTracker, FramePacker, TrackerParams
 
 # tools/tune_vos.py's default ranges (--penalty-k 0.0,0.1,0.03 --window-influence 0.3,0.5,0.04 --lr 0.8,1.01,0.05)
 # and IouMeter thresholds: a 4 x 5 x 5 grid, 11 thresholds
@@ -80,6 +85,7 @@ class ParamSweep:
         self._thrs_dev = torch.as_tensor(self.thrs, device=self.dev)
         self.G = 0
         self.f = self.T = 0
+        self._sched = None
 
     @property
     def K(self) -> int:
@@ -103,6 +109,7 @@ class ParamSweep:
         if G * K > net.max_batch or G * K > net.num_slots - self.tracker.slot0:
             raise ValueError(f"{G} videos x {K} combinations = {G * K} streams exceed the engine's max_batch "
                              f"({net.max_batch}) or free slots ({net.num_slots - self.tracker.slot0}); split the grid")
+        self._sched = None
         video = np.repeat(np.arange(G), K)
         self.tracker._clear()
         self.tracker.add(fr, np.repeat(boxes, K, axis=0), frame_index=video, hp=np.tile(self.combos, (G, 1)))
@@ -117,6 +124,8 @@ class ParamSweep:
         of this frame, required when it is scored (0 < f < T-1).  The frame's IoU rows (float32(intersection / union),
         1 where the union is empty) are written into a device buffer.  Returns the tracker's `TrackResult`."""
         f = self.f
+        if self._sched is not None:
+            raise ValueError("a queue run advances with step(); frame() belongs to open()")
         if not 1 <= f < self.T:
             raise ValueError("call open() first; at most num_frames - 1 frames follow it")
         fr = self.tracker._input(frames)
@@ -142,8 +151,144 @@ class ParamSweep:
 
     def result(self):
         """One D2H copy.  Returns (iou_list float32 [G,K,T] = IouMeter.value('mean') of every stream, per-frame IoU
-        float32 [num_frames-2, G, K, T]); rows of frames not tracked yet are 0, as in a partly filled IouMeter."""
-        per_frame = self._iou.cpu().numpy()
+        float32 [num_frames-2, G, K, T]); rows of frames not tracked yet are 0, as in a partly filled IouMeter.  After
+        a queue run the per-frame IoU is a list of G arrays float32 [T_g-2, K, T], one per video."""
         G, K, n = self.G, self.K, self.thrs.size
+        if self._sched is not None:
+            flat = self._iou.cpu().numpy()
+            rows = [flat[o:o + m] for o, m in zip(self._off, self._vT - 2)]
+            means = np.stack([iou_mean(r) for r in rows]).reshape(G, K, n)
+            return means, [np.stack(rows[g * K:(g + 1) * K], 1) for g in range(G)]
+        per_frame = self._iou.cpu().numpy()
         means = np.stack([iou_mean(per_frame[:, s]) for s in range(G * K)]).reshape(G, K, n)
         return means, per_frame.reshape(-1, G, K, n)
+
+    # ------------------------------------------------------------------ queue mode
+    @torch.no_grad()
+    def open_queue(self, boxes_xywh, num_frames):
+        """Queues every (video, combination) stream of a sweep of any size through the engine (`schedule.Scheduler`,
+        as `VotRunner.open_queue`): videos of different lengths and frame sizes, at most min(max_batch, free slots)
+        streams active, a stream admitted the step after a slot frees.  boxes_xywh: [G,4] top-left x, y, w, h of each
+        video's target on its frame 0; num_frames: [G] the videos' lengths (each >= 3).  Each stream scores its own
+        video's frames 1 .. T_g-2, as tune_vos's IouMeter(thrs, len(ims) - 2).  Drive it with
+
+            while sweep.pending:
+                need = sweep.needed()
+                sweep.step([frames[g][t] for g, t in need],
+                           [annos[g][t] if 0 < t < T[g] - 1 else None for g, t in need])
+
+        and read `result()`: iou_list [G,K,T] and one per-frame array [T_g-2, K, T] per video."""
+        boxes = np.asarray(boxes_xywh, dtype=np.float64)
+        T = np.asarray(num_frames).reshape(-1)
+        G, K = len(T), self.K
+        if G == 0:
+            raise ValueError("open_queue needs at least one video")
+        if boxes.shape != (G, 4):
+            raise ValueError(f"boxes_xywh must be [{G}, 4]")
+        if not np.issubdtype(T.dtype, np.integer) or (T < 3).any():
+            raise ValueError("num_frames must be integers >= 3 (the first and the last frame are not scored)")
+        net = self.tracker.net
+        cap = min(net.max_batch, net.num_slots - self.tracker.slot0)
+        if cap < 1:
+            raise ValueError("the engine has no free slot")
+        self._sched = Scheduler(T, K, cap)
+        self._plan = self._sched.step()
+        self._boxes, self._hw = boxes, [None] * G
+        self._qvideo = np.repeat(np.arange(G), K)
+        self._vT = T.astype(np.int64)[self._qvideo]
+        self._off = np.concatenate([[0], np.cumsum(self._vT - 2)[:-1]])      # stream s owns IoU rows off[s] ..
+        self._iou = torch.zeros(int((self._vT - 2).sum()), self.thrs.size, dtype=torch.float32, device=self.dev)
+        self._admit = np.full(G * K, -1, np.int64)
+        self._annos = FramePacker(self.dev)
+        self.tracker._clear()
+        self._stream_of, self._id_of = {}, [None] * (G * K)
+        self.G, self.T, self.f = G, T, 0
+        self._index_rows()
+        return self
+
+    @property
+    def pending(self) -> bool:
+        """Whether a queue run has steps left."""
+        return self._sched is not None and self._plan is not None
+
+    def needed(self) -> list:
+        """The distinct (video, frame) pairs the next `step` reads, in the order its frame and annotation lists follow."""
+        if not self.pending:
+            raise ValueError("no queue step is pending: call open_queue() first; the run has finished")
+        return list(self._plan.need)
+
+    def _index_rows(self):
+        """Each active tracker row's stream and the IoU row it writes at step 0 (add the step): uploaded only when the
+        set of active streams changes."""
+        self._row_streams = [self._stream_of[i] for i in self.tracker.ids]
+        s = np.asarray(self._row_streams, np.int64)
+        self._row_dest = torch.as_tensor(self._off[s] - 1 - self._admit[s], dtype=torch.long, device=self.dev)
+
+    @torch.no_grad()
+    def step(self, frames, annos):
+        """One step of a queue run: frames[i] / annos[i] are frame t of video g and its uint8 [H,W] annotation for
+        (g, t) = needed()[i]; an annotation is required where 0 < t < T_g - 1 and ignored elsewhere (None will do).
+        Tracks every running stream one frame of its own video, scores it with `sm_mask_iou_ragged` against the packed
+        annotations, retires the streams whose video ends, then templates the admitted streams from their frame 0.
+        Returns the tracker's `TrackResult` of the streams that tracked a frame, or None when none did."""
+        if not self.pending:
+            raise ValueError("no queue step is pending: call open_queue() first; the run has finished")
+        st, f, bt = self._plan, self.f, self.tracker
+        n = len(st.need)
+        if not isinstance(frames, (list, tuple)) or len(frames) != n:
+            raise ValueError(f"frames must be a list of {n} frames, one per needed() entry")
+        if not isinstance(annos, (list, tuple)) or len(annos) != n:
+            raise ValueError(f"annos must be a list of {n} entries, one per needed() entry")
+        scored = [0 < t < self.T[g] - 1 for g, t in st.need]
+        fr = bt._input(frames)
+        for i, (g, t) in enumerate(st.need):
+            hw = fr.shapes[i]
+            if self._hw[g] is not None and hw != self._hw[g]:
+                h, w = hw if hw is not None else (0, 0)
+                raise ValueError(f"frame {t} of video {g} is {h}x{w}, its frame 0 {self._hw[g][0]}x{self._hw[g][1]}")
+            if scored[i]:
+                a = annos[i]
+                if a is None:
+                    raise ValueError(f"frame {t} of video {g} is scored: its annotation is required")
+                if a.dtype not in (np.uint8, torch.uint8) or tuple(a.shape) != tuple(hw):
+                    raise ValueError(f"the annotation of frame {t} of video {g} must be uint8 [{hw[0]},{hw[1]}]")
+        r = None
+        if st.track:
+            want = [st.entry[self._stream_of[i]] for i in bt.ids]
+            if want != bt._fidx:                        # the frame list moved: only after admissions or departures
+                bt.set_frame_index(bt.ids, want)
+            r = bt.track(fr, mask=True, refine=self.p.out_size == 127, paste=False)
+            anno = self._annos.pack([a if s else None for a, s in zip(annos, scored)], 1)
+            masks, maps, video, dest = r.extras["mask_prob"], r.extras["maps"], bt._fidx_dev, self._row_dest + f
+            last = set(st.retire)
+            if last:                                    # rows on their video's last frame are not scored
+                keep = [j for j, s in enumerate(self._row_streams) if s not in last]
+                sel = torch.tensor(keep, dtype=torch.long, device=self.dev)
+                masks, maps, video, dest = masks[sel], maps[sel], video[sel], dest[sel]
+            if dest.numel():
+                hs, ws = zip(*[anno.shapes[i] for i in range(n) if scored[i]])
+                cnt = ops._mask_iou_ragged(masks, maps, anno.data, anno.desc, video, (max(hs), max(ws)),
+                                           self._thrs_dev)
+                inter, union = cnt[..., 0].double(), cnt[..., 1].double()
+                iou = torch.where(union > 0, (inter / union).float(), torch.ones_like(union, dtype=torch.float32))
+                self._iou.index_copy_(0, dest, iou)
+        gone = [self._id_of[s] for s in st.retire if self._id_of[s] is not None]
+        if gone:
+            bt.remove(gone)
+        for s in st.admit:
+            g = int(self._qvideo[s])
+            if self._hw[g] is None:
+                self._hw[g] = fr.shapes[st.entry[s]]
+            self._admit[s] = f
+        new = list(st.admit)
+        if new:
+            K = self.K
+            ids = bt.add(fr, self._boxes[self._qvideo[new]], frame_index=[st.entry[s] for s in new],
+                         hp=self.combos[[s % K for s in new]])
+            for s, i in zip(new, ids):
+                self._stream_of[i], self._id_of[s] = s, i
+        if gone or new:
+            self._index_rows()
+        self.f += 1
+        self._plan = self._sched.step() if not self._sched.done else None
+        return r

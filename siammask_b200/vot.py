@@ -24,6 +24,10 @@ upload small tables (the template rows, the active set) once.
 Sequences of different frame sizes run in one batch: pass each frame as a list of G frames (`BatchTracker` packs them;
 the entry of a sequence that has ended may be None).
 
+A run larger than the engine goes through `open_queue` / `needed` / `step`: the (sequence, combination) streams are
+queued (`schedule.Scheduler`), a freed slot is refilled on the next step, and each stream runs the same protocol from
+its own frame 0; the step's frame list holds one entry per distinct (sequence, frame).
+
 `VotScore` scores finished runs the way tools/eval.py does for VOT2016/2017/2018/2019 ('all' tag): pysot's
 AccuracyRobustnessBenchmark (accuracy, robustness, lost number) and EAOBenchmark (expected-overlap curve and EAO), for
 every hyper-parameter combination at once, from the runner's device record and without result files:
@@ -43,6 +47,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .schedule import Scheduler
 from .tracker import BatchTracker, TrackerParams
 
 # tools/tune_vot.py's argparse defaults: a 9 x 14 x 3 grid of (penalty_k, window_influence, lr)
@@ -129,10 +134,33 @@ class VotRunner:
             self.combos = c
         self.G = 0
         self.f = 0
+        self._sched = None
 
     @property
     def K(self) -> int:
         return 1 if self.combos is None else int(self.combos.shape[0])
+
+    @property
+    def ended(self) -> bool:
+        """Whether every stream of the run has tracked its sequence's last frame."""
+        if self._sched is not None:
+            return self._plan is None
+        return self.G > 0 and bool((self.T <= self.f).all())
+
+    def _load_gt(self, gt) -> int:
+        """Checks and uploads every gt row and computes get_axis_aligned_bbox of each on the host, in the reference's
+        arithmetic: self._init (cx, cy, w, h) [G, Tmax, 4]; returns G."""
+        gts = check_gt(gt)
+        self.T = np.array([a.shape[0] for a in gts])
+        Tmax = int(self.T.max()) if gts else 0
+        self._init = np.zeros((len(gts), Tmax, 4))
+        polys = np.zeros((len(gts), Tmax, 8), np.float32)
+        for g, a in enumerate(gts):
+            with np.errstate(divide="ignore", invalid="ignore"):
+                self._init[g, :len(a)] = [get_axis_aligned_bbox(row) for row in a]
+            polys[g, :len(a)] = a                            # Polygon() stores C floats
+        self._gt = torch.from_numpy(polys).to(self.dev)
+        return len(gts)
 
     @torch.no_grad()
     def open(self, frames0, gt):
@@ -146,23 +174,16 @@ class VotRunner:
             raise ValueError("frames0 must hold frame 0 of every sequence")
         G, self._hw = len(fr.shapes), list(fr.shapes)
         K = self.K
-        gts = check_gt(gt)
-        if len(gts) != G:
+        if len(check_gt(gt)) != G:
             raise ValueError(f"one gt array per sequence expected ({G})")
         net, S = self.tracker.net, G * K
         if S > net.max_batch or S > net.num_slots - self.tracker.slot0:
             raise ValueError(f"{G} sequences x {K} combinations = {S} streams exceed the engine's max_batch "
-                             f"({net.max_batch}) or free slots ({net.num_slots - self.tracker.slot0}); split the run")
-        self.T = np.array([a.shape[0] for a in gts])
+                             f"({net.max_batch}) or free slots ({net.num_slots - self.tracker.slot0}); split the run, "
+                             "or queue it with open_queue()")
+        self._sched = None
+        self._load_gt(gt)
         Tmax = int(self.T.max())
-        # get_axis_aligned_bbox of every gt row, on the host in the reference's arithmetic: (cx, cy, w, h) [G, Tmax, 4]
-        self._init = np.zeros((G, Tmax, 4))
-        polys = np.zeros((G, Tmax, 8), np.float32)
-        for g, a in enumerate(gts):
-            with np.errstate(divide="ignore", invalid="ignore"):
-                self._init[g, :len(a)] = [get_axis_aligned_bbox(row) for row in a]
-            polys[g, :len(a)] = a                            # Polygon() stores C floats
-        self._gt = torch.from_numpy(polys).to(self.dev)
         video = np.repeat(np.arange(G), K)
         self._video = video
         c0 = self._init[video, 0]
@@ -185,13 +206,15 @@ class VotRunner:
         return self
 
     def _index_rows(self):
-        """Stream and sequence of each active tracker row: a host list and device indices.  The upload waits for the
-        copy, so it runs only when the set of active streams changes."""
+        """Stream and sequence of each active tracker row (and, in a queue run, its admission step): a host list and
+        device indices.  The upload waits for the copy, so it runs only when the set of active streams changes."""
         self._row_streams = [self._stream_of[i] for i in self.tracker.ids]
         self._row_dev = torch.tensor(self._row_streams, dtype=torch.long, device=self.dev)
         self._row_video = torch.as_tensor(self._video[self._row_streams], dtype=torch.long, device=self.dev)
         wh = [self._hw[self._video[s]][::-1] for s in self._row_streams]     # each row's own (W, H)
         self._row_wh = torch.tensor(wh, dtype=torch.int32, device=self.dev).reshape(-1, 2)
+        if self._sched is not None:
+            self._row_admit = torch.as_tensor(self._admit[self._row_streams], dtype=torch.long, device=self.dev)
 
     def _retire(self):
         """Step 5: streams whose sequence ends with frame self.f leave the batch."""
@@ -207,6 +230,8 @@ class VotRunner:
         frame of the right size will do).  Returns the tracker's `TrackResult` of the streams that were active, whose
         rows are skipped or re-initialised streams too."""
         f = self.f
+        if self._sched is not None:
+            raise ValueError("a queue run advances with step(); frame() belongs to open()")
         if self.G == 0 or self.tracker.N == 0:
             raise ValueError("call open() first; every sequence has ended")
         fr = self.tracker._input(frames)
@@ -264,9 +289,153 @@ class VotRunner:
         int [G, K]."""
         rec = self._rec.cpu().numpy()
         G, K = self.G, self.K
-        n = np.minimum(self.T, self.f)
-        regions = [[regions_from_record(rec[:, g * K + k], int(n[g])) for k in range(K)] for g in range(G)]
+        if self._sched is None:
+            n = np.repeat(np.minimum(self.T, self.f), K)
+        else:                                           # frames 0 .. f - admission step - 1 of each admitted stream
+            n = np.where(self._admit >= 0, np.minimum(self._video_T, self.f - self._admit), 0)
+        regions = [[regions_from_record(rec[:, g * K + k], int(n[g * K + k])) for k in range(K)] for g in range(G)]
         return regions, rec[-1, :, 0].astype(np.int64).reshape(G, K)
+
+    # ------------------------------------------------------------------ queue mode
+    @torch.no_grad()
+    def open_queue(self, gt):
+        """Queues every (sequence, combination) stream of a run of any size through the engine (`schedule.Scheduler`):
+        at most min(max_batch, free slots) streams are active, and a stream is admitted the step after a slot frees,
+        sequences by descending length, then combinations in order.  Each stream tracks its own sequence from its own
+        frame 0; record, codes, overlap (within its sequence's (W, H)), lost_times and the failure -> skip 4 -> re-init
+        schedule are per stream, exactly as `open` / `frame` run them.  gt: G float64 arrays [T_g, 8].  Drive it with
+
+            while runner.pending:
+                runner.step([frames[g][t] for g, t in runner.needed()])
+
+        Frames may differ in size between sequences (not within one); `result()` and `VotScore.add` then work as for
+        `open`, stream (g, k) being row g*K + k."""
+        G, K = self._load_gt(gt), self.K
+        if G == 0:
+            raise ValueError("open_queue needs at least one sequence")
+        net = self.tracker.net
+        cap = min(net.max_batch, net.num_slots - self.tracker.slot0)
+        if cap < 1:
+            raise ValueError("the engine has no free slot")
+        S, Tmax = G * K, int(self.T.max())
+        self._sched = Scheduler(self.T, K, cap)
+        self._plan = self._sched.step()
+        self._hw = [None] * G                           # each sequence's (H, W), from its frame 0
+        self._video = np.repeat(np.arange(G), K)
+        self._video_T = self.T[self._video]
+        self._admit = np.full(S, -1, np.int64)          # the step at which each stream was templated
+        self.tracker._clear()
+        self._stream_of, self._id_of = {}, [None] * S
+        self._rec = torch.zeros(Tmax + 1, S, 5, dtype=torch.float64, device=self.dev)
+        self._rec[0, :, 0] = CODE_INIT
+        self._start = torch.zeros(S, dtype=torch.int32, device=self.dev)         # in the stream's own frames
+        self._flags = torch.zeros(S, dtype=torch.uint8, device=self.dev)
+        self._pinned = [torch.zeros(S, dtype=torch.uint8).pin_memory() for _ in range(SKIP_FRAMES + 1)]
+        self._events = [None] * (SKIP_FRAMES + 1)       # (step, event) of the flags in each pinned buffer
+        self.G, self.f = G, 0
+        self._index_rows()
+        return self
+
+    @property
+    def pending(self) -> bool:
+        """Whether a queue run has steps left."""
+        return self._sched is not None and self._plan is not None
+
+    def needed(self) -> list:
+        """The distinct (sequence, frame) pairs the next `step` reads, in the order its frame list must follow."""
+        if not self.pending:
+            raise ValueError("no queue step is pending: call open_queue() first; the run has finished")
+        return list(self._plan.need)
+
+    @torch.no_grad()
+    def step(self, frames):
+        """One step of a queue run: frames[i] is frame t of sequence g for (g, t) = needed()[i] (uint8 [H,W,3] numpy
+        arrays or CUDA tensors).  Tracks every running stream one frame of its own sequence, scores it, re-initialises
+        the streams lost 5 frames earlier, retires the streams whose sequence ends, then templates the admitted streams
+        from their frame 0.  A step waits for the device only when it re-initialises, admits or retires streams.
+        Returns the tracker's `TrackResult` of the streams that tracked a frame, or None when none did."""
+        if not self.pending:
+            raise ValueError("no queue step is pending: call open_queue() first; the run has finished")
+        st, f, bt = self._plan, self.f, self.tracker
+        if not isinstance(frames, (list, tuple)) or len(frames) != len(st.need):
+            raise ValueError(f"frames must be a list of {len(st.need)} frames, one per needed() entry")
+        fr = bt._input(frames)
+        for i, (g, t) in enumerate(st.need):
+            if self._hw[g] is not None and fr.shapes[i] != self._hw[g]:
+                h, w = fr.shapes[i] if fr.shapes[i] is not None else (0, 0)
+                raise ValueError(f"frame {t} of sequence {g} is {h}x{w}, its frame 0 {self._hw[g][0]}x{self._hw[g][1]}")
+        r = None
+        if st.track:
+            want = [st.entry[self._stream_of[i]] for i in bt.ids]
+            if want != bt._fidx:                        # the frame list moved: only after admissions or departures
+                bt.set_frame_index(bt.ids, want)
+            r = self._track(fr, f)
+        gone = [self._id_of[s] for s in st.retire if self._id_of[s] is not None]
+        if gone:
+            bt.remove(gone)
+        new = [s for s in st.admit if self._video_T[s] > 1]      # a one-frame sequence is its frame 0's init alone
+        for s in st.admit:
+            g = int(self._video[s])
+            if self._hw[g] is None:
+                self._hw[g] = fr.shapes[st.entry[s]]
+            self._admit[s] = f
+        if new:
+            c0 = self._init[self._video[new], 0]
+            K = self.K
+            hp = None if self.combos is None else self.combos[[s % K for s in new]]
+            ids = bt.add_state(fr, c0[:, 0:2], c0[:, 2:4], frame_index=[st.entry[s] for s in new], hp=hp)
+            for s, i in zip(new, ids):
+                self._stream_of[i], self._id_of[s] = s, i
+        if gone or new:
+            self._index_rows()
+        self.f += 1
+        self._plan = self._sched.step() if not self._sched.done else None
+        return r
+
+    def _track(self, fr, f: int):
+        """Steps 1-4 of `frame` for the running streams of a queue step f: each row at its own frame t = f - admission
+        step, its record row t and its gt row t."""
+        rows = self._row_dev
+        S, Tmax = self._rec.shape[1], self._gt.shape[1]
+        r = self.tracker.track(fr, mask=False)
+        st = r.state
+        x0 = st[:, 0] - st[:, 2] / 2
+        y0 = st[:, 1] - st[:, 3] / 2
+        x1, y1 = x0 + st[:, 2], y0 + st[:, 3]
+        loc = torch.stack([x0, y0, st[:, 2], st[:, 3]], 1)
+        pred = torch.stack([x0, y0, x1, y0, x1, y1, x0, y1], 1).float()
+        t = f - self._row_admit                          # each row's own frame, on the device
+        ov = ops._vot_overlap_sized(self._gt.view(-1, 8)[self._row_video * Tmax + t], pred, self._row_wh)
+        start = self._start[rows].long()
+        tracking = start < t
+        lost = tracking & (ov == 0)
+        code = torch.where(start == t, CODE_INIT, torch.where(lost, CODE_LOST, CODE_LOCATION * tracking.long()))
+        rec = self._rec.view(-1, 5)
+        at = t * S + rows
+        rec[at, 0] = code.double()
+        rec[at, 1:5] = torch.where(tracking & ~lost, 1, 0).unsqueeze(1) * loc
+        self._rec[-1, rows, 0] += lost.double()
+        self._start[rows] = torch.where(lost, t + SKIP_FRAMES, start).int()
+        self._flags.zero_()
+        self._flags[rows] = lost.to(torch.uint8)
+        slot = f % len(self._pinned)
+        self._pinned[slot].copy_(self._flags, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(self.dev))
+        self._events[slot] = (f, ev)
+        # re-initialise the streams lost at step f - 5 (every active stream advanced 5 frames since), from the gt of
+        # each one's own frame
+        old = self._events[(f - SKIP_FRAMES) % len(self._pinned)]
+        if old is not None and old[0] == f - SKIP_FRAMES:
+            if not old[1].query():                       # 5 steps old: as good as always complete
+                old[1].synchronize()
+            active = set(self._row_streams)
+            again = [int(s) for s in np.nonzero(self._pinned[(f - SKIP_FRAMES) % len(self._pinned)].numpy())[0]
+                     if int(s) in active]
+            if again:
+                c = self._init[self._video[again], f - self._admit[again]]
+                self.tracker.reinit([self._id_of[s] for s in again], fr, c[:, 0:2], c[:, 2:4])
+        return r
 
 
 
@@ -323,7 +492,7 @@ class VotScore:
         combo_index[k] (default k).  Reads the runner's device record in place; no host sync."""
         if runner.G == 0:
             raise ValueError("the runner has not been opened")
-        if (runner.T > runner.f).any():
+        if not runner.ended:
             raise ValueError(f"every sequence must have ended: frame {runner.f} of lengths {runner.T.tolist()}")
         sizes = [(int(h), int(w)) for h, w in runner._hw]
         self._add(runner._rec, runner._gt, runner.T, sizes, runner.K, combo_index)
