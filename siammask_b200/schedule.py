@@ -1,5 +1,5 @@
-"""Queue scheduling of (sequence, combination) streams through one engine: the admission plan `VotRunner.open_queue`
-and `ParamSweep.open_queue` follow.
+"""Queue scheduling of (sequence, combination) streams through one engine: the admission plan `VotRunner.open_queue`,
+`ParamSweep.open_queue` and `VideoSegmenter.open_queue` follow.
 
 A benchmark run is G sequences x K hyper-parameter combinations, one tracker stream each, and the engine holds at most
 `capacity` of them.  Run in fixed chunks, every stream of a chunk starts on frame 0 and the batch only shrinks, so a
@@ -7,8 +7,11 @@ chunk lasts as long as its longest sequence.  The queue instead refills a slot a
 
   - streams are admitted in a fixed order, sequences by descending length (ties by index), each sequence's
     combinations in order;
-  - at step f, as many waiting streams are admitted as there are free slots: the slots that streams leaving at step
-    f-1 freed (and, at step 0, all of them).  An admitted stream is templated from frame 0 of its sequence at step f
+  - at step f, waiting streams are admitted in that order while the next one fits into the free slots: the slots
+    that streams leaving at step f-1 freed (and, at step 0, all of them).  A stream holds one slot, or its sequence's
+    width (`widths`: a video whose objects are tracked at once holds as many slots as it has objects at its peak) from
+    its admission until it leaves.  A stream that does not fit waits, and so does every stream behind it: the plan
+    stays a pure function of the lengths, widths and capacity.  An admitted stream is templated from frame 0 of its sequence at step f
     and tracks frame t of its own sequence at step f + t;
   - a stream leaves after the step that reads its sequence's last frame.
 
@@ -39,15 +42,23 @@ class Step:
 
 class Scheduler:
     """The plan for sequences of `lengths` frames x K combinations through `capacity` slots, one `Step` per call of
-    `step()`; stream (g, k) is number g*K + k."""
+    `step()`; stream (g, k) is number g*K + k.  widths (optional): the slots each stream of sequence g holds, one
+    integer >= 1 per sequence (default 1); a width above the capacity is a ValueError."""
 
-    def __init__(self, lengths, K: int, capacity: int):
+    def __init__(self, lengths, K: int, capacity: int, widths=None):
         T = np.asarray(lengths).reshape(-1)
         if T.size == 0 or not np.issubdtype(T.dtype, np.integer) or (T < 1).any():
             raise ValueError("lengths must be one integer >= 1 per sequence (every sequence has a frame 0)")
         if int(K) < 1 or int(capacity) < 1:
             raise ValueError("K and capacity must be >= 1")
+        w = np.ones(T.size, np.int64) if widths is None else np.asarray(widths).reshape(-1)
+        if w.size != T.size or not np.issubdtype(w.dtype, np.integer) or (w < 1).any():
+            raise ValueError("widths must be one integer >= 1 per sequence")
+        if (w > int(capacity)).any():
+            g = int(np.argmax(w > int(capacity)))
+            raise ValueError(f"sequence {g} needs {int(w[g])} slots at once; the engine has {int(capacity)}")
         self.T, self.K, self.capacity = T.astype(np.int64), int(K), int(capacity)
+        self.width = w.astype(np.int64)
         seqs = sorted(range(T.size), key=lambda g: (-int(T[g]), g))
         self.order = [g * self.K + k for g in seqs for k in range(self.K)]
         self._next = 0                          # position in `order` of the next stream to admit
@@ -63,8 +74,11 @@ class Scheduler:
         if self.done:
             raise ValueError("every stream has finished")
         f = self.f
-        new = self.order[self._next:self._next + self.capacity - self._active]
-        self._next += len(new)
+        new, free = [], self.capacity - self._active
+        while self._next < len(self.order) and self.width[self.order[self._next] // self.K] <= free:
+            new.append(self.order[self._next])
+            free -= int(self.width[self.order[self._next] // self.K])
+            self._next += 1
         track = [s for _, _, streams in self._groups for s in streams]
         for s in new:
             g = s // self.K
@@ -72,20 +86,20 @@ class Scheduler:
                 self._groups[-1][2].append(s)
             else:
                 self._groups.append((g, f, [s]))
-        self._active += len(new)
+        self._active = self.capacity - free
         need = [(g, f - a) for g, a, _ in self._groups]
         entry = {s: i for i, (_, _, streams) in enumerate(self._groups) for s in streams}
         ending = [i for i, (g, a, _) in enumerate(self._groups) if f - a == self.T[g] - 1]
         retire = [s for i in ending for s in self._groups[i][2]]
         self._groups = [grp for i, grp in enumerate(self._groups) if i not in set(ending)]
-        self._active -= len(retire)
+        self._active -= int(sum(self.width[s // self.K] for s in retire))
         self.f += 1
         return Step(need, entry, track, list(new), retire)
 
 
-def plan(lengths, K: int, capacity: int) -> list[Step]:
-    """Every step of the queue, as a pure function of the lengths."""
-    s = Scheduler(lengths, K, capacity)
+def plan(lengths, K: int, capacity: int, widths=None) -> list[Step]:
+    """Every step of the queue, as a pure function of the lengths (and widths)."""
+    s = Scheduler(lengths, K, capacity, widths)
     out = []
     while not s.done:
         out.append(s.step())

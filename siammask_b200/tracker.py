@@ -74,6 +74,15 @@ class TrackerParams:
 IMAGE_DESC = np.dtype([("offset", "<i8"), ("h", "<i4"), ("w", "<i4")])      # sm_image_desc of include/siammask_b200.h
 
 
+def upload(values, dtype, dev) -> torch.Tensor:
+    """A small host table (list or array) as a device tensor of `dtype`, copied asynchronously from pinned memory: the
+    copy queues without waiting for the device (a pageable copy would wait for the stream)."""
+    host = torch.as_tensor(np.asarray(values)).to(dtype)
+    if torch.device(dev).type == "cuda" and host.numel():
+        host = host.pin_memory()
+    return host.to(dev, non_blocking=True)
+
+
 def image_table(shapes, channels: int) -> np.ndarray:
     """sm_image_desc rows of images packed back to back: shapes (h, w) per image, None for an empty entry (h = w = 0,
     occupying nothing); channels elements per pixel."""
@@ -129,10 +138,7 @@ class FramePacker:
         t = image_table(shapes, channels)
         if shared:
             t["offset"] = 0
-        host = torch.from_numpy(t.view(np.uint8).reshape(-1).copy())
-        if torch.device(self.dev).type == "cuda":
-            host = host.pin_memory()                # the copy below then queues without waiting for the device
-        dev = host.to(self.dev, non_blocking=True)
+        dev = upload(t.view(np.uint8).reshape(-1), torch.uint8, self.dev)
         self._tables[channels] = (key, dev, t)
         return dev, t
 
@@ -277,15 +283,15 @@ class BatchTracker:
         """Device copies of the active set (slot table, frame-index table) and per-frame work buffers; runs only when the
         set changes."""
         N, dev = self.N, self.dev
-        self._slots_dev = torch.tensor(self._slots, dtype=torch.int32, device=dev)
-        self._fidx_dev = torch.tensor(self._fidx, dtype=torch.int32, device=dev)
+        self._slots_dev = upload(np.asarray(self._slots, np.int64).reshape(N), torch.int32, dev)
+        self._fidx_dev = upload(np.asarray(self._fidx, np.int64).reshape(N), torch.int32, dev)
         self._max_fidx = max(self._fidx) if self._fidx else -1
-        self._hp_dev = torch.tensor(self._hp, dtype=torch.float64, device=dev).reshape(N, 3)
+        self._hp_dev = upload(np.asarray(self._hp, np.float64).reshape(N, 3), torch.float64, dev)
         self.boxes = torch.zeros(N, 8, dtype=torch.int32, device=dev)
         self.tsz = torch.zeros(N, 2, dtype=torch.float64, device=dev)
         self.aux = torch.zeros(N, 4, dtype=torch.float64, device=dev)
         self.maps = torch.zeros(N, 6, dtype=torch.float64, device=dev)
-        self.imsize = torch.tensor([[w, h] for h, w in self._size], dtype=torch.int32, device=dev).reshape(N, 2)
+        self.imsize = upload(np.asarray([[w, h] for h, w in self._size], np.int64).reshape(N, 2), torch.int32, dev)
         self._mask_table = None                         # paste-back table, buffer length, grid; built on first use
 
     def _template(self, fr: Packed, src: list[int], state: torch.Tensor, slots: list[int]) -> torch.Tensor:
@@ -442,10 +448,7 @@ class BatchTracker:
             return
         self._fidx = fidx
         self._max_fidx = max(fidx)
-        host = torch.tensor(fidx, dtype=torch.int32)
-        if torch.device(self.dev).type == "cuda":
-            host = host.pin_memory()                # the copy queues without waiting for the device
-        self._fidx_dev = host.to(self.dev, non_blocking=True)
+        self._fidx_dev = upload(fidx, torch.int32, self.dev)
 
     @torch.no_grad()
     def remove(self, ids) -> None:
@@ -458,7 +461,7 @@ class BatchTracker:
             return
         keep = [r for r, i in enumerate(self._ids) if i not in drop]
         with torch.cuda.device(self.dev):
-            rows = torch.tensor(keep, dtype=torch.long, device=self.dev)
+            rows = upload(np.asarray(keep, np.int64), torch.long, self.dev)
             self.state = self.state.index_select(0, rows).contiguous()
             self.avg = self.avg.index_select(0, rows).contiguous()
             self._ids = [self._ids[r] for r in keep]

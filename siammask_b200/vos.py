@@ -24,6 +24,11 @@ The reference has two branches, both restated as they are:
                  k+1 (by position, whatever id it was tracked with) on frames 1 .. num_frames-2;
   score="spans": start_frame / end_frame dicts.  Each object is scored against its own id on frames
                  start+1 .. end-2 (an empty window gives NaN).
+
+A whole dataset (videos of any length, frame size and object count) goes through `open_queue` / `needed` / `step`: the
+videos are queued by `schedule.Scheduler`, each holding as many slots as it has objects active at once (`peak_width`)
+from its admission until its last frame, and each admitted video advances one frame of its own per step, exactly as
+`frame` advances it.
 """
 from __future__ import annotations
 
@@ -32,7 +37,8 @@ import torch
 
 from . import ops
 from .ops import OBJ_IDLE, OBJ_INIT, OBJ_TRACKED
-from .tracker import BatchTracker, TrackerParams
+from .schedule import Scheduler
+from .tracker import BatchTracker, TrackerParams, upload
 from .tune import _check_thresholds
 
 UNBOUNDED = np.iinfo(np.int64).max
@@ -69,6 +75,13 @@ def score_windows(objects, num_frames: int, score: str):
     raise ValueError(f"score must be one of {SCORE_MODES}, got {score!r}")
 
 
+def peak_width(start, end) -> int:
+    """The most objects active at one frame: object k is active at frame f when start[k] <= f <= end[k] (it joins at
+    its start frame after the objects that stopped the frame before have left).  The slots a video holds in a queue."""
+    s, e = np.asarray(start, np.int64).reshape(-1), np.asarray(end, np.int64).reshape(-1)
+    return max((int(((s <= f) & (f <= e)).sum()) for f in s), default=0)
+
+
 def score_row(counts, lo: int, hi: int) -> np.ndarray:
     """One object's row of MultiBatchIouMeter from its integer counts int [frames, thrs, 2] (intersection, union):
     per threshold, np.mean of [intxn / union (float64), or 1 where union == 0] over frames lo .. hi-1, as float32; NaN for
@@ -94,6 +107,7 @@ class VideoSegmenter:
         self.dev = self.tracker.dev
         self.objects: list[tuple[int, int, int, int]] = []
         self.score = None
+        self._sched = None
 
     def open(self, objects, num_frames: int | None = None, num_videos: int | None = None, score: str | None = None,
              thrs=VOS_THRESHOLDS):
@@ -149,20 +163,22 @@ class VideoSegmenter:
             self._tid_key, self._tid = None, None
             # counts of frame f, entry i (kernel order, self.order[i]) and threshold t: (intersection, union)
             self._counts = torch.zeros(int(num_frames), len(objs), self.thrs.size, 2, dtype=torch.int32, device=self.dev)
+        self._sched = None
         self.tracker._clear()
         self.f = 0
         return self
 
-    def _target_ids(self, scored) -> torch.Tensor:
-        key = tuple(int(self._target[k]) if scored[k] else -1 for k in self.order)
+    def _target_ids(self, scored, order=None) -> torch.Tensor:
+        key = tuple(int(self._target[k]) if scored[k] else -1 for k in (self.order if order is None else order))
         if key != self._tid_key:              # changes only when an object's window opens or closes
             self._tid_key = key
-            self._tid = torch.tensor(key, dtype=torch.int32, device=self.dev)
+            self._tid = upload(np.asarray(key, np.int64), torch.int32, self.dev)
         return self._tid
 
-    def _entries(self, kinds, rows) -> torch.Tensor:
+    def _entries(self, kinds, rows, order=None) -> torch.Tensor:
+        """The kernel's object table: one (kind, arg) entry per object of `order` (default: every object, by video)."""
         ent = []
-        for k in self.order:
+        for k in (self.order if order is None else order):
             if kinds[k] == OBJ_TRACKED:
                 ent.append((OBJ_TRACKED, rows[self._sid[k]]))
             elif kinds[k] == OBJ_INIT:
@@ -172,7 +188,8 @@ class VideoSegmenter:
         key = tuple(ent)
         if key != self._table_key:            # the table changes only when an object starts, stops or a row moves
             self._table_key = key
-            self._table = torch.tensor(ent if ent else [(OBJ_IDLE, 0)], dtype=torch.int32, device=self.dev).reshape(-1, 2)
+            self._table = upload(np.asarray(ent if ent else [(OBJ_IDLE, 0)], np.int64).reshape(-1, 2), torch.int32,
+                                 self.dev)
         return self._table
 
     @torch.no_grad()
@@ -182,6 +199,8 @@ class VideoSegmenter:
         scored window.  Returns labels uint8 [G,H,W] on the device.  frames may instead be a list of G frames
         [H_g,W_g,3] of different sizes, with annos a list of G maps [H_g,W_g]; labels are then a list of G uint8
         [H_g,W_g] views of one packed buffer."""
+        if self._sched is not None:
+            raise ValueError("a queue run advances with step(); frame() belongs to open()")
         f, G = self.f, self.G
         # the schedule and scoring checks need no frames: they fail before any frame reaches the device
         kinds = schedule(self._start, self._end, f)
@@ -278,7 +297,9 @@ class VideoSegmenter:
         `open` order, from the counts of the frames processed so far.  One D2H copy; the IoU and the means are computed
         from the integer counts with the reference's float64 arithmetic (`score_row`); NaN for an empty window."""
         if self.score is None:
-            raise ValueError("open(..., score='whole' | 'spans') first")
+            raise ValueError("open(..., score='whole' | 'spans') or open_queue(..., score=...) first")
+        if self._sched is not None:
+            return self._queue_result()
         counts = self._counts.cpu().numpy()
         entry = {k: i for i, k in enumerate(self.order)}
         rows = [score_row(counts[:, entry[k]], int(self._lo[k]), min(int(self._hi[k]), self.f))
@@ -287,4 +308,223 @@ class VideoSegmenter:
         for g in range(self.G):
             r = [rows[k] for k in range(len(self.objects)) if self.objects[k][0] == g]
             out.append(np.stack(r) if r else np.zeros((0, self.thrs.size), np.float32))
+        return out
+
+    # ------------------------------------------------------------------ queue mode
+    def open_queue(self, objects, num_frames, score: str | None = None, thrs=VOS_THRESHOLDS):
+        """Queues G videos of any length, frame size and object count through the engine (`schedule.Scheduler`, K = 1):
+        video g holds `peak_width` of its objects' (start, end) slots from its admission until its last frame, and a
+        video waits until that many of min(max_batch, free slots) are free.  num_frames: [G] the videos' lengths;
+        objects: (video, object_id, start_frame[, end_frame]) as in `open`, end_frame defaulting to T_g - 1, with
+        0 <= start <= end <= T_g - 1; every video needs one object.  score: as in `open`, each video scored on its own
+        length ("whole": frames 1 .. T_g - 2).  Drive it with
+
+            while seg.pending:
+                need = seg.needed()
+                want = seg.needs_anno()
+                labels = seg.step([frames[g][t] for g, t in need],
+                                  [annos[g][t] if w else None for (g, t), w in zip(need, want)])
+
+        and read `result()` (G float32 arrays [objects of g, thresholds], objects in open order)."""
+        T = np.asarray(num_frames).reshape(-1)
+        if T.size == 0 or not np.issubdtype(T.dtype, np.integer) or (T < 1).any():
+            raise ValueError("num_frames must be one integer >= 1 per video")
+        if score not in SCORE_MODES:
+            raise ValueError(f"score must be one of {SCORE_MODES}, got {score!r}")
+        G = int(T.size)
+        objs = []
+        for o in objects:
+            o = tuple(int(v) for v in o)
+            if len(o) not in (3, 4) or not 0 <= o[0] < G or not 0 <= o[1] <= 255:
+                raise ValueError(f"bad object entry {o}: (video in 0..{G - 1}, id in 0..255, start[, end])")
+            if len(o) == 3:
+                o = o + (int(T[o[0]]) - 1,)
+            if not 0 <= o[2] <= o[3] <= T[o[0]] - 1:
+                raise ValueError(f"object {o}: needs 0 <= start_frame <= end_frame <= {int(T[o[0]]) - 1} "
+                                 f"(video {o[0]}'s last frame)")
+            objs.append(o)
+        members = [[k for k, o in enumerate(objs) if o[0] == g] for g in range(G)]
+        for g, ks in enumerate(members):
+            if not ks:
+                raise ValueError(f"video {g} has no object")
+            if len(ks) > 255:
+                raise ValueError(f"video {g}: at most 255 objects per video (labels are uint8)")
+        start = np.array([o[2] for o in objs], np.int64)
+        end = np.array([o[3] for o in objs], np.int64)
+        width = np.array([peak_width(start[ks], end[ks]) for ks in members], np.int64)
+        net = self.tracker.net
+        cap = min(net.max_batch, net.num_slots - self.tracker.slot0)
+        if cap < 1:
+            raise ValueError("the engine has no free slot")
+        sched = Scheduler(T, 1, cap, width)          # ValueError for a video wider than the engine
+        if score is not None:
+            self.thrs = _check_thresholds(thrs)
+            target, lo, hi = (np.zeros(len(objs), np.int64) for _ in range(3))
+            for g, ks in enumerate(members):
+                target[ks], lo[ks], hi[ks] = score_windows([objs[k] for k in ks], int(T[g]), score)
+                if np.unique(target[ks]).size != len(ks):
+                    raise ValueError(f"video {g}: scored object ids must be unique within a video")
+            self._target, self._lo, self._hi = target, lo, hi
+            n_rows = np.maximum(hi - lo, 0)
+            self._row0 = np.concatenate([[0], np.cumsum(n_rows)[:-1]]).astype(np.int64)
+            self._thrs_dev = torch.as_tensor(self.thrs, device=self.dev)
+            # (intersection, union) of object k at frame lo[k] + j, threshold t: row _row0[k] + j
+            self._rows = torch.zeros(int(n_rows.sum()), self.thrs.size, 2, dtype=torch.int32, device=self.dev)
+        self.objects, self.score, self.G = objs, score, G
+        self._start, self._end, self._members, self._qT = start, end, members, T.astype(np.int64)
+        self._sid = [None] * len(objs)
+        self._hw: list = [None] * G                  # frame size of each video, from its frame 0
+        self._admitted = np.full(G, -1, np.int64)   # the step that read each video's frame 0
+        self._done = np.zeros(G, np.int64)          # frames of each video processed
+        self._table_key = self._tid_key = self._off_key = self._copy_key = None
+        self._sched, self._plan = sched, sched.step()
+        self.tracker._clear()
+        self.f = 0
+        return self
+
+    @property
+    def pending(self) -> bool:
+        """Whether a queue run has steps left."""
+        return self._sched is not None and self._plan is not None
+
+    def needed(self) -> list:
+        """The (video g, frame t) pairs the next `step` reads, one per admitted video, in the order of its lists."""
+        if not self.pending:
+            raise ValueError("no queue step is pending: call open_queue() first; the run has finished")
+        return list(self._plan.need)
+
+    def _wants_anno(self, g: int, t: int) -> bool:
+        ks = self._members[g]
+        if (self._start[ks] == t).any():
+            return True
+        return self.score is not None and bool(((self._lo[ks] <= t) & (t < self._hi[ks])).any())
+
+    def needs_anno(self) -> list:
+        """Per `needed()` entry (g, t): whether `step` needs frame t's annotation of video g (an object of g starts at
+        t, or t lies in some object's scored window)."""
+        return [self._wants_anno(g, t) for g, t in self.needed()]
+
+    @staticmethod
+    def _size_of(im, what: str):
+        shape = tuple(int(v) for v in im.shape)
+        if len(shape) != (3 if what == "frame" else 2) or (what == "frame" and shape[2] != 3):
+            raise ValueError(f"each {what} must be {'[H,W,3]' if what == 'frame' else '[H,W]'}, got {shape}")
+        return shape[:2]
+
+    @torch.no_grad()
+    def step(self, frames, annos):
+        """One step of a queue run: frames[i] is frame t of video g for (g, t) = needed()[i] (uint8 [H_g,W_g,3], BGR),
+        annos[i] its uint8 [H_g,W_g] annotation label map where needs_anno()[i] (ignored elsewhere; None will do).  Does
+        for every admitted video what `frame` does at its frame t: objects start, are tracked and leave, and the fused
+        label map (with the scored objects' counts) comes from one ragged kernel pass over the step's videos.  Returns
+        the label maps, a list of uint8 [H_g,W_g] device views in needed() order."""
+        if not self.pending:
+            raise ValueError("no queue step is pending: call open_queue() first; the run has finished")
+        st, f, bt = self._plan, self.f, self.tracker
+        n = len(st.need)
+        if not isinstance(frames, (list, tuple)) or len(frames) != n:
+            raise ValueError(f"frames must be a list of {n} frames, one per needed() entry")
+        if not isinstance(annos, (list, tuple)) or len(annos) != n:
+            raise ValueError(f"annos must be a list of {n} entries, one per needed() entry")
+        # every check reads shapes on the host, before any device work
+        want = [self._wants_anno(g, t) for g, t in st.need]
+        for i, (g, t) in enumerate(st.need):
+            if frames[i] is None:
+                raise ValueError(f"frame {t} of video {g} is missing")
+            hw = self._size_of(frames[i], "frame")
+            if t > 0 and hw != self._hw[g]:
+                raise ValueError(f"frame {t} of video {g} is {hw[0]}x{hw[1]}, its frame 0 "
+                                 f"{self._hw[g][0]}x{self._hw[g][1]}")
+            if want[i]:
+                a = annos[i]
+                if a is None:
+                    raise ValueError(f"frame {t} of video {g}: an object starts or is scored, its annotation is "
+                                     "required")
+                if a.dtype not in (np.uint8, torch.uint8) or self._size_of(a, "annotation") != hw:
+                    raise ValueError(f"the annotation of frame {t} of video {g} must be uint8 [{hw[0]},{hw[1]}]")
+        fr = bt._input(frames)
+        for i, (g, t) in enumerate(st.need):
+            if t == 0:
+                self._hw[g], self._admitted[g] = fr.shapes[i], f
+        order = [k for g, _ in st.need for k in self._members[g]]
+        kinds = np.full(len(self.objects), OBJ_IDLE, np.int32)
+        scored = np.zeros(len(self.objects), bool)
+        for g, t in st.need:
+            ks = self._members[g]
+            kinds[ks] = schedule(self._start[ks], self._end[ks], t)
+            if self.score is not None:
+                scored[ks] = (self._lo[ks] <= t) & (t < self._hi[ks])
+        entry = {g: i for i, (g, _) in enumerate(st.need)}
+        starting = [k for k in order if kinds[k] == OBJ_INIT]
+        anno = None
+        if starting or scored.any():
+            # every video of the step gets a map in the frames' layout (the kernels read both through one table)
+            fill = [annos[i] if want[i] else
+                    (torch.zeros(hw, dtype=torch.uint8, device=frames[i].device) if torch.is_tensor(frames[i])
+                     else np.zeros(hw, np.uint8)) for i, hw in enumerate(fr.shapes)]
+            anno = bt.packer.pack(fill, 1).data
+        desc, ptable = bt.packer.table(fr.shapes, 1)
+        plane = (desc, int(ptable["offset"][-1]) + fr.shapes[-1][0] * fr.shapes[-1][1])
+        H, W = max(s[0] for s in fr.shapes), max(s[1] for s in fr.shapes)
+        if starting:
+            # init boxes: one D2H copy, at steps where objects start
+            queries = [(entry[self.objects[k][0]], self.objects[k][1]) for k in starting]
+            boxes = ops._label_boxes_ragged(anno, desc, n, queries).cpu().numpy()
+            missing = [self.objects[k][:2] for k, b in zip(starting, boxes) if b[2] == 0]
+            if missing:
+                raise ValueError(f"step {f}: (video, id) {missing} not in the annotation")
+        # objects that stopped and the objects of videos that ended in the last step (not in `order`: IDLE) leave
+        leaving = [k for k, s in enumerate(self._sid) if s is not None and kinds[k] != OBJ_TRACKED]
+        if leaving:
+            bt.remove([self._sid[k] for k in leaving])
+            for k in leaving:
+                self._sid[k] = None
+        masks = maps = None
+        rows = {}
+        if bt.N:
+            video = {self._sid[k]: self.objects[k][0] for k in order if self._sid[k] is not None}
+            idx = [entry[video[i]] for i in bt.ids]
+            if idx != bt._fidx:                          # the frame list moved: only after admissions or departures
+                bt.set_frame_index(bt.ids, idx)
+            r = bt.track(fr, mask=True, refine=self.p.out_size == 127, paste=False)
+            masks, maps = r.extras["mask_prob"], r.extras["maps"]
+            rows = {sid: i for i, sid in enumerate(r.extras["ids"])}
+            self.last = r
+        table = self._entries(kinds, rows, order)
+        if starting:
+            ids = bt.add(fr, boxes.astype(np.float64), frame_index=[entry[self.objects[k][0]] for k in starting])
+            for k, sid in zip(starting, ids):
+                self._sid[k] = sid
+        per = tuple(len(self._members[g]) for g, _ in st.need)
+        if per != self._off_key:                         # changes only when a video is admitted or retires
+            self._off_key = per
+            self._qoffsets = upload(np.concatenate([[0], np.cumsum(per)]), torch.int32, self.dev)
+        if not scored.any():
+            labels = ops._paste_labels(masks, maps, anno, self._qoffsets, table, (H, W), self.p.seg_thr, ragged=plane)
+        else:
+            labels, cnt = ops._paste_labels_iou(masks, maps, anno, self._qoffsets, table, self._target_ids(scored, order),
+                                                (H, W), self.p.seg_thr, self._thrs_dev, ragged=plane)
+            # object k's counts at its frame t = f - admitted go to row _row0[k] + t - lo[k]: a constant plus f
+            src = [i for i, k in enumerate(order) if scored[k]]
+            key = (tuple(src), tuple(int(self._row0[order[i]] - self._lo[order[i]]
+                                         - self._admitted[self.objects[order[i]][0]]) for i in src))
+            if key != self._copy_key:                    # changes only when a window opens or closes, or entries move
+                self._copy_key = key
+                self._copy_src = upload(np.asarray(key[0], np.int64), torch.long, self.dev)
+                self._copy_dst = upload(np.asarray(key[1], np.int64), torch.long, self.dev)
+            self._rows.index_copy_(0, self._copy_dst + f, cnt.index_select(0, self._copy_src))
+        for g, t in st.need:
+            self._done[g] = t + 1
+        self.f += 1
+        self._plan = self._sched.step() if not self._sched.done else None
+        return [labels[int(o):int(o) + h * w].view(h, w) for o, (h, w) in zip(ptable["offset"], fr.shapes)]
+
+    def _queue_result(self) -> list[np.ndarray]:
+        counts = self._rows.cpu().numpy()
+        out = []
+        for g, ks in enumerate(self._members):
+            # frames lo .. min(hi, frames processed) - 1 of each object, as `result` of a per-video run
+            out.append(np.stack([score_row(counts[self._row0[k]:self._row0[k] + max(self._hi[k] - self._lo[k], 0)], 0,
+                                           min(int(self._hi[k]), int(self._done[g])) - int(self._lo[k]))
+                                 for k in ks]))
         return out
