@@ -38,9 +38,10 @@ xcorr_depthwise = conv2d_dw_group
 
 
 def conv2d(x, weight, scale=None, shift=None, stride=1, padding=0, dilation=1, relu=False, backend="tensor",
-           precision="exact"):
+           precision="exact", out=None):
     """F.conv2d(x, weight) * scale[c] + shift[c] (+ReLU) through the engine's convolution kernels.
-    x f32[B,Cin,H,W] NCHW, weight f32[Cout,Cin,KH,KW]; returns f32 NCHW."""
+    x f32[B,Cin,H,W] NCHW, weight f32[Cout,Cin,KH,KW]; returns f32 NCHW, written into `out` when given (a contiguous
+    f32 tensor of the output's shape on x's device)."""
     if not x.is_cuda:
         raise RuntimeError("siammask_b200 operators run on CUDA tensors only; there is no CPU path")
     lib = _lib.load()
@@ -51,7 +52,11 @@ def conv2d(x, weight, scale=None, shift=None, stride=1, padding=0, dilation=1, r
     Cout, _, KH, KW = weight.shape
     Ho = (H + 2 * padding - dilation * (KH - 1) - 1) // stride + 1
     Wo = (W + 2 * padding - dilation * (KW - 1) - 1) // stride + 1
-    out = torch.empty(B, Cout, Ho, Wo, device=dev, dtype=torch.float32)
+    if out is None:
+        out = torch.empty(B, Cout, Ho, Wo, device=dev, dtype=torch.float32)
+    elif (tuple(out.shape) != (B, Cout, Ho, Wo) or out.dtype != torch.float32 or out.device != dev
+          or not out.is_contiguous()):
+        raise RuntimeError(f"out must be a contiguous float32 tensor of shape {(B, Cout, Ho, Wo)} on {dev}")
     sc = scale.to(dev, torch.float32).contiguous() if scale is not None else None
     sh = shift.to(dev, torch.float32).contiguous() if shift is not None else None
     be = {"tensor": _lib.SM_BACKEND_TENSOR, "simt": _lib.SM_BACKEND_SIMT}[backend]

@@ -97,6 +97,22 @@ class Scheduler:
         return Step(need, entry, track, list(new), retire)
 
 
+MAX_LANES = 2         # engine.cu kMaxLanes
+LANE_MIN_B = 8        # engine.cu kLaneMinB: a lane gets at least this many streams
+
+
+def lane_split(B: int, max_batch: int) -> list[int]:
+    """The streams each execution lane of an engine built for `max_batch` runs in a call of batch B, lane 0 first
+    (engine.cu lanes_for / chunk): B splits over two lanes once both get at least LANE_MIN_B streams, lane 0 taking the
+    odd one.  Every search-side and refine launch of the call runs once per lane with M = (lane streams) x Ho x Wo;
+    template calls are not split."""
+    if not 1 <= int(B) <= int(max_batch):
+        raise ValueError("need 1 <= B <= max_batch")
+    n = max(1, min(MAX_LANES, int(max_batch) // LANE_MIN_B))
+    n = max(1, min(n, int(B) // LANE_MIN_B))
+    return [int(B) // n + (1 if lane < int(B) % n else 0) for lane in range(n)]
+
+
 def plan(lengths, K: int, capacity: int, widths=None) -> list[Step]:
     """Every step of the queue, as a pure function of the lengths (and widths)."""
     s = Scheduler(lengths, K, capacity, widths)

@@ -312,6 +312,101 @@ def tau_for(peak, fmt, calibrated):
     return 2.0 ** -24 * (peak / 256.0 if calibrated else 1.0)
 
 
+# ---------------------------------------------------------------------------------------------------- launch shapes
+def _patch_ro(w):
+    """conv3x3_patch_sm90.cu patch_pw / patch_ro: image rows per 128-pixel tile (0: the geometry is not supported)."""
+    pw = (w + 1 + 7) // 8 * 8
+    return 128 // pw if pw <= 64 and 128 % pw == 0 else 0
+
+
+def _cout_pad(cout):
+    """conv_gemm_sm90.cu gemm_cout_pad."""
+    for p in (16, 32, 64, 128):
+        if cout <= p:
+            return p
+    return (cout + 255) // 256 * 256
+
+
+def launches(search_size, B, max_batch=None, with_mask=True, refine=True):
+    """Every tensor-core conv, stem and engine-xcorr launch of one template + track_mask + track_refine at batch B on
+    the tensor backend, as dicts (side, name, kernel, lane, M, tiles).  Template launches run once over all B streams;
+    search-side and refine launches run once per lane on that lane's streams (schedule.lane_split).  M is the launch's
+    output rows (streams x Ho x Wo); tiles counts the persistent kernels' work items (GEMM / stem: 128-row M tiles x
+    N tiles; patch conv: RO-row blocks per image; xcorr: its blocks of 32 channels x row band per stream)."""
+    from siammask_b200.checkpoint import expected_keys
+    from siammask_b200.schedule import lane_split
+
+    shapes = expected_keys(with_mask, refine)
+    sides = [("template", template_taps("tensor", with_mask), [B])]
+    lanes = lane_split(B, max_batch or B)
+    sides.append(("search", search_taps(backend="tensor", with_mask=with_mask, mask_head=with_mask), lanes))
+    if refine:
+        sides.append(("refine", refine_taps(), lanes))
+    out, size = [], {}
+    for side, taps, chunks in sides:
+        if side != "refine":                                   # refine reads the search side's tensors
+            size = {"x": search_size, "z": 127}
+        for t in taps:
+            h = size[t.inputs[0]]
+            kernel = None
+            if t.op in ("conv", "small"):
+                co = sum(shapes[k + ".weight"][0] for k, _ in t.keys)
+                _, ci, kh, kw = shapes[t.keys[0][0] + ".weight"]
+                if t.op == "small":
+                    h = t.geom["up"] or h
+                ho = (h + 2 * t.pad - t.dil * (kh - 1) - 1) // t.stride + 1
+                if family(t) == "gemm":
+                    if t.name == "stem":
+                        kernel, ntile = "stem", 1
+                    elif (kh == kw == 3 and t.stride == 1 and t.pad == 1 and t.dil == 1 and ci == co in (64, 128)
+                          and t.second is None and not t.residual and t.name not in F32_OUT and _patch_ro(h)):
+                        kernel = "patch"
+                    else:
+                        kernel, ntile = "gemm", _cout_pad(co) // min(_cout_pad(co), 128)
+            elif t.op == "maxpool":
+                ho = (h + 2 - 3) // 2 + 1
+            elif t.op == "crop_center":
+                ho = h - 8
+            elif t.op == "xcorr":
+                ho, kernel = h - 4, "xcorr"
+                bands = 1
+                while (-(-ho // bands) + 4) * h * 32 * 4 > 160 * 1024:        # launch_xcorr_nhwc's row bands
+                    bands += 1
+            elif t.op == "refine_crop":
+                ho = t.geom["size"]
+            elif t.op == "gather":
+                ho = 1
+            else:                                                           # deconv
+                ho = 15
+            size[t.name] = ho
+            if kernel is None:
+                continue
+            for lane, b in enumerate(chunks):
+                M = b * ho * ho
+                if kernel == "patch":
+                    tiles = b * -(-ho // _patch_ro(ho))
+                elif kernel == "xcorr":
+                    tiles = 8 * b * bands
+                else:
+                    tiles = -(-M // 128) * ntile
+                out.append(dict(side=side, name=t.name, kernel=kernel, lane=lane, M=M, tiles=tiles))
+    return out
+
+
+def tile_classes(launch, num_sms=132):
+    """The ragged-tile classes a launch exercises: 'a' when its last 128-row tile ends in the first warpgroup's 64 rows
+    (the second consumer warpgroup has no row to store), 'b' when it ends in the second's, 'c' when there are more
+    tiles than SMs (persistent CTAs take a second tile)."""
+    r, cls = launch["M"] % 128, set()
+    if 0 < r <= 64:
+        cls.add("a")
+    elif r > 64:
+        cls.add("b")
+    if launch["tiles"] > num_sms:
+        cls.add("c")
+    return cls
+
+
 # ---------------------------------------------------------------------------------------------------- mutations
 def round_sig(t, bits=11):
     """Round the significand to `bits` significant bits, round-to-nearest-even, no exponent range (nothing is flushed):
