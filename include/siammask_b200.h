@@ -280,12 +280,12 @@ int sm_vot_eao_accumulate(const float* eao, const float* acc, const double* rec,
 /* Score / box post-processing + argmax of siamese_track — tools/test.py:205-254 — on the device, so that
  * sm_track -> sm_select -> sm_refine needs no host round trip.  All pointers are device pointers:
  * cls/loc as returned by sm_track; anchors f32 [A*R*R][4] = (cx,cy,w,h) in generate_anchor order (tools/test.py:113-129);
- * window f32 [A*R*R] (tiled hanning, :157-161); target_sz_in_crop f64 [B][2] = target_sz * scale_x (:226; float64 as
+ * window f64 [A*R*R] (tiled hanning, :157-161, float64 as the reference builds it); target_sz_in_crop f64 [B][2] = target_sz * scale_x (:226; float64 as
  * in the reference, whose penalty terms are evaluated in float64).
  * Outputs: best_idx int32 [B] (np.argmax of pscore, :237 — incl. its NaN rule: the first NaN wins), pos int32 [B][2] =
  * (delta_y, delta_x) (:253-254), records f32 [B][8] = decoded box cx,cy,w,h of the winner in crop units (:209-212),
  * score, penalty, pscore, best index (exact: < 2^24). */
-int sm_select(sm_engine* e, int32_t B, const float* cls, const float* loc, const float* anchors, const float* window,
+int sm_select(sm_engine* e, int32_t B, const float* cls, const float* loc, const float* anchors, const double* window,
               const double* target_sz_in_crop, double penalty_k, double window_influence, int32_t* best_idx, int32_t* pos,
               float* records, void* stream);
 
@@ -320,7 +320,7 @@ int sm_tracker_update_hp(int32_t B, double* state, const float* records, const d
  * SM_TRACK_MASK_HEAD and `mask`).  Unlike the three separate calls, the engine's two lanes run their halves of the
  * batch start to end without meeting in between.  refine_out / mask / mask_col may be NULL. */
 int sm_step(sm_engine* e, int32_t slot0, int32_t B, const float* x_nchw, const double* target_sz_in_crop,
-            const float* anchors, const float* window, double penalty_k, double window_influence, int32_t flags,
+            const float* anchors, const double* window, double penalty_k, double window_influence, int32_t flags,
             float* cls, float* loc, float* mask, int32_t* best_idx, int32_t* pos, float* records, float* refine_out,
             float* mask_col, void* stream);
 
@@ -328,7 +328,7 @@ int sm_step(sm_engine* e, int32_t slot0, int32_t B, const float* x_nchw, const d
  * owned, entries in [0, num_slots); out-of-range entries as in sm_template_slots).  Under graph replay the table's
  * contents are read at run time, so a caller may rewrite it between calls that reuse the same pointer. */
 int sm_step_slots(sm_engine* e, int32_t B, const int32_t* slots, const float* x_nchw, const double* target_sz_in_crop,
-                  const float* anchors, const float* window, double penalty_k, double window_influence, int32_t flags,
+                  const float* anchors, const double* window, double penalty_k, double window_influence, int32_t flags,
                   float* cls, float* loc, float* mask, int32_t* best_idx, int32_t* pos, float* records, float* refine_out,
                   float* mask_col, void* stream);
 
@@ -337,7 +337,7 @@ int sm_step_slots(sm_engine* e, int32_t B, const int32_t* slots, const float* x_
  * different tracker settings, e.g. a grid search over them.  Stream b's selection, including records[b][5] (its
  * penalty), uses row b.  Like the slot table, the hp table's contents are read at run time under graph replay. */
 int sm_step_slots_hp(sm_engine* e, int32_t B, const int32_t* slots, const double* hp, const float* x_nchw,
-                     const double* target_sz_in_crop, const float* anchors, const float* window, int32_t flags,
+                     const double* target_sz_in_crop, const float* anchors, const double* window, int32_t flags,
                      float* cls, float* loc, float* mask, int32_t* best_idx, int32_t* pos, float* records,
                      float* refine_out, float* mask_col, void* stream);
 
@@ -350,7 +350,8 @@ typedef struct sm_step_io {
   const float* x_host;        /* f32 [B,3,S,S] */
   const double* tsz_host;     /* f64 [B,2] target_sz * scale_x */
   const float* anchors_dev;   /* f32 [A*R*R,4] device */
-  const float* window_dev;    /* f32 [A*R*R] device */
+  const float* window_dev;    /* f32 [A*R*R] device; the selection uses these float32 values (sm_step takes the
+                                 reference's float64 window, whose distinct values float32 can merge into ties) */
   double penalty_k, window_influence;
   int32_t flags;              /* SM_TRACK_* */
   float* records_host;        /* f32 [B,8], required */

@@ -201,7 +201,7 @@ def siamese_init(im, target_pos, target_sz, model, hp=None, device="cuda"):
                  target_pos=np.asarray(target_pos, dtype=np.float64), target_sz=np.asarray(target_sz, dtype=np.float64))
     if hasattr(model, "select"):      # device copies for the on-device post-processing
         state["anchor_dev"] = torch.from_numpy(p.anchor).to(device)
-        state["window_dev"] = torch.from_numpy(window.astype(np.float32)).to(device)
+        state["window_dev"] = torch.from_numpy(window).to(device)
     return state
 
 

@@ -211,10 +211,12 @@ void launch_tracker_update(int B, double* state, const float* rec, const double*
 void launch_crop_resize(const uint8_t* frames, size_t frame_stride, int H, int W, const int32_t* box, int B, int model,
                         float* out, cudaStream_t st, const int32_t* frame_idx = nullptr,
                         const sm_image_desc* desc = nullptr);
-// hp (optional): device f64 [B][3] per-stream table; stream b then uses hp[b][0] / hp[b][1] instead of the scalars
-void launch_select(const float* cls, const float* loc, const float* anchors, const float* window, const double* tsz,
-                   int B, int A, int R, double penalty_k, double window_influence, int32_t* best_idx, int32_t* pos,
-                   float* rec, cudaStream_t st, const double* hp = nullptr);
+// hp (optional): device f64 [B][3] per-stream table; stream b then uses hp[b][0] / hp[b][1] instead of the scalars.
+// window f64 [A*R*R], or null and window_f32 (the float32 window of sm_step_io)
+void launch_select(const float* cls, const float* loc, const float* anchors, const double* window,
+                   const float* window_f32, const double* tsz, int B, int A, int R, double penalty_k,
+                   double window_influence, int32_t* best_idx, int32_t* pos, float* rec, cudaStream_t st,
+                   const double* hp = nullptr);
 // sm_mask_iou (include/siammask_b200.h): fused paste-back + IouMeter counts; counts must hold B*T*2 int32.  desc
 // (optional, sm_mask_iou_ragged): annotation g is desc[g] of a packed buffer, and H, W bound every image
 void launch_mask_iou(const float* masks, int side, const double* maps, const uint8_t* anno, const int32_t* video, int B,

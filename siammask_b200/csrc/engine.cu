@@ -125,7 +125,8 @@ class Engine {
     const float* x = nullptr;            // device or (host path) staged input
     const double* tsz = nullptr;         // [B][2] target_sz * scale_x
     const float* anchors = nullptr;      // device [A*R*R][4]
-    const float* window = nullptr;       // device [A*R*R]
+    const double* window = nullptr;      // device [A*R*R]
+    const float* window_f32 = nullptr;   // device [A*R*R], the float32 window of sm_step_io (when window is null)
     double penalty_k = 0, window_influence = 0;
     const double* hp = nullptr;          // device [B][3] per-stream (penalty_k, window_influence, lr) or null: scalars
     int flags = 0;
@@ -1572,7 +1573,7 @@ Engine::StepIO slice_io(const Engine::StepIO& io, int b0, size_t S, size_t A, si
 void Engine::step_lane(Lane& ln, int slot0, int B, const StepIO& io, cudaStream_t st, const int32_t* slots) {
   track_lane(ln, slot0, B, io.x, io.cls, io.loc, io.mask, io.flags, st, slots);
   launch(st, 1, "select", "select", 0, 4.0 * B * 6.0 * cfg_.anchor_num * R_ * R_, [&] {
-    launch_select(io.cls, io.loc, io.anchors, io.window, io.tsz, B, cfg_.anchor_num, R_, io.penalty_k,
+    launch_select(io.cls, io.loc, io.anchors, io.window, io.window_f32, io.tsz, B, cfg_.anchor_num, R_, io.penalty_k,
                   io.window_influence, io.best, io.pos, io.rec, st, io.hp);
   });
   if (io.refine != nullptr) refine_lane(ln, B, io.pos, io.refine, st);
@@ -1586,7 +1587,7 @@ void Engine::do_step(int slot0, int B, const StepIO& io, cudaStream_t st, const 
   SMK_CHECK(weights_ready_, "weights not loaded");
   SMK_CHECK(B >= 1 && B <= cfg_.max_batch && (slots != nullptr || (slot0 >= 0 && slot0 + B <= cfg_.num_slots)),
             "step batch/slot range");
-  SMK_CHECK(io.x && io.tsz && io.anchors && io.window && io.cls && io.loc && io.best && io.pos && io.rec, "null argument");
+  SMK_CHECK(io.x && io.tsz && io.anchors && (io.window || io.window_f32) && io.cls && io.loc && io.best && io.pos && io.rec, "null argument");
   const bool want_feats = (io.flags & SM_TRACK_MASK_FEATURES) != 0, want_head = (io.flags & SM_TRACK_MASK_HEAD) != 0;
   SMK_CHECK(!(want_feats || want_head || io.refine) || cfg_.with_mask, "engine was built without the mask branch");
   SMK_CHECK(io.refine == nullptr || want_feats, "refine output needs SM_TRACK_MASK_FEATURES");
@@ -1602,7 +1603,7 @@ void Engine::do_step(int slot0, int B, const StepIO& io, cudaStream_t st, const 
                                      (uint64_t)io.loc, (uint64_t)io.mask, (uint64_t)io.flags, (uint64_t)io.pos,
                                      (uint64_t)io.rec, (uint64_t)io.refine, (uint64_t)io.mask_col, (uint64_t)st,
                                      (uint64_t)io.anchors, (uint64_t)io.window, (uint64_t)slots, pk_bits, wi_bits,
-                                     (uint64_t)io.hp};
+                                     (uint64_t)io.hp, (uint64_t)io.window_f32};
   const size_t S = cfg_.search_size, A = cfg_.anchor_num, RR = (size_t)R_ * R_;
   run_with_graph(key, st, [&] {
     split_batch(B);
@@ -1631,7 +1632,7 @@ int Engine::step_host_async(int slot0, int B, const sm_step_io& h, cudaStream_t 
     SMK_CUDA(cudaMalloc(&mask_raw_, (size_t)cfg_.max_batch * 3969 * RR * sizeof(float)));
   const int t = next_set();
   StepIO io;
-  io.x = stage_x_[t]; io.tsz = stage_tsz_[t]; io.anchors = h.anchors_dev; io.window = h.window_dev;
+  io.x = stage_x_[t]; io.tsz = stage_tsz_[t]; io.anchors = h.anchors_dev; io.window_f32 = h.window_dev;
   io.penalty_k = h.penalty_k; io.window_influence = h.window_influence; io.flags = h.flags;
   io.cls = stage_cls_[t]; io.loc = stage_loc_[t]; io.mask = want_head ? mask_raw_ : nullptr;
   io.best = stage_best_[t]; io.pos = stage_pos_[t]; io.rec = stage_rec_[t];
@@ -1943,7 +1944,7 @@ int sm_track_host_wait(sm_engine* e, int32_t ticket) {
 }
 
 int sm_step(sm_engine* e, int32_t slot0, int32_t B, const float* x, const double* target_sz_in_crop, const float* anchors,
-            const float* window, double penalty_k, double window_influence, int32_t flags, float* cls, float* loc,
+            const double* window, double penalty_k, double window_influence, int32_t flags, float* cls, float* loc,
             float* mask, int32_t* best_idx, int32_t* pos, float* records, float* refine_out, float* mask_col,
             void* stream) {
   SM_API_BEGIN
@@ -1965,7 +1966,7 @@ int sm_template_slots(sm_engine* e, int32_t B, const int32_t* slots, const float
 }
 
 int sm_step_slots(sm_engine* e, int32_t B, const int32_t* slots, const float* x, const double* target_sz_in_crop,
-                  const float* anchors, const float* window, double penalty_k, double window_influence, int32_t flags,
+                  const float* anchors, const double* window, double penalty_k, double window_influence, int32_t flags,
                   float* cls, float* loc, float* mask, int32_t* best_idx, int32_t* pos, float* records, float* refine_out,
                   float* mask_col, void* stream) {
   SM_API_BEGIN
@@ -1980,7 +1981,7 @@ int sm_step_slots(sm_engine* e, int32_t B, const int32_t* slots, const float* x,
 }
 
 int sm_step_slots_hp(sm_engine* e, int32_t B, const int32_t* slots, const double* hp, const float* x,
-                     const double* target_sz_in_crop, const float* anchors, const float* window, int32_t flags, float* cls,
+                     const double* target_sz_in_crop, const float* anchors, const double* window, int32_t flags, float* cls,
                      float* loc, float* mask, int32_t* best_idx, int32_t* pos, float* records, float* refine_out,
                      float* mask_col, void* stream) {
   SM_API_BEGIN
@@ -2271,14 +2272,14 @@ int sm_tracker_update_hp(int32_t B, double* state, const float* records, const d
   SM_API_END
 }
 
-int sm_select(sm_engine* e, int32_t B, const float* cls, const float* loc, const float* anchors, const float* window,
+int sm_select(sm_engine* e, int32_t B, const float* cls, const float* loc, const float* anchors, const double* window,
               const double* target_sz_in_crop, double penalty_k, double window_influence, int32_t* best_idx, int32_t* pos,
               float* records, void* stream) {
   SM_API_BEGIN
   SMK_CHECK(e && cls && loc && anchors && window && target_sz_in_crop && best_idx && pos && records, "null argument");
   SMK_CHECK(B >= 1, "batch");
   const smk::Engine& eng = *e->impl;
-  smk::launch_select(cls, loc, anchors, window, target_sz_in_crop, B, eng.cfg().anchor_num, eng.score_size(), penalty_k,
+  smk::launch_select(cls, loc, anchors, window, nullptr, target_sz_in_crop, B, eng.cfg().anchor_num, eng.score_size(), penalty_k,
                      window_influence,
                      best_idx, pos, records, static_cast<cudaStream_t>(stream));
   SM_API_END

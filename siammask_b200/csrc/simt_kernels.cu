@@ -691,9 +691,13 @@ __global__ void __launch_bounds__(256) small_conv3x3_kernel(const float* __restr
 //   score = softmax(cls)[:,1]; box = anchor decode of loc (:209-212); scale / ratio penalty (:214-232);
 //   pscore = penalty*score*(1-wi) + window*wi (:235-236); argmax (:237, first maximum wins like np.argmax);
 //   (dy, dx) = unravel(best, (A, R, R))[1:] (:253-254).
-// cls f32 [B][2A][R][R], loc f32 [B][4A][R][R], anchors f32 [A*R*R][4] (cx,cy,w,h), window f32 [A*R*R],
-// tsz f64 [B][2] = target_sz * scale_x (float64 as in the reference).  The network part is fp32 as in the reference;
-// the penalty is evaluated in fp64 (numpy promotes those expressions to float64 through the float64 target size).
+// cls f32 [B][2A][R][R], loc f32 [B][4A][R][R], anchors f32 [A*R*R][4] (cx,cy,w,h), window f64 [A*R*R] (the
+// reference's np.outer(np.hanning(R), np.hanning(R)) is float64: rounded to float32, distinct window values collapse
+// and candidates that numpy ranks become ties), or window_f32 when window is null (the host-buffer step's float32
+// window), tsz f64 [B][2] = target_sz * scale_x (float64 as in the reference).  The network part is fp32 as in the
+// reference; the penalty is evaluated in fp64 (numpy promotes those expressions to float64 through the float64 target
+// size), every product rounded before it is added, as numpy evaluates it: a contracted FMA moves pscore by an ulp and
+// decides ties differently.
 // np.argmax semantics incl. NaN: the first NaN wins over every number (a NaN/Inf network output or a 0/0 target
 // size must not leave `besti` unset: rec/pos are always in range).  rec[7] = best index (exact in fp32).
 // float32 exp evaluated the way numpy's SIMD float32 np.exp does it: Cody-Waite reduction by round(x*log2(e))*ln2,
@@ -721,7 +725,8 @@ __device__ __forceinline__ float np_expf(float x) {
 constexpr int SEL_THREADS = 512;   // latency-bound (fp64 exp / divides per candidate): more threads, fewer serial candidates each
 __global__ void __launch_bounds__(SEL_THREADS) select_kernel(const float* __restrict__ cls, const float* __restrict__ loc,
                                                      const float* __restrict__ anchors,
-                                                     const float* __restrict__ window,
+                                                     const double* __restrict__ window,
+                                                     const float* __restrict__ window_f32,
                                                      const double* __restrict__ tsz, int A, int R, double penalty_k,
                                                      double window_influence, int32_t* __restrict__ best_idx,
                                                      int32_t* __restrict__ pos, float* __restrict__ rec,
@@ -761,8 +766,9 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(const float* __rest
     double rc = tratio / (double)(w / h);
     rc = fmax(rc, 1.0 / rc);
     const double pk = hp != nullptr ? hp[3 * b] : penalty_k, wi = hp != nullptr ? hp[3 * b + 1] : window_influence;
-    const double penalty = exp(-(rc * sc - 1.0) * pk);
-    const double ps = penalty * (double)score * (1.0 - wi) + (double)window[idx] * wi;
+    const double penalty = exp(-__dadd_rn(__dmul_rn(rc, sc), -1.0) * pk);
+    const double win = window != nullptr ? window[idx] : (double)window_f32[idx];
+    const double ps = __dadd_rn(__dmul_rn(__dmul_rn(penalty, (double)score), 1.0 - wi), __dmul_rn(win, wi));
     const int isn = ps != ps ? 1 : 0;
     if (better(isn, ps, idx, bestnan, best, besti)) { best = ps; besti = idx; bestnan = isn; }
   }
@@ -808,7 +814,7 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(const float* __rest
     o[2] = w;
     o[3] = h;
     o[4] = score;
-    o[5] = (float)exp(-(rc * sc - 1.0) * (hp != nullptr ? hp[3 * b] : penalty_k));
+    o[5] = (float)exp(-__dadd_rn(__dmul_rn(rc, sc), -1.0) * (hp != nullptr ? hp[3 * b] : penalty_k));
     o[6] = (float)sv[0];
     o[7] = (float)idx;
   }
@@ -822,7 +828,7 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(const float* __rest
 //  dst = (((b0*(S0>>4))>>16) + ((b1*(S1>>4))>>16) + 2) >> 2; x fractions are clamped at the borders, y ROWS are) —
 // and emit the float CHW tensor the network consumes (:61-64).  box = int32 [B][8]: xmin, ymin, sz, avg0, avg1, avg2.
 __device__ __forceinline__ void cv_coeff(int d, double scale, int src_n, bool clamp_frac, int& s0, int& a0, int& a1) {
-  float f = (float)(((double)d + 0.5) * scale - 0.5);
+  float f = (float)__dadd_rn(__dmul_rn((double)d + 0.5, scale), -0.5);   // rounded product, as OpenCV evaluates it
   int s = (int)floorf(f);
   f -= (float)s;
   if (clamp_frac) {
@@ -890,11 +896,12 @@ __global__ void crop_resize_kernel(const uint8_t* __restrict__ frames, size_t fr
 // the same values bit for bit.
 __device__ __forceinline__ void warp_invert_map(const double* __restrict__ m, double inv[6]) {
   double M0 = m[0], M1 = m[1], M2 = m[2], M3 = m[3], M4 = m[4], M5 = m[5];
-  double D = M0 * M4 - M1 * M3;
+  // products rounded before they are added, as OpenCV's invertAffineTransform evaluates them (no FMA contraction)
+  double D = __dadd_rn(__dmul_rn(M0, M4), -__dmul_rn(M1, M3));
   D = D != 0.0 ? 1.0 / D : 0.0;
   const double A11 = M4 * D, A22 = M0 * D;
   M0 = A11; M1 *= -D; M3 *= -D; M4 = A22;
-  const double b1 = -M0 * M2 - M1 * M5, b2 = -M3 * M2 - M4 * M5;
+  const double b1 = __dadd_rn(__dmul_rn(-M0, M2), -__dmul_rn(M1, M5)), b2 = __dadd_rn(__dmul_rn(-M3, M2), -__dmul_rn(M4, M5));
   inv[0] = M0; inv[1] = M1; inv[2] = b1; inv[3] = M3; inv[4] = M4; inv[5] = b2;
 }
 
@@ -909,7 +916,8 @@ struct WarpTap {
 
 __device__ __forceinline__ WarpTap warp_tap(const double inv[6], int x, int y) {
   const long long adelta = llrint(inv[0] * x * 1024.0), bdelta = llrint(inv[3] * x * 1024.0);
-  const long long X0 = llrint((inv[1] * y + inv[2]) * 1024.0) + 16, Y0 = llrint((inv[4] * y + inv[5]) * 1024.0) + 16;
+  const long long X0 = llrint(__dadd_rn(__dmul_rn(inv[1], y), inv[2]) * 1024.0) + 16;
+  const long long Y0 = llrint(__dadd_rn(__dmul_rn(inv[4], y), inv[5]) * 1024.0) + 16;
   const long long X = (X0 + adelta) >> 5, Y = (Y0 + bdelta) >> 5;
   long long sx = X >> 5, sy = Y >> 5;
   sx = sx < -32768 ? -32768 : (sx > 32767 ? 32767 : sx);     // saturate_cast<short>
@@ -1701,8 +1709,9 @@ __global__ void tracker_prepare_kernel(int B, const double* __restrict__ state, 
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   const double px = state[4 * b], py = state[4 * b + 1], sw = state[4 * b + 2], sh = state[4 * b + 3];
-  const double wc_x = sh + hp.context_amount * (sw + sh);      // :180-181 (names as in the reference)
-  const double hc_x = sw + hp.context_amount * (sw + sh);
+  // :180-181 (names as in the reference); the product is rounded before the add, as numpy evaluates it
+  const double wc_x = __dadd_rn(sh, __dmul_rn(hp.context_amount, sw + sh));
+  const double hc_x = __dadd_rn(sw, __dmul_rn(hp.context_amount, sw + sh));
   double s_x = sqrt(wc_x * hc_x);
   const double scale_x = (double)hp.exemplar_size / s_x;
   const double d_search = (double)(hp.instance_size - hp.exemplar_size) / 2.0;
@@ -1746,7 +1755,7 @@ __global__ void tracker_update_kernel(int B, double* __restrict__ state, const f
   sc = fmax(sc, 1.0 / sc);
   double rc = (tw / th) / (double)(w / h);
   rc = fmax(rc, 1.0 / rc);
-  const double penalty = exp(-(rc * sc - 1.0) * penalty_k);
+  const double penalty = exp(-__dadd_rn(__dmul_rn(rc, sc), -1.0) * penalty_k);
   const double lr = penalty * (double)score * hp_lr;            // :241
   const double p0 = (double)r[0] / scale_x, p1 = (double)r[1] / scale_x, p2 = (double)w / scale_x, p3 = (double)h / scale_x;
   double res_x = p0 + px, res_y = p1 + py;
@@ -1760,8 +1769,9 @@ __global__ void tracker_update_kernel(int B, double* __restrict__ state, const f
     const int pidx = idx % (R * R);
     const double delta_y = pidx / R, delta_x = pidx % R;
     double s = sxr / (double)hp.instance_size;
-    const double sb0 = cx0 + (delta_x - hp.base_size / 2.0) * hp.total_stride * s;
-    const double sb1 = cy0 + (delta_y - hp.base_size / 2.0) * hp.total_stride * s;
+    // (delta - base/2) * stride is an exact integer; its product with s is rounded before the add (no FMA)
+    const double sb0 = __dadd_rn(cx0, __dmul_rn((delta_x - hp.base_size / 2.0) * hp.total_stride, s));
+    const double sb1 = __dadd_rn(cy0, __dmul_rn((delta_y - hp.base_size / 2.0) * hp.total_stride, s));
     const double sb2 = s * hp.exemplar_size;
     s = (double)hp.out_size / sb2;
     const double bb0 = -sb0 * s, bb1 = -sb1 * s, bb2 = im_w * s, bb3 = im_h * s;
@@ -2015,11 +2025,12 @@ void launch_warp_affine(const float* src, int sh, int sw, const double* maps, fl
   SMK_CUDA(cudaGetLastError());
 }
 
-void launch_select(const float* cls, const float* loc, const float* anchors, const float* window, const double* tsz,
-                   int B, int A, int R, double penalty_k, double window_influence, int32_t* best_idx, int32_t* pos,
-                   float* rec, cudaStream_t st, const double* hp) {
-  select_kernel<<<B, SEL_THREADS, 0, st>>>(cls, loc, anchors, window, tsz, A, R, penalty_k, window_influence, best_idx, pos,
-                                           rec, hp);
+void launch_select(const float* cls, const float* loc, const float* anchors, const double* window,
+                   const float* window_f32, const double* tsz, int B, int A, int R, double penalty_k,
+                   double window_influence, int32_t* best_idx, int32_t* pos, float* rec, cudaStream_t st,
+                   const double* hp) {
+  select_kernel<<<B, SEL_THREADS, 0, st>>>(cls, loc, anchors, window, window_f32, tsz, A, R, penalty_k, window_influence,
+                                           best_idx, pos, rec, hp);
   SMK_CUDA(cudaGetLastError());
 }
 

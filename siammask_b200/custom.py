@@ -368,12 +368,13 @@ class Custom:
     @torch.no_grad()
     def select(self, cls, loc, anchors, window, target_sz_in_crop, penalty_k: float, window_influence: float):
         """On-device restatement of tools/test.py:205-254.  cls/loc: outputs of track/track_mask; anchors f32
-        [A*R*R,4] (cx,cy,w,h) and window f32 [A*R*R] as built by siamese_init; target_sz_in_crop f32 [B,2].
+        [A*R*R,4] (cx,cy,w,h) and window [A*R*R] as built by siamese_init (used in float64, as the reference's
+        np.hanning window is); target_sz_in_crop [B,2] (used in float64).
         Returns (best_idx int32 [B], pos int32 [B,2] = (delta_y, delta_x), records f32 [B,8])."""
         B = cls.shape[0]
         dev = self._device
         anchors = anchors.to(dev, torch.float32).contiguous()
-        window = window.to(dev, torch.float32).contiguous()
+        window = window.to(dev, torch.float64).contiguous()
         tsz = torch.as_tensor(target_sz_in_crop).to(dev, torch.float64).reshape(B, 2).contiguous()
         n = self.anchor_num * self.score_size ** 2
         if anchors.shape != (n, 4) or window.numel() != n:
@@ -420,7 +421,7 @@ class Custom:
         B, A, R = x.shape[0], self.anchor_num, self.score_size
         n = A * R * R
         anchors = anchors.to(dev, torch.float32).contiguous()
-        window = window.to(dev, torch.float32).contiguous()
+        window = window.to(dev, torch.float64).contiguous()
         if anchors.shape != (n, 4) or window.numel() != n:
             raise ValueError(f"anchors/window must have {n} entries")
         tsz = torch.as_tensor(target_sz_in_crop).to(dev, torch.float64).reshape(B, 2).contiguous()

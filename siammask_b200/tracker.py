@@ -216,7 +216,7 @@ class BatchTracker:
         self.lib = _lib.load()
         R, A = self.p.score_size, net.anchor_num
         self.anchors = torch.from_numpy(generate_anchor(net.anchors, R)).to(self.dev)
-        self.window = torch.from_numpy(cosine_window(R, A, self.p.windowing).astype(np.float32)).to(self.dev)
+        self.window = torch.from_numpy(cosine_window(R, A, self.p.windowing)).to(self.dev)
         self.hp = self.p.c_struct()
         self.packer = FramePacker(self.dev)
         self._next_id = 0

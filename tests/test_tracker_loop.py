@@ -68,7 +68,7 @@ def test_device_select_matches_numpy(calib_sd):
     anchor = tracker.generate_anchor(smb.DEFAULT_ANCHORS, 25)
     window = np.tile(np.outer(np.hanning(25), np.hanning(25)).flatten(), 5)
     tsz = np.array([[60.0, 40.0], [35.5, 80.25], [100.0, 100.0]])
-    best, pos, rec = m.select(cls, loc, torch.from_numpy(anchor), torch.from_numpy(window.astype(np.float32)),
+    best, pos, rec = m.select(cls, loc, torch.from_numpy(anchor), torch.from_numpy(window),
                               torch.from_numpy(tsz), 0.04, 0.4)
     best, pos, rec = best.cpu().numpy(), pos.cpu().numpy(), rec.cpu().numpy()
     for b in range(3):
