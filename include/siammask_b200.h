@@ -379,16 +379,31 @@ int sm_track_host_async(sm_engine* e, int32_t slot0, int32_t B, const float* x_h
 int sm_track_host_wait(sm_engine* e, int32_t ticket);
 
 /* conv2d_dw_group — models/rpn.py:32-38, standalone: x f32 [B,C,H,W], k f32 [B,C,kh,kw] ->
- * out f32 [B,C,H-kh+1,W-kw+1], all device pointers. */
+ * out f32 [B,C,H-kh+1,W-kw+1], all device pointers.  B, C, kh, kw >= 1, H >= kh, W >= kw and every tensor below 2^31
+ * elements; the arguments are checked before the device is touched. */
 int sm_xcorr_depthwise(const float* x, const float* k, float* out, int32_t B, int32_t C, int32_t H, int32_t W,
                        int32_t kh, int32_t kw, void* stream);
 
 /* F.conv2d + folded affine (+ReLU) as a standalone operator, used by the kernel-level parity tests:
  * x f32 NCHW [B,Cin,H,W], w f32 [Cout,Cin,KH,KW], scale/shift f32 [Cout] (may be NULL), out f32 NCHW.
- * backend/precision as in sm_config. */
+ * backend/precision as in sm_config.  Accepted geometry (checked before the device is touched, see sm_conv2d_route):
+ * sizes >= 1, stride and dilation >= 1, pad >= 0, an output of at least 1 x 1, every tensor below 2^31 elements; the
+ * tensor backend also needs Cin % 64 == 0 and, off the 1x1 / stride 1 / pad 0 path, stride <= 8 and the im2col
+ * corners -pad and pad - (k-1)*dil inside [-128, 127] (the TMA limits of a rank-4 im2col map).  Inputs are stored at
+ * a power-of-two scale chosen from max |x| and weights at a per-channel one, so the fp16 operand planes hold neither
+ * infinities nor subnormals for max |x| in about [2^-54, 2^74] and max |w| per channel in about [2^-48, 2^76]. */
 int sm_conv2d(const float* x, const float* w, const float* scale, const float* shift, float* out, int32_t B,
               int32_t Cin, int32_t H, int32_t W, int32_t Cout, int32_t KH, int32_t KW, int32_t stride, int32_t pad,
               int32_t dil, int32_t relu, int32_t backend, int32_t precision, void* stream);
+
+/* Which kernel sm_conv2d runs for a geometry, without a device: *route = SM_CONV_ROUTE_*.  Returns -1 (and
+ * sm_last_error) for the arguments sm_conv2d rejects. */
+enum { SM_CONV_ROUTE_SIMT = 0,         /* CUDA-core reference conv (SM_BACKEND_SIMT) */
+       SM_CONV_ROUTE_GEMM_TILED = 1,   /* wgmma implicit GEMM, 2-D tiled operand loads (1x1, stride 1, pad 0) */
+       SM_CONV_ROUTE_GEMM_IM2COL = 2,  /* wgmma implicit GEMM, im2col operand loads */
+       SM_CONV_ROUTE_PATCH = 3         /* resident-patch 3x3 kernel (fp16 split-plane output, re-expanded to f32) */ };
+int sm_conv2d_route(int32_t B, int32_t Cin, int32_t H, int32_t W, int32_t Cout, int32_t KH, int32_t KW, int32_t stride,
+                    int32_t pad, int32_t dil, int32_t backend, int32_t precision, int32_t* route);
 
 /* Copies a cached intermediate of the last sm_template / sm_track as f32 NCHW (parity checks):
  * "p0","p1","p2","p3","search","corr_cls","corr_loc","corr_mask","zf".  shape4 receives [B,C,H,W];

@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(HERE, "libsiammask_b200.so")
 
 SM_PRECISION_EXACT, SM_PRECISION_FAST = 0, 1
 SM_BACKEND_TENSOR, SM_BACKEND_SIMT = 0, 1
+SM_CONV_ROUTE_SIMT, SM_CONV_ROUTE_GEMM_TILED, SM_CONV_ROUTE_GEMM_IM2COL, SM_CONV_ROUTE_PATCH = 0, 1, 2, 3
 SM_TRACK_MASK_FEATURES, SM_TRACK_MASK_HEAD = 1, 2
 
 
@@ -105,6 +106,7 @@ SIGNATURES = {
                                      C.POINTER(C.c_int32)]),
     "sm_xcorr_depthwise": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int32] * 6 + [C.c_void_p]),
     "sm_conv2d": (C.c_int, [C.c_void_p] * 5 + [C.c_int32] * 13 + [C.c_void_p]),
+    "sm_conv2d_route": (C.c_int, [C.c_int32] * 12 + [C.POINTER(C.c_int32)]),
     "sm_export": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "sm_engine_set_graphs": (C.c_int, [C.c_void_p, C.c_int32]),
     "sm_profile_enable": (C.c_int, [C.c_void_p, C.c_int32]),

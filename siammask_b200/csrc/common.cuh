@@ -26,7 +26,8 @@ struct Act {
 
 struct ConvGeom {
   int Cin, Cout, KH, KW, stride, pad, dil;
-  __host__ __device__ int out_size(int in) const { return (in + 2 * pad - dil * (KH - 1) - 1) / stride + 1; }
+  __host__ __device__ int out_h(int in) const { return (in + 2 * pad - dil * (KH - 1) - 1) / stride + 1; }
+  __host__ __device__ int out_w(int in) const { return (in + 2 * pad - dil * (KW - 1) - 1) / stride + 1; }
 };
 
 enum OutMode : int { OUT_NHWC_SPLIT = 0, OUT_NHWC_F32 = 1, OUT_NCHW_F32 = 2 };
@@ -136,7 +137,8 @@ CUtensorMap make_map_tiled_nd(const __half* base, int rank, const uint64_t* dims
                               const uint32_t* box, int swizzle_bytes);
 
 // conv3x3_patch_sm90.cu : 3x3 / s1 / p1 / Cin == Cout in {64, 128} on a resident input patch (no im2col traffic)
-bool patch_conv_supported(const Act& in, const ConvGeom& g);
+// nsplit as in launch_conv3x3_patch: the two patch buffers of 2 planes at 128 channels and PW 64 exceed shared memory
+bool patch_conv_supported(const Act& in, const ConvGeom& g, int nsplit);
 void launch_conv3x3_patch(const Act& in, const ConvGeom& g, const __half* w_hi, const __half* w_lo, int w_ld,
                           const Epilogue& ep, int nsplit, int num_sms, cudaStream_t st);
 
@@ -194,8 +196,9 @@ void launch_gather_corr(const Act& corr, const int32_t* pos, float* out, float m
 void launch_gather_mask_col(const float* mask, const int32_t* pos, int B, int C, int R, float* out, cudaStream_t st);
 void launch_deconv(const float* p3, const float* w, const float* bias, float* out, int B, int Cin, int N,
                    int cout, cudaStream_t st);
-void launch_split_to_f32(const Act& in, float* out, cudaStream_t st, float mul = 1.f);
-void launch_import_nchw(const float* x_nchw, Act out, cudaStream_t st);
+// NHWC split planes -> NCHW fp32, times mul or, when cmul is given, times the per-channel cmul[c] (device [C])
+void launch_split_to_f32(const Act& in, float* out, cudaStream_t st, float mul = 1.f, const float* cmul = nullptr);
+void launch_import_nchw(const float* x_nchw, Act out, cudaStream_t st, float mul = 1.f);
 // dst_desc (optional, sm_warp_affine_ragged): image b is dst_desc[b].h x dst_desc[b].w at dst + dst_desc[b].offset,
 // and dh, dw are the largest h, w
 void launch_warp_affine(const float* src, int sh, int sw, const double* maps, float* dst, int dh, int dw, float border,

@@ -251,11 +251,18 @@ int patch_ro(int W) {
   return 128 % pw == 0 ? 128 / pw : 0;
 }
 
+int patch_panel_bytes(int W) { return ((patch_ro(W) + 2) * patch_pw(W) + 2 * P_SLACK_ROWS) * 128; }
+
+// two patch buffers of nsplit panels, the weight ring, barriers and alignment slack (PCfg)
+int patch_smem_bytes(int W, int cm, int nsplit) {
+  return 2 * nsplit * patch_panel_bytes(W) + 3 * nsplit * cm * 128 + 256 + 1024;
+}
+
 template <int CM, int NSPLIT>
 void launch_patch(const PatchParams& p, int num_sms, cudaStream_t st) {
   using C = PCfg<CM, NSPLIT>;
   const int smem = 2 * NSPLIT * p.panel_bytes + C::B_STAGES * C::B_STAGE_BYTES + 256 + 1024;
-  SMK_CHECK(smem <= 227 * 1024, "patch conv: shared memory budget");
+  SMK_CHECK(smem == patch_smem_bytes(p.W, CM, NSPLIT) && smem <= 227 * 1024, "patch conv: shared memory budget");
   auto kern = conv3x3_patch_kernel<CM, NSPLIT>;
   static unsigned long long attr = 0;
   ensure_dynamic_smem(kern, 227 * 1024, attr);
@@ -266,16 +273,16 @@ void launch_patch(const PatchParams& p, int num_sms, cudaStream_t st) {
 
 }  // namespace
 
-bool patch_conv_supported(const Act& in, const ConvGeom& g) {
+bool patch_conv_supported(const Act& in, const ConvGeom& g, int nsplit) {
   if (!(g.KH == 3 && g.KW == 3 && g.stride == 1 && g.pad == 1 && g.dil == 1 && g.Cin == g.Cout)) return false;
   if (!(g.Cin == 64 || g.Cin == 128)) return false;
   if (in.H != in.W) return false;
-  return patch_ro(in.W) >= 1 && patch_pw(in.W) <= 64;
+  return patch_ro(in.W) >= 1 && patch_pw(in.W) <= 64 && patch_smem_bytes(in.W, g.Cin, nsplit) <= 227 * 1024;
 }
 
 void launch_conv3x3_patch(const Act& in, const ConvGeom& g, const __half* w_hi, const __half* w_lo, int w_ld,
                           const Epilogue& ep, int nsplit, int num_sms, cudaStream_t st) {
-  SMK_CHECK(patch_conv_supported(in, g), "patch conv: unsupported geometry");
+  SMK_CHECK(patch_conv_supported(in, g, nsplit), "patch conv: unsupported geometry");
   SMK_CHECK(ep.out_mode == OUT_NHWC_SPLIT && ep.res_hi == nullptr, "patch conv writes NHWC split planes, no residual");
   SMK_CHECK(nsplit == 1 || (in.lo != nullptr && w_lo != nullptr && ep.out_lo != nullptr), "exact mode needs lo planes");
   SMK_CHECK(w_ld >= 9 * g.Cin, "weight row length");
@@ -286,7 +293,7 @@ void launch_conv3x3_patch(const Act& in, const ConvGeom& g, const __half* w_hi, 
   p.tiles_per_img = (in.H + p.RO - 1) / p.RO;
   p.num_tiles = in.B * p.tiles_per_img;
   p.patch_rows = (p.RO + 2) * p.PW;
-  p.panel_bytes = (p.patch_rows + 2 * P_SLACK_ROWS) * 128;
+  p.panel_bytes = patch_panel_bytes(in.W);
   SMK_CHECK(p.panel_bytes % 1024 == 0, "patch panels must keep the 1024-byte swizzle alignment");
   p.ep = ep;
   for (int s = 0; s < nsplit; ++s) {

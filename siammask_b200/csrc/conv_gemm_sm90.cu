@@ -632,7 +632,7 @@ void launch_gemm_multi(const GemmInput* convs, int nconv, const Act* residual, c
   SMK_CHECK(nconv >= 1 && nconv <= 2, "1 or 2 convolution segments");
   const ConvGeom& g0 = convs[0].g;
   const Act& in0 = convs[0].in;
-  const int Ho = g0.out_size(in0.H), Wo = g0.out_size(in0.W);
+  const int Ho = g0.out_h(in0.H), Wo = g0.out_w(in0.W);
   GemmParams p;
   std::memset(&p, 0, sizeof p);
   p.M = in0.B * Ho * Wo;
@@ -653,7 +653,7 @@ void launch_gemm_multi(const GemmInput* convs, int nconv, const Act* residual, c
     const Act& in = convs[i].in;
     SMK_CHECK(gemm_conv_supported(g), "Cin must be a multiple of 64 for the tensor-core conv");
     SMK_CHECK(in.C == g.Cin && g.Cout == g0.Cout && in.B == in0.B, "segment channels/batch mismatch");
-    SMK_CHECK(g.out_size(in.H) == Ho && g.out_size(in.W) == Wo, "segments must produce the same output size");
+    SMK_CHECK(g.out_h(in.H) == Ho && g.out_w(in.W) == Wo, "segments must produce the same output size");
     SMK_CHECK(nsplit == 1 || (in.lo != nullptr && w_lo != nullptr), "exact mode needs lo planes");
     GemmSegment& sg = p.seg[i];
     sg.KW = g.KW;

@@ -1038,7 +1038,7 @@ F32T Engine::alloc_f32(Arena& ar, int B, int H, int W, int C) {
 void Engine::conv_into(const Act& in, const ConvW& Lw, Epilogue ep, cudaStream_t st, const Act* res,
                        const Act* in2) {
   ep.beta = Lw.beta;
-  const double M = (double)in.B * Lw.g.out_size(in.H) * Lw.g.out_size(in.W);
+  const double M = (double)in.B * Lw.g.out_h(in.H) * Lw.g.out_w(in.W);
   double K = (double)Lw.g.KH * Lw.g.KW * Lw.g.Cin;
   const bool tc = cfg_.backend == SM_BACKEND_TENSOR && Lw.gemm_ok;
   SMK_CHECK(in2 == nullptr || (tc && Lw.fused2), "fused second input needs the tensor-core path");
@@ -1076,7 +1076,7 @@ void Engine::conv_into(const Act& in, const ConvW& Lw, Epilogue ep, cudaStream_t
   if (res != nullptr && res->numel() > big->numel()) big = res;
   // bottleneck conv2 (3x3 / s1 / p1, 64 or 128 channels): resident-patch kernel, walks its tiles front to back
   const bool use_patch = in2 == nullptr && res == nullptr && ep.out_mode == OUT_NHWC_SPLIT &&
-                         patch_conv_supported(in, Lw.g);
+                         patch_conv_supported(in, Lw.g, exact_ ? 2 : 1);
   const bool reverse = !use_patch && end_of(*big) > 0;
   GemmInput gi[2] = {{in, Lw.g, 0}, {in, Lw.g, 0}};
   int nconv = 1;
@@ -1129,7 +1129,7 @@ void Engine::note_tensor(const F32T& t, const std::string& name) {
 
 Act Engine::conv(const Act& in, const ConvW& Lw, bool relu, const Act* res, Arena& ar, cudaStream_t st,
                  const Act* in2) {
-  Act out = alloc_act(ar, in.B, Lw.g.out_size(in.H), Lw.g.out_size(in.W), Lw.g.Cout);
+  Act out = alloc_act(ar, in.B, Lw.g.out_h(in.H), Lw.g.out_w(in.W), Lw.g.Cout);
   Epilogue ep;
   ep.relu = relu ? 1 : 0;
   ep.out_mode = OUT_NHWC_SPLIT;
@@ -1142,7 +1142,7 @@ Act Engine::conv(const Act& in, const ConvW& Lw, bool relu, const Act* res, Aren
 }
 
 F32T Engine::conv_f32(const Act& in, const ConvW& Lw, bool relu, Arena& ar, cudaStream_t st) {
-  F32T out = alloc_f32(ar, in.B, Lw.g.out_size(in.H), Lw.g.out_size(in.W), Lw.g.Cout);
+  F32T out = alloc_f32(ar, in.B, Lw.g.out_h(in.H), Lw.g.out_w(in.W), Lw.g.Cout);
   Epilogue ep;
   ep.relu = relu ? 1 : 0;
   ep.out_mode = OUT_NHWC_F32;
@@ -1725,36 +1725,84 @@ std::string Engine::profile_dump() {
 // ================================================================================================
 // standalone conv operator (kernel-level parity tests)
 
+// The arguments sm_conv2d accepts and the kernel it runs them on (SM_CONV_ROUTE_*); throws for the rest.  No device.
+static int conv2d_route(int B, int Cin, int H, int W, int Cout, int KH, int KW, int stride, int pad, int dil,
+                        int backend, int precision) {
+  SMK_CHECK(B >= 1 && Cin >= 1 && H >= 1 && W >= 1 && Cout >= 1 && KH >= 1 && KW >= 1, "sizes must be >= 1");
+  SMK_CHECK(stride >= 1 && dil >= 1 && pad >= 0, "stride and dilation must be >= 1 and padding >= 0");
+  SMK_CHECK(backend == SM_BACKEND_TENSOR || backend == SM_BACKEND_SIMT, "unknown backend");
+  SMK_CHECK(precision == SM_PRECISION_EXACT || precision == SM_PRECISION_FAST, "unknown precision");
+  // output size in 64 bits: ConvGeom::out_h / out_w truncate a negative span towards zero
+  const int64_t span_h = (int64_t)H + 2 * (int64_t)pad - (int64_t)dil * (KH - 1) - 1;
+  const int64_t span_w = (int64_t)W + 2 * (int64_t)pad - (int64_t)dil * (KW - 1) - 1;
+  SMK_CHECK(span_h >= 0 && span_w >= 0, "the (dilated) kernel does not fit the padded input: empty output");
+  const int64_t Ho = span_h / stride + 1, Wo = span_w / stride + 1, lim = (int64_t)1 << 31;
+  SMK_CHECK((int64_t)B * Cin * H * W < lim && (int64_t)Cout * Cin * KH * KW < lim && (int64_t)B * Cout * Ho * Wo < lim,
+            "every tensor must have fewer than 2^31 elements");
+  if (backend == SM_BACKEND_SIMT) return SM_CONV_ROUTE_SIMT;
+  const ConvGeom g{Cin, Cout, KH, KW, stride, pad, dil};
+  SMK_CHECK(gemm_conv_supported(g), "tensor-core conv needs Cin % 64 == 0");
+  Act in;
+  in.B = B; in.H = H; in.W = W; in.C = Cin;
+  if (patch_conv_supported(in, g, precision == SM_PRECISION_EXACT ? 2 : 1)) return SM_CONV_ROUTE_PATCH;
+  if (KH == 1 && KW == 1 && stride == 1 && pad == 0) return SM_CONV_ROUTE_GEMM_TILED;   // launch_gemm_multi's mode 0
+  // rank-4 im2col tensor map (make_map_im2col_raw): elementStrides <= 8, corners in [-128, 127]
+  SMK_CHECK(stride <= 8, "tensor-core conv: stride must be <= 8 (TMA element stride)");
+  const int64_t up_w = pad - (int64_t)(KW - 1) * dil, up_h = pad - (int64_t)(KH - 1) * dil;
+  SMK_CHECK(pad <= 128 && up_w >= -128 && up_w <= 127 && up_h >= -128 && up_h <= 127,
+            "tensor-core conv: -pad and pad - (k-1)*dil must lie in [-128, 127] (TMA im2col corners)");
+  return SM_CONV_ROUTE_GEMM_IM2COL;
+}
+
+// power-of-two exponent that brings max |w| of a weight column to ~2^14.  Clamped only so that the epilogue's
+// 2^-(e + s_in) stays a normal float (|e| <= 62, |s_in| <= 64): the engine's narrower weight_exp clamp would leave a
+// column below ~2^-27 with a subnormal lo plane.
+static int op_weight_exp(float amax) {
+  const int e = amax > 0.f ? (int)std::floor(std::log2(16384.0 / (double)amax)) : 0;
+  return std::max(-62, std::min(62, e));
+}
+
 static void conv2d_op(const float* x, const float* w, const float* scale, const float* shift, float* out, int B,
                       int Cin, int H, int W, int Cout, int KH, int KW, int stride, int pad, int dil, int relu,
                       int backend, int precision, cudaStream_t st) {
+  const int route = conv2d_route(B, Cin, H, W, Cout, KH, KW, stride, pad, dil, backend, precision);
   ConvGeom g{Cin, Cout, KH, KW, stride, pad, dil};
   const bool exact = precision == SM_PRECISION_EXACT;
-  const bool use_gemm = backend == SM_BACKEND_TENSOR;
-  SMK_CHECK(!use_gemm || gemm_conv_supported(g), "tensor-core conv needs Cin % 64 == 0");
+  const bool use_gemm = route != SM_CONV_ROUTE_SIMT;
   const size_t K = (size_t)KH * KW * Cin;
   const int cout_pad = use_gemm ? gemm_cout_pad(Cout) : Cout;
-  std::vector<float> hw(K * Cout), hs(Cout, 1.f), hb(Cout, 0.f);
+  const size_t nx = (size_t)B * Cin * H * W;
+  std::vector<float> hx(nx), hw(K * Cout), hs(Cout, 1.f), hb(Cout, 0.f);
   SMK_CUDA(cudaStreamSynchronize(st));
+  SMK_CUDA(cudaMemcpy(hx.data(), x, nx * sizeof(float), cudaMemcpyDeviceToHost));
   SMK_CUDA(cudaMemcpy(hw.data(), w, hw.size() * sizeof(float), cudaMemcpyDeviceToHost));
   if (scale) SMK_CUDA(cudaMemcpy(hs.data(), scale, Cout * sizeof(float), cudaMemcpyDeviceToHost));
   if (shift) SMK_CUDA(cudaMemcpy(hb.data(), shift, Cout * sizeof(float), cudaMemcpyDeviceToHost));
+  // Input exponent: x is stored as x * 2^s_in with max |x| * 2^s_in near 2^10, where calibrate() puts the engine's
+  // activations, so large inputs do not overflow the fp16 planes and small ones keep their lo plane out of fp16's
+  // subnormals.  Folded into alpha with the weight exponent.
+  float xmax = 0.f;
+  for (float v : hx) xmax = std::max(xmax, std::fabs(v));
+  const int s_in = xmax > 0.f && std::isfinite(xmax)
+                       ? std::max(-64, std::min(64, (int)std::floor(std::log2(1024.0 / (double)xmax)))) : 0;
   std::vector<float> wref(K * Cout), alpha(cout_pad, 0.f), beta(cout_pad, 0.f);
   std::vector<__half> whi((size_t)cout_pad * K, __float2half_rn(0.f)), wlo((size_t)cout_pad * K, __float2half_rn(0.f));
   const int HW = KH * KW;
+  const bool patch = route == SM_CONV_ROUTE_PATCH;
+  std::vector<int> s_out(Cout, 0);
+  std::vector<float> out_mul(Cout, 1.f);
   for (int n = 0; n < Cout; ++n) {
     float amax = 0.f;
+    double wsum = 0.0;
     for (int c = 0; c < Cin; ++c)
       for (int t = 0; t < HW; ++t) {
         const float fw = (float)((double)hw[((size_t)n * Cin + c) * HW + t] * (double)hs[n]);
         wref[((size_t)t * Cin + c) * Cout + n] = fw;
         amax = std::max(amax, std::fabs(fw));
+        wsum += std::fabs((double)fw);
       }
-    beta[n] = hb[n];
-    alpha[n] = 1.f;
+    const int e = use_gemm ? op_weight_exp(amax) : 0;
     if (use_gemm) {
-      const int e = weight_exp(amax);
-      alpha[n] = std::ldexp(1.f, -e);
       for (int c = 0; c < Cin; ++c)
         for (int t = 0; t < HW; ++t) {
           const float fw = std::ldexp(wref[((size_t)t * Cin + c) * Cout + n], e);
@@ -1763,12 +1811,23 @@ static void conv2d_op(const float* x, const float* w, const float* scale, const 
           wlo[((size_t)n * HW + t) * Cin + c] = __float2half_rn(fw - __half2float(h));
         }
     }
+    // Output exponent of the patch route, whose fp16 split planes hold |v| <= 65504 and lose precision below ~2^-3:
+    // channel n is stored at 2^s_out[n] with bound * 2^s_out[n] near 2^15, where bound = max|x| * sum |w| + |shift|
+    // bounds |out| (then re-expanded by the export).  Clamped so that alpha and the export's 2^-s_out stay normal
+    // floats.  The GEMM and SIMT routes write fp32 directly.
+    const double bound = (double)xmax * wsum + std::fabs((double)hb[n]);
+    if (patch && bound > 0.0 && std::isfinite(bound)) {
+      const int lo = std::max(-126, e + s_in - 126), hi = std::min(126, e + s_in + 126);
+      s_out[n] = std::max(lo, std::min(hi, (int)std::floor(std::log2(32768.0 / bound))));
+      out_mul[n] = std::ldexp(1.f, -s_out[n]);
+    }
+    alpha[n] = std::ldexp(1.f, s_out[n] - e - s_in);
+    beta[n] = (float)std::ldexp((double)hb[n], s_out[n]);
   }
-  const int Ho = g.out_size(H), Wo = g.out_size(W);
   Act in;
   in.B = B; in.H = H; in.W = W; in.C = Cin;
   __half *d_whi = nullptr, *d_wlo = nullptr;
-  float *d_wref = nullptr, *d_alpha = nullptr, *d_beta = nullptr;
+  float *d_wref = nullptr, *d_alpha = nullptr, *d_beta = nullptr, *d_mul = nullptr;
   SMK_CUDA(cudaMalloc(&in.hi, in.numel() * sizeof(__half)));
   if (exact) SMK_CUDA(cudaMalloc(&in.lo, in.numel() * sizeof(__half)));
   SMK_CUDA(cudaMalloc(&d_whi, whi.size() * sizeof(__half)));
@@ -1781,7 +1840,7 @@ static void conv2d_op(const float* x, const float* w, const float* scale, const 
   SMK_CUDA(cudaMemcpy(d_wref, wref.data(), wref.size() * sizeof(float), cudaMemcpyHostToDevice));
   SMK_CUDA(cudaMemcpy(d_alpha, alpha.data(), alpha.size() * sizeof(float), cudaMemcpyHostToDevice));
   SMK_CUDA(cudaMemcpy(d_beta, beta.data(), beta.size() * sizeof(float), cudaMemcpyHostToDevice));
-  launch_import_nchw(x, in, st);
+  launch_import_nchw(x, in, st, std::ldexp(1.f, s_in));
   Epilogue ep;
   ep.alpha = d_alpha;
   ep.beta = d_beta;
@@ -1791,11 +1850,10 @@ static void conv2d_op(const float* x, const float* w, const float* scale, const 
   int dev = 0, sms = 132;
   SMK_CUDA(cudaGetDevice(&dev));
   SMK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  (void)Ho; (void)Wo;
-  if (use_gemm && patch_conv_supported(in, g)) {
+  if (patch) {
     // the engine runs this geometry on the resident-patch kernel (NHWC split output): same here, then export
     Act o;
-    o.B = B; o.H = Ho; o.W = Wo; o.C = Cout;
+    o.B = B; o.H = g.out_h(H); o.W = g.out_w(W); o.C = Cout;
     SMK_CUDA(cudaMalloc(&o.hi, o.numel() * sizeof(__half)));
     if (exact) SMK_CUDA(cudaMalloc(&o.lo, o.numel() * sizeof(__half)));
     Epilogue e2 = ep;
@@ -1804,9 +1862,11 @@ static void conv2d_op(const float* x, const float* w, const float* scale, const 
     e2.out_lo = o.lo;
     e2.out_f32 = nullptr;
     launch_conv3x3_patch(in, g, d_whi, d_wlo, (int)K, e2, exact ? 2 : 1, sms, st);
-    launch_split_to_f32(o, out, st);
+    SMK_CUDA(cudaMalloc(&d_mul, Cout * sizeof(float)));
+    SMK_CUDA(cudaMemcpy(d_mul, out_mul.data(), Cout * sizeof(float), cudaMemcpyHostToDevice));
+    launch_split_to_f32(o, out, st, 1.f, d_mul);
     SMK_CUDA(cudaStreamSynchronize(st));
-    cudaFree(o.hi); cudaFree(o.lo);
+    cudaFree(o.hi); cudaFree(o.lo); cudaFree(d_mul);
   } else if (use_gemm) launch_gemm_conv(in, g, d_whi, d_wlo, cout_pad, ep, exact ? 2 : 1, sms, st);
   else launch_ref_conv(in, g, d_wref, ep, st);
   SMK_CUDA(cudaStreamSynchronize(st));
@@ -2005,6 +2065,10 @@ int sm_xcorr_depthwise(const float* x, const float* k, float* out, int32_t B, in
                        int32_t kw, void* stream) {
   SM_API_BEGIN
   SMK_CHECK(x && k && out, "null argument");
+  SMK_CHECK(B >= 1 && C >= 1 && kh >= 1 && kw >= 1, "sizes must be >= 1");
+  SMK_CHECK(H >= kh && W >= kw, "the kernel must fit the input (valid correlation)");
+  SMK_CHECK((int64_t)B * C * H * W < ((int64_t)1 << 31) && (int64_t)B * C * kh * kw < ((int64_t)1 << 31),
+            "every tensor must have fewer than 2^31 elements");
   require_device();
   smk::launch_xcorr_nchw_f32(x, k, out, B * C, H, W, kh, kw, static_cast<cudaStream_t>(stream));
   SM_API_END
@@ -2015,9 +2079,18 @@ int sm_conv2d(const float* x, const float* w, const float* scale, const float* s
               int32_t relu, int32_t backend, int32_t precision, void* stream) {
   SM_API_BEGIN
   SMK_CHECK(x && w && out, "null argument");
+  smk::conv2d_route(B, Cin, H, W, Cout, KH, KW, stride, pad, dil, backend, precision);   // arguments first
   require_device();
   smk::conv2d_op(x, w, scale, shift, out, B, Cin, H, W, Cout, KH, KW, stride, pad, dil, relu, backend, precision,
                  static_cast<cudaStream_t>(stream));
+  SM_API_END
+}
+
+int sm_conv2d_route(int32_t B, int32_t Cin, int32_t H, int32_t W, int32_t Cout, int32_t KH, int32_t KW, int32_t stride,
+                    int32_t pad, int32_t dil, int32_t backend, int32_t precision, int32_t* route) {
+  SM_API_BEGIN
+  SMK_CHECK(route, "null argument");
+  *route = smk::conv2d_route(B, Cin, H, W, Cout, KH, KW, stride, pad, dil, backend, precision);
   SM_API_END
 }
 

@@ -578,27 +578,28 @@ __global__ void absmax_kernel(const __half* __restrict__ hi, size_t n8, float* _
   }
 }
 
-// NCHW fp32 -> NHWC split planes (standalone-operator entry, sm_conv2d).
-__global__ void import_nchw_kernel(const float* __restrict__ x, Act out) {
+// NCHW fp32 -> NHWC split planes of x * mul (standalone-operator entry, sm_conv2d; mul a power of two).
+__global__ void import_nchw_kernel(const float* __restrict__ x, Act out, float mul) {
   const size_t total = out.numel();
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
     const int c = idx % out.C;
     const int w = (idx / out.C) % out.W;
     const int h = (idx / ((size_t)out.C * out.W)) % out.H;
     const int b = idx / ((size_t)out.C * out.W * out.H);
-    split_store(out.hi, out.lo, idx, x[(((size_t)b * out.C + c) * out.H + h) * out.W + w]);
+    split_store(out.hi, out.lo, idx, x[(((size_t)b * out.C + c) * out.H + h) * out.W + w] * mul);
   }
 }
 
-// NHWC split planes -> NCHW fp32 (exports cached features for parity checks / the Python boundary).
-__global__ void export_nchw_kernel(Act in, float* __restrict__ out, float mul) {
+// NHWC split planes -> NCHW fp32 (exports cached features for parity checks / the Python boundary), times mul or, when
+// given, the per-channel cmul[c].
+__global__ void export_nchw_kernel(Act in, float* __restrict__ out, float mul, const float* __restrict__ cmul) {
   const size_t total = in.numel();
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
     const int w = idx % in.W;
     const int h = (idx / in.W) % in.H;
     const int c = (idx / ((size_t)in.W * in.H)) % in.C;
     const int b = idx / ((size_t)in.W * in.H * in.C);
-    out[idx] = mul * split_load(in.hi, in.lo, (((size_t)b * in.H + h) * in.W + w) * in.C + c);
+    out[idx] = (cmul != nullptr ? cmul[c] : mul) * split_load(in.hi, in.lo, (((size_t)b * in.H + h) * in.W + w) * in.C + c);
   }
 }
 
@@ -1899,7 +1900,7 @@ inline int grid_for(size_t total, int block) {
 
 // ================================================================================================
 void launch_ref_conv(const Act& in, const ConvGeom& g, const float* w, const Epilogue& ep, cudaStream_t st) {
-  const int Ho = g.out_size(in.H), Wo = g.out_size(in.W);
+  const int Ho = g.out_h(in.H), Wo = g.out_w(in.W);
   const size_t total = (size_t)in.B * Ho * Wo * g.Cout;
   ref_conv_kernel<<<grid_for(total, 256), 256, 0, st>>>(in, g, w, ep, Ho, Wo);
   SMK_CUDA(cudaGetLastError());
@@ -2008,13 +2009,13 @@ void launch_absmax(const Act& a, float* slot, cudaStream_t st) {
   SMK_CUDA(cudaGetLastError());
 }
 
-void launch_split_to_f32(const Act& in, float* out, cudaStream_t st, float mul) {
-  export_nchw_kernel<<<grid_for(in.numel(), 256), 256, 0, st>>>(in, out, mul);
+void launch_split_to_f32(const Act& in, float* out, cudaStream_t st, float mul, const float* cmul) {
+  export_nchw_kernel<<<grid_for(in.numel(), 256), 256, 0, st>>>(in, out, mul, cmul);
   SMK_CUDA(cudaGetLastError());
 }
 
-void launch_import_nchw(const float* x, Act out, cudaStream_t st) {
-  import_nchw_kernel<<<grid_for(out.numel(), 256), 256, 0, st>>>(x, out);
+void launch_import_nchw(const float* x, Act out, cudaStream_t st, float mul) {
+  import_nchw_kernel<<<grid_for(out.numel(), 256), 256, 0, st>>>(x, out, mul);
   SMK_CUDA(cudaGetLastError());
 }
 

@@ -37,11 +37,35 @@ def conv2d_dw_group(x: torch.Tensor, kernel: torch.Tensor) -> torch.Tensor:
 xcorr_depthwise = conv2d_dw_group
 
 
+CONV_ROUTES = {_lib.SM_CONV_ROUTE_SIMT: "simt", _lib.SM_CONV_ROUTE_GEMM_TILED: "gemm_tiled",
+               _lib.SM_CONV_ROUTE_GEMM_IM2COL: "gemm_im2col", _lib.SM_CONV_ROUTE_PATCH: "patch"}
+
+
+def conv2d_route(x_shape, w_shape, stride=1, padding=0, dilation=1, backend="tensor", precision="exact") -> str:
+    """The kernel `conv2d` runs for these shapes (C ABI `sm_conv2d_route`, no device needed): 'simt', 'gemm_tiled',
+    'gemm_im2col' or 'patch'.  Raises RuntimeError for the arguments `conv2d` rejects."""
+    if len(x_shape) != 4 or len(w_shape) != 4 or int(w_shape[1]) != int(x_shape[1]):
+        raise RuntimeError(f"conv2d needs x [B,Cin,H,W] and weight [Cout,Cin,KH,KW], got {tuple(x_shape)} and "
+                           f"{tuple(w_shape)}")
+    be = {"tensor": _lib.SM_BACKEND_TENSOR, "simt": _lib.SM_BACKEND_SIMT}[backend]
+    pr = {"exact": _lib.SM_PRECISION_EXACT, "fast": _lib.SM_PRECISION_FAST}[precision]
+    B, Cin, H, W = (int(v) for v in x_shape)
+    Cout, _, KH, KW = (int(v) for v in w_shape)
+    route = C.c_int32(-1)
+    _lib.check(_lib.load().sm_conv2d_route(B, Cin, H, W, Cout, KH, KW, int(stride), int(padding), int(dilation), be, pr,
+                                           C.byref(route)))
+    return CONV_ROUTES[route.value]
+
+
 def conv2d(x, weight, scale=None, shift=None, stride=1, padding=0, dilation=1, relu=False, backend="tensor",
            precision="exact", out=None):
     """F.conv2d(x, weight) * scale[c] + shift[c] (+ReLU) through the engine's convolution kernels.
     x f32[B,Cin,H,W] NCHW, weight f32[Cout,Cin,KH,KW]; returns f32 NCHW, written into `out` when given (a contiguous
-    f32 tensor of the output's shape on x's device)."""
+    f32 tensor of the output's shape on x's device).  The geometry is checked first (`conv2d_route`)."""
+    conv2d_route(x.shape, weight.shape, stride, padding, dilation, backend, precision)
+    for name, t in (("scale", scale), ("shift", shift)):
+        if t is not None and t.numel() != weight.shape[0]:
+            raise RuntimeError(f"{name} must have one entry per output channel ({weight.shape[0]})")
     if not x.is_cuda:
         raise RuntimeError("siammask_b200 operators run on CUDA tensors only; there is no CPU path")
     lib = _lib.load()
