@@ -254,6 +254,14 @@ int sm_vot_trajectory_overlap(const double* rec, int32_t T, int32_t S, const flo
                               const int32_t* seq, const int32_t* wh, const int32_t* lengths, float* acc, float* eao,
                               void* stream);
 
+/* sm_vot_trajectory_overlap for a mask-mode record: a location entry's vertices are the 8 values poly[(f * S + s) * 8]
+ * (device f64 [>= T][S][8], tools/test.py's rotated box), each read back through rint((double)(float)v * 1e4) / 1e4 and
+ * stored as a float, as load_tracker reads an 8-value line; rec supplies the entry codes only.  Everything else, the
+ * outputs and the preconditions are those of sm_vot_trajectory_overlap. */
+int sm_vot_trajectory_overlap_poly(const double* rec, const double* poly, int32_t T, int32_t S, const float* gt,
+                                   int32_t gt_frames, const int32_t* seq, const int32_t* wh, const int32_t* lengths,
+                                   float* acc, float* eao, void* stream);
+
 /* Bytes of device workspace sm_vot_eao_accumulate needs for T frames and S streams (0 for bad sizes). */
 size_t sm_vot_eao_workspace_size(int32_t T, int32_t S);
 
@@ -313,6 +321,35 @@ int sm_tracker_update(int32_t B, double* state, const float* records, const doub
 int sm_tracker_update_hp(int32_t B, double* state, const float* records, const double* aux, const int32_t* im_wh,
                          const sm_tracker_hp* hp, const double* hp_table, int32_t anchor_num, int32_t score_size,
                          double* maps, double* out, void* stream);
+
+/* sm_tracker_update_hp that also writes unclamped (device f64 [B][4], may be NULL): target_pos and target_sz after the
+ * lr update and before the frame clamps (tools/test.py:299-303 build the mask-mode fallback rectangle from these). */
+int sm_tracker_update_hp_ex(int32_t B, double* state, const float* records, const double* aux, const int32_t* im_wh,
+                            const sm_tracker_hp* hp, const double* hp_table, int32_t anchor_num, int32_t score_size,
+                            double* maps, double* out, double* unclamped, void* stream);
+
+/* SiamMask's rotated box of tools/test.py:284-303 for N masks of different sizes, all pointers device pointers.
+ * masks: packed uint8 buffer of thresholded masks (0 background, anything else foreground; a torch bool tensor),
+ * mask b at masks + desc[b].offset, desc[b].h x desc[b].w bytes; total = the buffer's length; max_h / max_w bound
+ * every h / w (they size the launch).  fallback: f64 [N][4] = (cx, cy, w, h), target_pos and target_sz before the
+ * clamps (sm_tracker_update_hp_ex's unclamped).  Per mask:
+ *   components: the 8-connected components of the foreground, pixels outside the frame background;
+ *   area2: twice the area of each component's outer border as cv2.findContours(RETR_EXTERNAL, CHAIN_APPROX_NONE)
+ *     traces it (Suzuki & Abe's border following from the raster-first pixel), which cv2.contourArea halves;
+ *   selection: the largest area; on equal areas the component whose raster-first pixel is last in raster order
+ *     (cv2's contour order and np.argmax); used if its area is over 100 (area2 > 200);
+ *   poly f64 [N][8]: then the least-area rectangle over the edges of the component's convex hull (Andrew's monotone
+ *     chain over the row extremes sorted by (y, x), collinear points dropped; areas compared exactly in integers, the
+ *     first edge on ties), vertices p + (a e + b n) / |e|^2 in float64 rounded to float32, in cv2.boxPoints' order
+ *     (cv2 4.x, angle in [-90, 0)); otherwise cxy_wh_2_rect(fallback) as (x0,y0), (x0+w,y0), (x0+w,y0+h), (x0,y0+h);
+ *   flag int32 [N]: 1 contour, 0 fallback; area2 int64 [N]: twice the largest contour area (0 without foreground).
+ * The polygon is a deterministic float64 rule; cv2's own minAreaRect may pick another edge on near-ties.
+ * workspace: device memory of sm_rotated_box_workspace_size(total, N, max_h) bytes, 16-byte aligned.
+ * Preconditions: h, w <= max_h, max_w <= 32767; N <= 65535.  Equal inputs give equal bits. */
+size_t sm_rotated_box_workspace_size(int64_t total, int32_t N, int32_t max_h);
+int sm_rotated_box_ragged(const uint8_t* masks, const sm_image_desc* desc, int32_t N, int32_t max_h, int32_t max_w,
+                          int64_t total, const double* fallback, void* workspace, size_t workspace_bytes, double* poly,
+                          int32_t* flag, int64_t* area2, void* stream);
 
 /* One whole frame of siamese_track (tools/test.py:201-261) on the device, all pointers device pointers:
  * sm_track(flags) -> sm_select -> sm_refine at the position sm_select chose (refine_out != NULL needs

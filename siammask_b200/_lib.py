@@ -75,6 +75,14 @@ SIGNATURES = {
     "sm_tracker_update_hp": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.POINTER(SmTrackerHp), C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
                                        C.c_void_p, C.c_void_p]),
+    "sm_tracker_update_hp_ex": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.POINTER(SmTrackerHp), C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sm_rotated_box_workspace_size": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32]),
+    "sm_rotated_box_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] +
+                              [C.c_void_p] * 2 + [C.c_size_t] + [C.c_void_p] * 4),
+    "sm_vot_trajectory_overlap_poly": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32] +
+                                       [C.c_void_p] * 6),
     "sm_mask_iou": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 3 + [C.c_int32] * 3 +
                     [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "sm_crop_resize_indexed": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,

@@ -9,7 +9,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsiammask_b200.so")
-SOURCES = ["conv_gemm_sm90.cu", "conv3x3_patch_sm90.cu", "stem_sm90.cu", "simt_kernels.cu", "xcorr_bulk.cu", "engine.cu"]
+SOURCES = ["conv_gemm_sm90.cu", "conv3x3_patch_sm90.cu", "stem_sm90.cu", "simt_kernels.cu", "xcorr_bulk.cu", "rbox_sm90.cu",
+           "engine.cu"]
 HEADERS = ["common.cuh", "ptx.cuh", os.path.join("..", "..", "include", "siammask_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]

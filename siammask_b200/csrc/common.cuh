@@ -177,9 +177,17 @@ void launch_vot_overlap(const float* poly_a, const float* poly_b, int B, int W, 
                         const int32_t* wh = nullptr);
 // sm_vot_trajectory_overlap / sm_vot_eao_accumulate (include/siammask_b200.h); the workspace of the latter holds
 // vot_eao_workspace_size(T, S) bytes, 8-byte aligned
+// (with poly, f64 [T][S][8], a location's 8 polygon values are read from there instead of rec's x, y, w, h)
 void launch_vot_trajectory_overlap(const double* rec, int T, int S, const float* gt, int gt_frames, const int32_t* seq,
-                                   const int32_t* wh, const int32_t* lengths, float* acc, float* eao, cudaStream_t st);
+                                   const int32_t* wh, const int32_t* lengths, float* acc, float* eao, cudaStream_t st,
+                                   const double* poly = nullptr);
 size_t vot_eao_workspace_size(int T, int S);
+// sm_rotated_box_ragged (include/siammask_b200.h, rbox_sm90.cu); the workspace holds rotated_box_workspace_size bytes,
+// 16-byte aligned
+size_t rotated_box_workspace_size(int64_t total, int N, int max_h);
+void launch_rotated_box(const uint8_t* masks, const sm_image_desc* desc, int N, int max_h, int max_w,
+                        const double* fallback, void* workspace, double* poly, int32_t* flag, int64_t* area2,
+                        int64_t total, cudaStream_t st);
 void launch_vot_eao_accumulate(const float* eao, const float* acc, const double* rec, int T, int S,
                                const int32_t* lengths, const int32_t* combo, int R, int cap, int tail_from,
                                const double* tail_in, double* tail_out, double* num, double* den, double* stats,
@@ -208,7 +216,7 @@ void launch_tracker_prepare(int B, const double* state, const int32_t* avg, cons
 // hp_table (optional): device f64 [B][3] = (penalty_k, window_influence, lr) per stream, replacing hp.penalty_k / hp.lr
 void launch_tracker_update(int B, double* state, const float* rec, const double* aux, const int32_t* imsize,
                            const TrackerHp& hp, int A, int R, double* maps, double* out, cudaStream_t st,
-                           const double* hp_table = nullptr);
+                           const double* hp_table = nullptr, double* unclamped = nullptr);
 // frame_idx == nullptr: stream b crops frames + b * frame_stride; else frames + frame_idx[b] * frame_stride, or, with
 // desc (sm_crop_resize_ragged), the frame desc[frame_idx[b]] (frame_stride, H and W are then unused)
 void launch_crop_resize(const uint8_t* frames, size_t frame_stride, int H, int W, const int32_t* box, int B, int model,

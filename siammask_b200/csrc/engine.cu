@@ -2191,6 +2191,41 @@ int sm_vot_trajectory_overlap(const double* rec, int32_t T, int32_t S, const flo
   SM_API_END
 }
 
+int sm_vot_trajectory_overlap_poly(const double* rec, const double* poly, int32_t T, int32_t S, const float* gt,
+                                   int32_t gt_frames, const int32_t* seq, const int32_t* wh, const int32_t* lengths,
+                                   float* acc, float* eao, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(T >= 1 && S >= 1 && gt_frames >= T, "bad argument");
+  SMK_CHECK(2 * (int64_t)T * S <= INT32_MAX, "2 * T * S must fit in int32 (two blocks per frame and stream)");
+  SMK_CHECK(rec && poly && gt && seq && wh && lengths && acc && eao, "null argument");
+  require_device();
+  smk::launch_vot_trajectory_overlap(rec, T, S, gt, gt_frames, seq, wh, lengths, acc, eao,
+                                     static_cast<cudaStream_t>(stream), poly);
+  SM_API_END
+}
+
+size_t sm_rotated_box_workspace_size(int64_t total, int32_t N, int32_t max_h) {
+  return total >= 0 && N >= 1 && max_h >= 1 ? smk::rotated_box_workspace_size(total, N, max_h) : 0;
+}
+
+int sm_rotated_box_ragged(const uint8_t* masks, const sm_image_desc* desc, int32_t N, int32_t max_h, int32_t max_w,
+                          int64_t total, const double* fallback, void* workspace, size_t workspace_bytes, double* poly,
+                          int32_t* flag, int64_t* area2, void* stream) {
+  SM_API_BEGIN
+  SMK_CHECK(N >= 0 && N <= 65535 && total >= 0, "bad argument: 0 <= N <= 65535, total >= 0");
+  SMK_CHECK(max_h >= 1 && max_w >= 1 && max_h <= 32767 && max_w <= 32767,
+            "bad argument: 1 <= max_h, max_w <= 32767");
+  if (N == 0) return 0;
+  SMK_CHECK(masks && desc && fallback && workspace && poly && flag && area2, "null argument");
+  SMK_CHECK(workspace_bytes >= smk::rotated_box_workspace_size(total, N, max_h) &&
+                reinterpret_cast<uintptr_t>(workspace) % 16 == 0,
+            "workspace too small or not 16-byte aligned (sm_rotated_box_workspace_size)");
+  require_device();
+  smk::launch_rotated_box(masks, desc, N, max_h, max_w, fallback, workspace, poly, flag, area2, total,
+                          static_cast<cudaStream_t>(stream));
+  SM_API_END
+}
+
 size_t sm_vot_eao_workspace_size(int32_t T, int32_t S) {
   return T >= 1 && S >= 1 ? smk::vot_eao_workspace_size(T, S) : 0;
 }
@@ -2334,15 +2369,22 @@ int sm_tracker_update(int32_t B, double* state, const float* records, const doub
   SM_API_END
 }
 
-int sm_tracker_update_hp(int32_t B, double* state, const float* records, const double* aux, const int32_t* im_wh,
-                         const sm_tracker_hp* hp, const double* hp_table, int32_t anchor_num, int32_t score_size,
-                         double* maps, double* out, void* stream) {
+int sm_tracker_update_hp_ex(int32_t B, double* state, const float* records, const double* aux, const int32_t* im_wh,
+                            const sm_tracker_hp* hp, const double* hp_table, int32_t anchor_num, int32_t score_size,
+                            double* maps, double* out, double* unclamped, void* stream) {
   SM_API_BEGIN
   SMK_CHECK(state && records && aux && im_wh && hp && hp_table && B >= 1 && score_size >= 1, "bad argument");
   require_device();
   smk::launch_tracker_update(B, state, records, aux, im_wh, to_hp(hp), anchor_num, score_size, maps, out,
-                             static_cast<cudaStream_t>(stream), hp_table);
+                             static_cast<cudaStream_t>(stream), hp_table, unclamped);
   SM_API_END
+}
+
+int sm_tracker_update_hp(int32_t B, double* state, const float* records, const double* aux, const int32_t* im_wh,
+                         const sm_tracker_hp* hp, const double* hp_table, int32_t anchor_num, int32_t score_size,
+                         double* maps, double* out, void* stream) {
+  return sm_tracker_update_hp_ex(B, state, records, aux, im_wh, hp, hp_table, anchor_num, score_size, maps, out,
+                                 nullptr, stream);
 }
 
 int sm_select(sm_engine* e, int32_t B, const float* cls, const float* loc, const float* anchors, const double* window,

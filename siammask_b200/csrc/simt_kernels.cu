@@ -1510,7 +1510,7 @@ __device__ __forceinline__ double vot_result_value(double v) {
 __global__ void __launch_bounds__(VO_THREADS) vot_trajectory_overlap_kernel(
     const double* __restrict__ rec, int S, const float* __restrict__ gt, int gt_frames, const int32_t* __restrict__ seq,
     const int32_t* __restrict__ wh, const int32_t* __restrict__ lengths, float* __restrict__ acc,
-    float* __restrict__ eao) {
+    float* __restrict__ eao, const double* __restrict__ poly) {
   __shared__ float s_pred[8];
   const int eao_pass = blockIdx.x & 1;                   // block 2q computes acc[q], block 2q + 1 eao[q]
   const unsigned q = blockIdx.x >> 1;
@@ -1525,7 +1525,9 @@ __global__ void __launch_bounds__(VO_THREADS) vot_trajectory_overlap_kernel(
     if (threadIdx.x == 0) out[o] = entry_nan();
     return;
   }
-  if (threadIdx.x == 0) {
+  if (threadIdx.x == 0 && poly != nullptr) {              // a polygon entry: its 8 values read back one by one
+    for (int i = 0; i < 8; ++i) s_pred[i] = (float)vot_result_value(poly[8 * o + i]);
+  } else if (threadIdx.x == 0) {
     const double x = vot_result_value(r[1]), y = vot_result_value(r[2]);
     const double x1 = __dadd_rn(x, vot_result_value(r[3])), y1 = __dadd_rn(y, vot_result_value(r[4]));
     s_pred[0] = (float)x;  s_pred[1] = (float)y;  s_pred[2] = (float)x1; s_pred[3] = (float)y;
@@ -1737,7 +1739,7 @@ __global__ void tracker_prepare_kernel(int B, const double* __restrict__ state, 
 __global__ void tracker_update_kernel(int B, double* __restrict__ state, const float* __restrict__ rec,
                                       const double* __restrict__ aux, const int32_t* __restrict__ imsize, TrackerHp hp,
                                       int A, int R, double* __restrict__ maps, double* __restrict__ out,
-                                      const double* __restrict__ hp_table) {
+                                      const double* __restrict__ hp_table, double* __restrict__ unclamped) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   // per-stream (penalty_k, window_influence, lr) rows replace the struct's penalty_k and lr (sm_tracker_update_hp)
@@ -1782,6 +1784,10 @@ __global__ void tracker_update_kernel(int B, double* __restrict__ state, const f
     m[3] = 0.0; m[4] = bq; m[5] = -bq * bb1;
   }
   (void)A;
+  if (unclamped != nullptr) {                                   // target_pos / target_sz before the clamps (:299-303)
+    double* u = unclamped + 4 * b;
+    u[0] = res_x; u[1] = res_y; u[2] = res_w; u[3] = res_h;
+  }
   res_x = fmax(0.0, fmin(im_w, res_x));                         // :305-308
   res_y = fmax(0.0, fmin(im_h, res_y));
   res_w = fmax(10.0, fmin(im_w, res_w));
@@ -2043,8 +2049,9 @@ void launch_tracker_prepare(int B, const double* state, const int32_t* avg, cons
 
 void launch_tracker_update(int B, double* state, const float* rec, const double* aux, const int32_t* imsize,
                            const TrackerHp& hp, int A, int R, double* maps, double* out, cudaStream_t st,
-                           const double* hp_table) {
-  tracker_update_kernel<<<(B + 127) / 128, 128, 0, st>>>(B, state, rec, aux, imsize, hp, A, R, maps, out, hp_table);
+                           const double* hp_table, double* unclamped) {
+  tracker_update_kernel<<<(B + 127) / 128, 128, 0, st>>>(B, state, rec, aux, imsize, hp, A, R, maps, out, hp_table,
+                                                         unclamped);
   SMK_CUDA(cudaGetLastError());
 }
 
@@ -2106,9 +2113,10 @@ void launch_vot_overlap(const float* poly_a, const float* poly_b, int B, int W, 
 }
 
 void launch_vot_trajectory_overlap(const double* rec, int T, int S, const float* gt, int gt_frames, const int32_t* seq,
-                                   const int32_t* wh, const int32_t* lengths, float* acc, float* eao, cudaStream_t st) {
+                                   const int32_t* wh, const int32_t* lengths, float* acc, float* eao, cudaStream_t st,
+                                   const double* poly) {
   vot_trajectory_overlap_kernel<<<2u * (unsigned)T * (unsigned)S, VO_THREADS, 0, st>>>(rec, S, gt, gt_frames, seq, wh,
-                                                                                  lengths, acc, eao);
+                                                                                  lengths, acc, eao, poly);
   SMK_CUDA(cudaGetLastError());
 }
 

@@ -525,19 +525,26 @@ def _vot_overlap_sized(poly_a, poly_b, wh, out=None) -> torch.Tensor:
     return out
 
 
-def _vot_trajectory_overlap(rec, T: int, S: int, gt, seq, wh, lengths):
+def _vot_trajectory_overlap(rec, T: int, S: int, gt, seq, wh, lengths, poly=None):
     """C ABI `sm_vot_trajectory_overlap` without host-side checks: rec float64 CUDA [>= T, S, 5] (a `VotRunner` record),
     gt float32 CUDA [G, >= T, 8], seq / lengths int32 CUDA [S], wh int32 CUDA [S, 2] = (W, H), all inside the
     precondition.  Returns (acc, eao) float32 [T, S]: pysot's per-frame overlaps with bounds (W, H) and burn-in 10, and
-    with bounds (W-1, H-1)."""
+    with bounds (W-1, H-1).  With poly float64 CUDA [>= T, S, 8] (a mask-mode record's polygons), a location entry is
+    that polygon (`sm_vot_trajectory_overlap_poly`) and rec supplies the entry codes only."""
     lib = _lib.load()
     dev = rec.device
     acc = torch.empty(T, S, dtype=torch.float32, device=dev)
     eao = torch.empty(T, S, dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
-        _lib.check(lib.sm_vot_trajectory_overlap(rec.data_ptr(), T, S, gt.data_ptr(), int(gt.shape[1]), seq.data_ptr(),
-                                                 wh.data_ptr(), lengths.data_ptr(), acc.data_ptr(), eao.data_ptr(),
-                                                 _stream(dev)))
+        if poly is None:
+            _lib.check(lib.sm_vot_trajectory_overlap(rec.data_ptr(), T, S, gt.data_ptr(), int(gt.shape[1]),
+                                                     seq.data_ptr(), wh.data_ptr(), lengths.data_ptr(), acc.data_ptr(),
+                                                     eao.data_ptr(), _stream(dev)))
+        else:
+            _lib.check(lib.sm_vot_trajectory_overlap_poly(rec.data_ptr(), poly.data_ptr(), T, S, gt.data_ptr(),
+                                                          int(gt.shape[1]), seq.data_ptr(), wh.data_ptr(),
+                                                          lengths.data_ptr(), acc.data_ptr(), eao.data_ptr(),
+                                                          _stream(dev)))
     return acc, eao
 
 
@@ -556,3 +563,63 @@ def _vot_eao_accumulate(eao, acc, rec, lengths, combo, tail_from, tail_in, tail_
                                              combo.data_ptr(), R, cap, int(tail_from), tail_in.data_ptr(),
                                              tail_out.data_ptr(), num.data_ptr(), den.data_ptr(), stats.data_ptr(),
                                              ws.data_ptr(), ws.numel() * 8, _stream(dev)))
+
+
+RBOX_MAX_SIDE = 32767             # frame side bound of sm_rotated_box_ragged
+
+
+def rotated_box(masks, fallback_cxcywh):
+    """SiamMask's rotated box (tools/test.py:284-303, C ABI `sm_rotated_box_ragged`) for N thresholded masks: the
+    minimum-area rectangle of the largest outer contour if its area is over 100, else the rectangle of the fallback
+    state.  masks: a bool (or uint8, nonzero = foreground) CUDA tensor [N,H,W], or a list of N CUDA tensors [H_i,W_i]
+    (as `BatchTracker.track(mask=True, paste=True)` returns them); fallback_cxcywh: float64 [N,4] = target_pos,
+    target_sz before the clamps (host or device).  Returns (poly float64 [N,8] in cv2.boxPoints' vertex order, or the
+    fallback's 4 corners; flag int32 [N], 1 contour / 0 fallback; area2 int64 [N], twice the largest contour area),
+    all on the masks' device, without a host sync.  Contour areas, selection and fallback equal cv2's exactly; the
+    rectangle is a deterministic float64 rule (include/siammask_b200.h) that may differ from cv2's minAreaRect where
+    two orientations give nearly equal areas."""
+    if torch.is_tensor(masks):
+        if masks.dim() != 3:
+            raise ValueError(f"masks must be [N,H,W] or a list of [H,W] tensors, got {tuple(masks.shape)}")
+        masks = list(masks.unbind(0))
+    if not isinstance(masks, (list, tuple)):
+        raise ValueError("masks must be a CUDA tensor [N,H,W] or a list of CUDA tensors [H,W]")
+    N = len(masks)
+    for i, m in enumerate(masks):
+        if not (torch.is_tensor(m) and m.is_cuda and m.dim() == 2 and m.dtype in (torch.bool, torch.uint8)):
+            raise ValueError(f"masks[{i}] must be a bool or uint8 CUDA tensor [H,W]")
+        if not 1 <= min(m.shape) or max(m.shape) > RBOX_MAX_SIDE:
+            raise ValueError(f"masks[{i}]: sides must lie in [1, {RBOX_MAX_SIDE}], got {tuple(m.shape)}")
+    if not 1 <= N <= 65535:
+        raise ValueError(f"1 <= N <= 65535 masks expected, got {N}")
+    dev = masks[0].device
+    if any(m.device != dev for m in masks):
+        raise ValueError("masks must all be on one device")
+    fb = fallback_cxcywh if torch.is_tensor(fallback_cxcywh) else torch.as_tensor(np.asarray(fallback_cxcywh,
+                                                                                                np.float64))
+    if tuple(fb.shape) != (N, 4):
+        raise ValueError(f"fallback_cxcywh must be [{N}, 4] (cx, cy, w, h), got {tuple(fb.shape)}")
+    from .tracker import FramePacker
+    packed = FramePacker(dev).pack([m.to(torch.uint8) if m.dtype != torch.uint8 else m for m in masks], 1)
+    hs, ws = zip(*packed.shapes)
+    return _rotated_box(packed.data, packed.desc, N, (max(hs), max(ws)), fb.to(dev, torch.float64))
+
+
+def _rotated_box(data, desc, N: int, max_hw, fallback):
+    """`rotated_box` without host-side checks: data the packed mask buffer (bool or uint8, CUDA), desc its device
+    sm_image_desc table of N masks, max_hw bounds of their sides, fallback float64 CUDA [N,4].  The workspace comes
+    from torch's caching allocator."""
+    lib = _lib.load()
+    dev = data.device
+    total = int(data.numel())
+    nbytes = int(lib.sm_rotated_box_workspace_size(total, N, int(max_hw[0])))
+    ws = torch.empty((nbytes + 15) // 16 * 2, dtype=torch.float64, device=dev)
+    poly = torch.empty(N, 8, dtype=torch.float64, device=dev)
+    flag = torch.empty(N, dtype=torch.int32, device=dev)
+    area2 = torch.empty(N, dtype=torch.int64, device=dev)
+    fallback = fallback.contiguous()
+    with torch.cuda.device(dev):
+        _lib.check(lib.sm_rotated_box_ragged(data.data_ptr(), desc.data_ptr(), N, int(max_hw[0]), int(max_hw[1]), total,
+                                             fallback.data_ptr(), ws.data_ptr(), ws.numel() * 8, poly.data_ptr(),
+                                             flag.data_ptr(), area2.data_ptr(), _stream(dev)))
+    return poly, flag, area2

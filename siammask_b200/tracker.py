@@ -12,7 +12,8 @@ mask paste-back — runs here as a fixed sequence of kernels over all streams (C
     sm_warp_affine_ragged   127x127 sigmoid mask -> frame, threshold                      (:263-284)
 
 The state (target_pos, target_sz, float64) lives on the device; a frame costs one small D2H copy only if the caller
-asks for the numbers (`TrackResult.cpu()`).  Contour extraction / minAreaRect (:285-303) is not part of this module.
+asks for the numbers (`TrackResult.cpu()`).  The rotated box of the pasted masks (contours + minAreaRect, :285-303) is
+`ops.rotated_box`, which `VotRunner(mask=True)` runs on every frame's packed masks.
 
 Streams join and leave a running tracker: `add` templates new streams into free engine slots, `remove` frees them.  The
 active streams are kept as compact rows (state, slot, frame index, hyper-parameters), and every frame runs exactly those
@@ -191,7 +192,10 @@ class TrackResult:
     [N,8] = x, y, w, h (new target_pos / target_sz), score, penalty, lr (from the stream's own lr), best index; mask:
     bool [N,H,W] frame-sized masks (or None), or, when the streams' frames differ in size, a list of N bool [H_i,W_i]
     views of one packed buffer in row order.  With mask=True, extras also holds "mask_prob" f32 [N,side,side] (sigmoid
-    masks) and "maps" f64 [N,6] (their paste-back maps, overwritten by the next frame)."""
+    masks), "maps" f64 [N,6] (their paste-back maps, overwritten by the next frame) and "unclamped" f64 [N,4]
+    (target_pos, target_sz before the frame clamps: the mask-mode fallback of tools/test.py:299-303); with paste=True
+    also "packed_mask" = (flat bool buffer, device sm_image_desc table, (max h, max w)) of the pasted masks, which
+    `ops._rotated_box` reads in place."""
     state: torch.Tensor
     mask: torch.Tensor | list | None = None
     extras: dict = field(default_factory=dict)
@@ -506,10 +510,12 @@ class BatchTracker:
                                  refine=use_refine, mask_head=use_head, mask_col=use_head, slots=self._slots_dev,
                                  hp=self._hp_dev)
             res = torch.empty(N, 8, dtype=torch.float64, device=self.dev)
-            _lib.check(self.lib.sm_tracker_update_hp(N, self.state.data_ptr(), out["records"].data_ptr(),
-                                                     self.aux.data_ptr(), self.imsize.data_ptr(), C.byref(self.hp),
-                                                     self._hp_dev.data_ptr(), self.net.anchor_num, p.score_size,
-                                                     self.maps.data_ptr() if mask else None, res.data_ptr(), st))
+            unclamped = torch.empty(N, 4, dtype=torch.float64, device=self.dev) if mask else None
+            _lib.check(self.lib.sm_tracker_update_hp_ex(N, self.state.data_ptr(), out["records"].data_ptr(),
+                                                        self.aux.data_ptr(), self.imsize.data_ptr(), C.byref(self.hp),
+                                                        self._hp_dev.data_ptr(), self.net.anchor_num, p.score_size,
+                                                        self.maps.data_ptr() if mask else None, res.data_ptr(),
+                                                        unclamped.data_ptr() if mask else None, st))
             extras = {"records": out["records"], "pos": out["pos"], "x_crop": x, "ids": list(self._ids)}
             mask_out = None
             if mask:
@@ -518,7 +524,7 @@ class BatchTracker:
                 if side != p.out_size:
                     raise ValueError(f"out_size {p.out_size} does not match the mask source ({side})")
                 m = logits.sigmoid().view(N, side, side).contiguous()
-                extras["mask_prob"], extras["maps"] = m, self.maps
+                extras["mask_prob"], extras["maps"], extras["unclamped"] = m, self.maps, unclamped
                 if paste:                                   # every row's mask in one packed buffer
                     if self._mask_table is None:
                         desc, table = self.packer.table(self._size, 1)
@@ -526,6 +532,7 @@ class BatchTracker:
                         self._mask_table = desc, table, int(table["offset"][-1]) + hs[-1] * ws[-1], (max(hs), max(ws))
                     desc, table, total, max_hw = self._mask_table
                     flat = ops._warp_affine_ragged(m, self.maps, desc, max_hw, total) > p.seg_thr
+                    extras["packed_mask"] = (flat, desc, max_hw)
                     if len(set(self._size)) == 1:                  # one frame size: rows back to back, [N,H,W]
                         mask_out = flat.view(N, *max_hw)
                     else:

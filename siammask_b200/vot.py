@@ -39,7 +39,14 @@ every hyper-parameter combination at once, from the runner's device record and w
        cuts at each failure.  A column's sums depend only on its index, so runs of any split of the dataset (by
        sequence or by combination) add up; the curve is read out up to the longest sequence added.
 
-Mask-mode VOT (the rotated box of tools/test.py:284-303), per-attribute EAO tags and the OTB branch are not here.
+Mask mode (`VotRunner(mask=True)`, tools/test.py's --mask, as SiamMask reports its VOT results): step 1 also computes
+each stream's (refined) mask and pastes it into the frame, and `ops._rotated_box` turns the packed masks into the
+rotated box of tools/test.py:284-303 (the largest contour's minimum-area rectangle, or the rectangle of the state before
+its clamps) on the device.  That polygon is scored in step 2 and recorded as the location.  The polygons live in a
+second device plane beside the entry codes, so the record rows, the failure schedule and everything that reads the
+codes are the same in both modes; `result()`, `write_result` and `VotScore` give 8-value locations.
+
+Per-attribute EAO tags and the OTB branch are not here.
 """
 from __future__ import annotations
 
@@ -90,12 +97,16 @@ def check_gt(gt) -> list[np.ndarray]:
     return out
 
 
-def regions_from_record(rec: np.ndarray, T: int) -> list:
-    """One stream's regions in the reference's form from its rows rec float64 [>=T, 5] = (code, location[4])."""
+def regions_from_record(rec: np.ndarray, T: int, poly: np.ndarray | None = None) -> list:
+    """One stream's regions in the reference's form from its rows rec float64 [>=T, 5] = (code, location[4]); with
+    poly float64 [>=T, 8] (mask mode) a location is the frame's 8 polygon values instead."""
     regions = []
     for f in range(T):
         c = int(rec[f, 0])
-        regions.append(rec[f, 1:5].copy() if c == CODE_LOCATION else c)
+        if c != CODE_LOCATION:
+            regions.append(c)
+        else:
+            regions.append(rec[f, 1:5].copy() if poly is None else poly[f].copy())
     return regions
 
 
@@ -118,9 +129,23 @@ class VotRunner:
     window_influence, lr) rows (tune_vot's grid is `tune.grid(DEFAULT_PENALTY_K, DEFAULT_WINDOW_INFLUENCE,
     DEFAULT_LR)`, in its nested-loop order) each sequence runs every combination, and stream (g, k) is row g*K + k of
     every output, as in `ParamSweep`.  `net` is a `siammask_b200.Custom` (with or without the mask branch) whose
-    max_batch and num_slots cover G*K streams."""
+    max_batch and num_slots cover G*K streams.
 
-    def __init__(self, net, params: TrackerParams | None = None, combos=None):
+    mask=True runs tools/test.py's mask mode: each frame's location is the rotated box of the pasted mask
+    (`ops.rotated_box`), an 8-value polygon.  refine=True takes the mask from the refine module (siammask_sharp,
+    out_size 127), refine=False from the 63x63 mask-head column (siammask_base, out_size 63); with params=None the
+    tracker's out_size follows.  mask=True needs an engine with the mask branch."""
+
+    def __init__(self, net, params: TrackerParams | None = None, combos=None, mask: bool = False, refine: bool = True):
+        self.mask, self.refine = bool(mask), bool(refine)
+        if self.mask:
+            if not getattr(net, "with_mask", False):
+                raise ValueError("mask=True needs an engine with the mask branch (Custom(mask=True))")
+            side = 127 if self.refine else 63
+            if params is None:
+                params = TrackerParams(instance_size=net.search_size, out_size=side)
+            elif params.out_size != side:
+                raise ValueError(f"refine={self.refine} gives {side}x{side} masks; params.out_size is {params.out_size}")
         self.tracker = BatchTracker(net, params)
         self.p = self.tracker.p
         self.dev = self.tracker.dev
@@ -195,6 +220,7 @@ class VotRunner:
         # rows [0, Tmax) of stream s: (entry code, location x, y, w, h); row Tmax: (lost_times, 0, 0, 0, 0)
         self._rec = torch.zeros(Tmax + 1, S, 5, dtype=torch.float64, device=self.dev)
         self._rec[0, :, 0] = CODE_INIT
+        self._poly = torch.zeros(Tmax, S, 8, dtype=torch.float64, device=self.dev) if self.mask else None
         self._start = torch.zeros(S, dtype=torch.int32, device=self.dev)
         self._flags = torch.zeros(S, dtype=torch.uint8, device=self.dev)
         self._pinned = [torch.zeros(S, dtype=torch.uint8).pin_memory() for _ in range(SKIP_FRAMES + 1)]
@@ -242,14 +268,8 @@ class VotRunner:
             raise ValueError(f"frames must be [{self.G},H,W,3]")
         rows = self._row_dev
         # 1. track every active stream (skipped ones too: their outputs are discarded below)
-        r = self.tracker.track(fr, mask=False)
-        st = r.state
-        # 2. overlap of the gt polygon with the rectangle of the clamped state: float64 vertices, stored as C floats
-        x0 = st[:, 0] - st[:, 2] / 2
-        y0 = st[:, 1] - st[:, 3] / 2
-        x1, y1 = x0 + st[:, 2], y0 + st[:, 3]
-        loc = torch.stack([x0, y0, st[:, 2], st[:, 3]], 1)
-        pred = torch.stack([x0, y0, x1, y0, x1, y1, x0, y1], 1).float()
+        # 2. overlap of the gt polygon with the predicted polygon, stored as C floats
+        r, loc, pred = self._predict(fr)
         ov = ops._vot_overlap_sized(self._gt[self._row_video, f], pred, self._row_wh)
         # 3. bookkeeping on the device: init / track / skip by the stream's start frame; only an overlap of exactly 0
         #    is a failure (NaN is truthy)
@@ -258,7 +278,7 @@ class VotRunner:
         lost = tracking & (ov == 0)
         code = torch.where(start == f, CODE_INIT, torch.where(lost, CODE_LOST, CODE_LOCATION * tracking.long()))
         self._rec[f, rows, 0] = code.double()
-        self._rec[f, rows, 1:5] = torch.where(tracking & ~lost, 1, 0).unsqueeze(1) * loc
+        self._locations()[f * self._rec.shape[1] + rows] = torch.where(tracking & ~lost, 1, 0).unsqueeze(1) * loc
         self._rec[-1, rows, 0] += lost.double()
         self._start[rows] = torch.where(lost, f + SKIP_FRAMES, start)
         self._flags.zero_()
@@ -284,16 +304,19 @@ class VotRunner:
         return r
 
     def result(self):
-        """One D2H copy.  Returns (regions, lost_times): regions[g][k] is stream (g, k)'s list in the reference's form
-        (1 init, 2 lost, 0 skipped, or a float64 [4] location x, y, w, h) over the frames tracked so far; lost_times
-        int [G, K]."""
+        """One D2H copy (two in mask mode).  Returns (regions, lost_times): regions[g][k] is stream (g, k)'s list in the
+        reference's form (1 init, 2 lost, 0 skipped, or a float64 location: [4] x, y, w, h, or in mask mode [8] the
+        rotated box's vertices) over the frames tracked so far; lost_times int [G, K]."""
         rec = self._rec.cpu().numpy()
+        poly = self._poly.cpu().numpy() if self.mask else None
         G, K = self.G, self.K
         if self._sched is None:
             n = np.repeat(np.minimum(self.T, self.f), K)
         else:                                           # frames 0 .. f - admission step - 1 of each admitted stream
             n = np.where(self._admit >= 0, np.minimum(self._video_T, self.f - self._admit), 0)
-        regions = [[regions_from_record(rec[:, g * K + k], int(n[g * K + k])) for k in range(K)] for g in range(G)]
+        regions = [[regions_from_record(rec[:, g * K + k], int(n[g * K + k]),
+                                        None if poly is None else poly[:, g * K + k]) for k in range(K)]
+                   for g in range(G)]
         return regions, rec[-1, :, 0].astype(np.int64).reshape(G, K)
 
     # ------------------------------------------------------------------ queue mode
@@ -328,6 +351,7 @@ class VotRunner:
         self._stream_of, self._id_of = {}, [None] * S
         self._rec = torch.zeros(Tmax + 1, S, 5, dtype=torch.float64, device=self.dev)
         self._rec[0, :, 0] = CODE_INIT
+        self._poly = torch.zeros(Tmax, S, 8, dtype=torch.float64, device=self.dev) if self.mask else None
         self._start = torch.zeros(S, dtype=torch.int32, device=self.dev)         # in the stream's own frames
         self._flags = torch.zeros(S, dtype=torch.uint8, device=self.dev)
         self._pinned = [torch.zeros(S, dtype=torch.uint8).pin_memory() for _ in range(SKIP_FRAMES + 1)]
@@ -392,18 +416,35 @@ class VotRunner:
         self._plan = self._sched.step() if not self._sched.done else None
         return r
 
-    def _track(self, fr, f: int):
-        """Steps 1-4 of `frame` for the running streams of a queue step f: each row at its own frame t = f - admission
-        step, its record row t and its gt row t."""
-        rows = self._row_dev
-        S, Tmax = self._rec.shape[1], self._gt.shape[1]
+    def _predict(self, fr):
+        """Step 1 for every active row: (TrackResult, location float64 [n, 4 or 8] as the record keeps it, predicted
+        polygon float32 [n, 8]).  Box mode: the rectangle of the clamped state, float64 vertices.  Mask mode: the
+        rotated box of each row's pasted mask; the TrackResult's extras["rbox"] holds (polygon, flag, area2)."""
+        if self.mask:
+            r = self.tracker.track(fr, mask=True, refine=self.refine, paste=True)
+            flat, desc, max_hw = r.extras["packed_mask"]
+            poly, flag, area2 = ops._rotated_box(flat, desc, self.tracker.N, max_hw, r.extras["unclamped"])
+            r.extras["rbox"] = (poly, flag, area2)
+            return r, poly, poly.float()
         r = self.tracker.track(fr, mask=False)
         st = r.state
         x0 = st[:, 0] - st[:, 2] / 2
         y0 = st[:, 1] - st[:, 3] / 2
         x1, y1 = x0 + st[:, 2], y0 + st[:, 3]
         loc = torch.stack([x0, y0, st[:, 2], st[:, 3]], 1)
-        pred = torch.stack([x0, y0, x1, y0, x1, y1, x0, y1], 1).float()
+        return r, loc, torch.stack([x0, y0, x1, y0, x1, y1, x0, y1], 1).float()
+
+    def _locations(self) -> torch.Tensor:
+        """The record's location columns as a [(Tmax) * S, 4 or 8] view, row f * S + s: rec[..., 1:5] in box mode,
+        the polygon plane in mask mode."""
+        return self._poly.view(-1, 8) if self.mask else self._rec.view(-1, 5)[:, 1:5]
+
+    def _track(self, fr, f: int):
+        """Steps 1-4 of `frame` for the running streams of a queue step f: each row at its own frame t = f - admission
+        step, its record row t and its gt row t."""
+        rows = self._row_dev
+        S, Tmax = self._rec.shape[1], self._gt.shape[1]
+        r, loc, pred = self._predict(fr)
         t = f - self._row_admit                          # each row's own frame, on the device
         ov = ops._vot_overlap_sized(self._gt.view(-1, 8)[self._row_video * Tmax + t], pred, self._row_wh)
         start = self._start[rows].long()
@@ -413,7 +454,7 @@ class VotRunner:
         rec = self._rec.view(-1, 5)
         at = t * S + rows
         rec[at, 0] = code.double()
-        rec[at, 1:5] = torch.where(tracking & ~lost, 1, 0).unsqueeze(1) * loc
+        self._locations()[at] = torch.where(tracking & ~lost, 1, 0).unsqueeze(1) * loc
         self._rec[-1, rows, 0] += lost.double()
         self._start[rows] = torch.where(lost, t + SKIP_FRAMES, start).int()
         self._flags.zero_()
@@ -495,14 +536,15 @@ class VotScore:
         if not runner.ended:
             raise ValueError(f"every sequence must have ended: frame {runner.f} of lengths {runner.T.tolist()}")
         sizes = [(int(h), int(w)) for h, w in runner._hw]
-        self._add(runner._rec, runner._gt, runner.T, sizes, runner.K, combo_index)
+        self._add(runner._rec, runner._gt, runner.T, sizes, runner.K, combo_index, runner._poly)
         return self
 
     @torch.no_grad()
     def add_regions(self, regions, gt, sizes, combo_index=None):
         """Adds trajectories in the form `VotRunner.result()` returns: regions[g][k] is the list of sequence g under
-        combination k (1 init, 2 lost, 0 skipped, or a location x, y, w, h), gt[g] its float64 [T_g, 8] polygons and
-        sizes[g] its frame (H, W).  Every list must have T_g entries."""
+        combination k (1 init, 2 lost, 0 skipped, or a location: x, y, w, h, or 8 polygon values as pysot reads an
+        8-value result line), gt[g] its float64 [T_g, 8] polygons and sizes[g] its frame (H, W).  Every list must have
+        T_g entries, and every location of one call the same number of values."""
         gts = check_gt(gt)
         G = len(gts)
         if len(regions) != G or len(sizes) != G or G == 0:
@@ -513,6 +555,12 @@ class VotScore:
         T = np.array([len(a) for a in gts])
         Tmax = int(T.max())
         rec = np.zeros((Tmax, G * K, 5))
+        sizes_seen = {np.asarray(x).size for r in regions for traj in r for x in traj
+                      if not isinstance(x, (int, np.integer))}
+        if len(sizes_seen) > 1 or not sizes_seen <= {4, 8}:
+            raise ValueError("every location must have 4 values (x, y, w, h) or every one 8 (a polygon)")
+        width = sizes_seen.pop() if sizes_seen else 4
+        poly = np.zeros((Tmax, G * K, 8)) if width == 8 else None
         for g in range(G):
             for k in range(K):
                 traj = regions[g][k]
@@ -525,20 +573,27 @@ class VotScore:
                         rec[f, g * K + k, 0] = x
                     else:
                         loc = np.asarray(x, np.float64).reshape(-1)
-                        if loc.size != 4 or not np.isfinite(loc).all():
-                            raise ValueError(f"regions[{g}][{k}][{f}]: a location is 4 finite values")
-                        rec[f, g * K + k] = (CODE_LOCATION, *loc)
+                        if not np.isfinite(loc).all():
+                            raise ValueError(f"regions[{g}][{k}][{f}]: a location is {width} finite values")
+                        if poly is None:
+                            rec[f, g * K + k] = (CODE_LOCATION, *loc)
+                        else:
+                            rec[f, g * K + k, 0] = CODE_LOCATION
+                            poly[f, g * K + k] = loc
         locs = rec[..., 1:]
         if (np.abs(locs[..., :2]) + np.abs(locs[..., 2:]) > ops.VOT_COORD_LIMIT / 2).any():
             raise ValueError("locations must lie within +-2^19 px")
+        if poly is not None and (np.abs(poly) > ops.VOT_COORD_LIMIT / 2).any():
+            raise ValueError("polygon locations must lie within +-2^19 px")
         polys = np.zeros((G, Tmax, 8), np.float32)
         for g, a in enumerate(gts):
             polys[g, :len(a)] = a
         self._add(torch.from_numpy(rec).to(self.dev), torch.from_numpy(polys).to(self.dev), T,
-                  [(int(h), int(w)) for h, w in sizes], K, combo_index)
+                  [(int(h), int(w)) for h, w in sizes], K, combo_index,
+                  None if poly is None else torch.from_numpy(poly).to(self.dev))
         return self
 
-    def _add(self, rec, gt, T, sizes, K, combo_index):
+    def _add(self, rec, gt, T, sizes, K, combo_index, poly=None):
         rows = self._rows(combo_index, K)
         G = len(T)
         wh = np.array([(w, h) for h, w in sizes], np.int64)
@@ -554,7 +609,7 @@ class VotScore:
         t = torch.from_numpy(table).to(self.dev)                       # one upload: seq, lengths, combo, (W, H)
         seq_d, len_d, combo_d, wh_d = t[:S], t[S:2 * S], t[2 * S:3 * S], t[3 * S:]
         with torch.cuda.device(self.dev):
-            acc, eao = ops._vot_trajectory_overlap(rec, Tmax, S, gt, seq_d, wh_d, len_d)
+            acc, eao = ops._vot_trajectory_overlap(rec, Tmax, S, gt, seq_d, wh_d, len_d, poly)
             old = self.cap
             if Tmax > old:                                             # grow: earlier fragments reach the new columns
                 num = torch.zeros(self.K, Tmax, dtype=torch.float64, device=self.dev)

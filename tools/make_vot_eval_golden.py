@@ -12,6 +12,13 @@ frame 1; failures in the last 5 frames (point dropped); a failure at exactly T-5
 failures; NaN overlaps from a degenerate gt in a sequence without and with failures; T below low, between low and high,
 above high; a 2x2 frame; locations on exact .xxxx5 ties and ones printed as -0.0000; three trackers; EAO with the
 VOT2018 and the VOT2019 bounds.
+
+    python tools/make_vot_eval_golden.py --poly
+
+writes tests/golden/vot_eval_poly.npz instead: the same sequences and entry codes, with every location an 8-value
+polygon (mask-mode track_vot's rotated box, which load_tracker reads back as a Polygon) made by `to_polygons`: rotated
+quads with exact .xxxx5 ties, values printed as -0.0000, negative coordinates and quads partly off the frame; the NaN
+frames of the degenerate gt keep a quad inside its pixel.  rec is then [K, G, T, 9] = (code, 8 values).
 """
 from __future__ import annotations
 
@@ -29,6 +36,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 OUT = os.path.join(ROOT, "tests", "golden", "vot_eval.npz")
+OUT_POLY = os.path.join(ROOT, "tests", "golden", "vot_eval_poly.npz")
 REF = os.environ.get("SIAMMASK_REFERENCE", "/root/reference")
 
 # (T, W, H, failure plan per tracker, degenerate gt frames)
@@ -97,6 +105,40 @@ def make_inputs(rng):
     return gts, sizes, regions
 
 
+def to_polygons(regions, sizes, rng):
+    """regions with every (x, y, w, h) location replaced by an 8-value polygon around it."""
+    out = []
+    for g, per_k in enumerate(regions):
+        W, H = sizes[g]
+        out.append([])
+        for traj in per_k:
+            poly_traj = []
+            for x in traj:
+                if isinstance(x, int):
+                    poly_traj.append(x)
+                    continue
+                bx, by, w, h = x
+                if w < 0.1:                                             # the degenerate gt's frames: stays NaN
+                    poly_traj.append(np.array([bx, by, bx + w, by, bx + w, by + h, bx, by + h]))
+                    continue
+                a = rng.uniform(-0.6, 0.6)
+                c, s = np.cos(a), np.sin(a)
+                cx, cy = bx + w / 2, by + h / 2
+                u = rng.rand()
+                if u < 0.15:                                            # partly off the frame, negative coordinates
+                    cx, cy = rng.choice([-0.3 * w, W + 0.3 * w]), rng.choice([-0.3 * h, cy])
+                pts = [(-w / 2, -h / 2), (w / 2, -h / 2), (w / 2, h / 2), (-w / 2, h / 2)]
+                p = np.array([v for dx, dy in pts for v in (cx + c * dx - s * dy, cy + s * dx + c * dy)])
+                p += rng.uniform(-0.02, 0.02, 8) * max(w, h)
+                if 0.15 <= u < 0.35:                                    # exact ties at the 5th decimal
+                    p = np.floor(p) + rng.choice([1, 3, 5, 7, 9, 11, 13, 29], 8) / 32.0
+                elif 0.35 <= u < 0.42:
+                    p[rng.randint(8)] = -rng.uniform(0, 4.9e-5)         # printed as -0.0000
+                poly_traj.append(p)
+            out[-1].append(poly_traj)
+    return out
+
+
 def build_region(tmp):
     """The reference's Cython region module, compiled in tmp; returns the extension's path."""
     src = os.path.join(REF, "utils", "pysot", "utils")
@@ -140,10 +182,12 @@ class Dataset:
         return iter(self.videos.values())
 
 
-def main():
+def main(poly: bool = False):
     from siammask_b200 import vot
     rng = np.random.RandomState(7)
     gts, sizes, regions = make_inputs(rng)
+    if poly:
+        regions = to_polygons(regions, sizes, np.random.RandomState(11))
     G = len(gts)
     names = [f"seq{g}" for g in range(G)]
     trackers = [f"combo{k}" for k in range(K)]
@@ -202,23 +246,26 @@ def main():
         n = int(np.sum([f for f in ar[t]["failures"].values()]))
         lost.append(n)
         robustness.append(n / len(ov) * 100)
-    rec = np.zeros((K, G, Tmax, 5))
+    rec = np.zeros((K, G, Tmax, 9 if poly else 5))
     for g in range(G):
         for k in range(K):
             for f, x in enumerate(regions[g][k]):
-                rec[k, g, f] = (x, 0, 0, 0, 0) if isinstance(x, int) else (3, *x)
+                rec[k, g, f, 0] = x if isinstance(x, int) else 3
+                if not isinstance(x, int):
+                    rec[k, g, f, 1:] = x
     gt = np.zeros((G, Tmax, 8))
     for g in range(G):
         gt[g, :T[g]] = gts[g]
-    np.savez_compressed(OUT, rec=rec, gt=gt, length=np.asarray(T, np.int32), size=np.asarray(sizes, np.int32),
+    out = OUT_POLY if poly else OUT
+    np.savez_compressed(out, rec=rec, gt=gt, length=np.asarray(T, np.int32), size=np.asarray(sizes, np.int32),
                         acc_overlap_bits=acc_bits, eao_overlap_bits=eao_bits, accuracy=np.asarray(accuracy),
                         robustness=np.asarray(robustness), lost_number=np.asarray(lost, np.int64),
                         curve=np.asarray(curves, np.float32), eao_vot2018=np.asarray([eao18[t]["all"] for t in trackers]),
                         eao_vot2019=np.asarray([eao19[t]["all"] for t in trackers]))
-    print(f"wrote {OUT}: {K} trackers x {G} sequences, lengths {T}; accuracy {np.round(accuracy, 4).tolist()}, "
+    print(f"wrote {out}: {K} trackers x {G} sequences, lengths {T}; accuracy {np.round(accuracy, 4).tolist()}, "
           f"lost {lost}, EAO 2018 {[round(eao18[t]['all'], 4) for t in trackers]}, "
           f"2019 {[round(eao19[t]['all'], 4) for t in trackers]}")
 
 
 if __name__ == "__main__":
-    main()
+    main(poly="--poly" in sys.argv[1:])
