@@ -329,10 +329,12 @@ def _cout_pad(cout):
 
 def launches(search_size, B, max_batch=None, with_mask=True, refine=True):
     """Every tensor-core conv, stem and engine-xcorr launch of one template + track_mask + track_refine at batch B on
-    the tensor backend, as dicts (side, name, kernel, lane, M, tiles).  Template launches run once over all B streams;
-    search-side and refine launches run once per lane on that lane's streams (schedule.lane_split).  M is the launch's
-    output rows (streams x Ho x Wo); tiles counts the persistent kernels' work items (GEMM / stem: 128-row M tiles x
-    N tiles; patch conv: RO-row blocks per image; xcorr: its blocks of 32 channels x row band per stream)."""
+    the tensor backend, as dicts (side, name, kernel, lane, M, tiles, s0, hw, ho, ntile).  Template launches run once
+    over all B streams; search-side and refine launches run once per lane on that lane's streams (schedule.lane_split).
+    M is the launch's output rows (streams x Ho x Wo); tiles counts the persistent kernels' work items (GEMM / stem:
+    128-row M tiles x N tiles; patch conv: RO-row blocks per image; xcorr: its blocks of 32 channels x row band per
+    stream).  s0 is the lane's first stream, hw = ho * ho the output rows per stream, ntile the GEMM's N tiles (the
+    patch conv's row blocks per image)."""
     from siammask_b200.checkpoint import expected_keys
     from siammask_b200.schedule import lane_split
 
@@ -381,22 +383,29 @@ def launches(search_size, B, max_batch=None, with_mask=True, refine=True):
             size[t.name] = ho
             if kernel is None:
                 continue
+            if kernel == "patch":
+                ntile = -(-ho // _patch_ro(ho))
+            elif kernel == "xcorr":
+                ntile = 8 * bands
+            s0 = 0
             for lane, b in enumerate(chunks):
                 M = b * ho * ho
-                if kernel == "patch":
-                    tiles = b * -(-ho // _patch_ro(ho))
-                elif kernel == "xcorr":
-                    tiles = 8 * b * bands
-                else:
-                    tiles = -(-M // 128) * ntile
-                out.append(dict(side=side, name=t.name, kernel=kernel, lane=lane, M=M, tiles=tiles))
+                tiles = b * ntile if kernel in ("patch", "xcorr") else -(-M // 128) * ntile
+                out.append(dict(side=side, name=t.name, kernel=kernel, lane=lane, M=M, tiles=tiles, s0=s0,
+                                hw=ho * ho, ho=ho, ntile=ntile))
+                s0 += b
     return out
 
 
 def tile_classes(launch, num_sms=132):
     """The ragged-tile classes a launch exercises: 'a' when its last 128-row tile ends in the first warpgroup's 64 rows
     (the second consumer warpgroup has no row to store), 'b' when it ends in the second's, 'c' when there are more
-    tiles than SMs (persistent CTAs take a second tile)."""
+    tiles than SMs (persistent CTAs take a second tile), 'd' when there are more than two tiles per CTA of the
+    persistent grid, min(tiles, num_sms) (conv_gemm_sm90.cu launch_cfg, stem_sm90.cu, conv3x3_patch_sm90.cu
+    launch_patch): only from the third tile on do the producer's stage ring and the mbarrier phase parities, the
+    epilogue's per-warpgroup staging buffers and the patch conv's cross-tile patch prefetch come back round to the state
+    they started from.  The xcorr is not persistent: one block per work item, nothing carried from one to the next, so
+    it has no (d); its (c) means a second wave of blocks."""
     r, cls = launch["M"] % 128, set()
     if 0 < r <= 64:
         cls.add("a")
@@ -404,7 +413,50 @@ def tile_classes(launch, num_sms=132):
         cls.add("b")
     if launch["tiles"] > num_sms:
         cls.add("c")
+        if launch.get("kernel") != "xcorr" and launch["tiles"] > 2 * num_sms:
+            cls.add("d")
     return cls
+
+
+def work_rows(launch, t, reverse_m=False):
+    """Output rows [r0, r1) of the launch (lane-local) that work item t computes.  GEMM / stem: M block t // ntile,
+    counted from the end with reverse_m (conv_gemm_sm90.cu m_block); patch conv: image t // ntile, its RO-row block
+    t % ntile (conv3x3_patch_sm90.cu)."""
+    M, hw, ho = launch["M"], launch["hw"], launch["ho"]
+    if launch["kernel"] == "patch":
+        b, blk = divmod(t, launch["ntile"])
+        ro = _patch_ro(ho)
+        return b * hw + blk * ro * ho, b * hw + min(ho, (blk + 1) * ro) * ho
+    mb = t // launch["ntile"]
+    if reverse_m:
+        mb = -(-M // 128) - 1 - mb
+    return mb * 128, min(M, (mb + 1) * 128)
+
+
+def rows_streams(launch, r0, r1):
+    """The streams (global index) holding the lane-local output rows [r0, r1)."""
+    return set(range(launch["s0"] + r0 // launch["hw"], launch["s0"] + (r1 - 1) // launch["hw"] + 1))
+
+
+def last_tile_streams(launch):
+    """The streams holding rows of the launch's last 128-row M tile (the ragged one, wherever a CTA meets it)."""
+    return rows_streams(launch, (-(-launch["M"] // 128) - 1) * 128, launch["M"])
+
+
+def pass_streams(launch, num_sms=132):
+    """The streams holding the first rows of the work items a persistent CTA takes on its second and third pass (work
+    items grid and 2 grid, grid = min(tiles, num_sms)), for the GEMM in both M orders: the engine picks reverse_m per
+    launch from where the layer's biggest input was last written (engine.cu conv_into, last_end_), which is keyed by
+    buffer address and so depends on the calls an engine ran before.  The xcorr has no passes."""
+    if launch["kernel"] == "xcorr":
+        return set()
+    grid, out = min(launch["tiles"], num_sms), set()
+    for t in (grid, 2 * grid):
+        if t < launch["tiles"]:
+            for rev in ((False, True) if launch["kernel"] == "gemm" else (False,)):
+                r0 = work_rows(launch, t, rev)[0]
+                out |= rows_streams(launch, r0, r0 + 1)
+    return out
 
 
 # ---------------------------------------------------------------------------------------------------- mutations

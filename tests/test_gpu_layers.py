@@ -95,13 +95,26 @@ def _rows(t, rows):
 
 
 class Run:
-    """The exported tensors of one engine call sequence, restricted to the checked streams."""
+    """The exported tensors of one engine call sequence, restricted to the checked streams.  tap_streams (optional):
+    tap name -> the subset of `streams` checked at that tap (default: all of them); mutation_streams (optional): the
+    subset of `streams` every tap's mutations are evaluated at (default: the tap's checked streams)."""
 
-    def __init__(self, m, z, x, streams, pos, outputs, kernel_rows=None, calibrated=False):
+    def __init__(self, m, z, x, streams, pos, outputs, kernel_rows=None, calibrated=False, tap_streams=None,
+                 mutation_streams=None):
         self.m, self.streams, self.outputs, self.calibrated = m, list(streams), outputs, calibrated
         self.kernel_rows = list(kernel_rows) if kernel_rows is not None else self.streams
         self.base = {"z": _rows(z, streams), "x": _rows(x, streams), "pos": np.asarray(pos)[self.streams]}
         self.cache = {}
+        self.tap_streams, self.mutation_streams = tap_streams, mutation_streams
+
+    def select(self, name, mutation=False):
+        """Positions in `streams` of the streams checked at tap `name` (mutation: of the streams its mutations are
+        evaluated at), or None for all of them."""
+        if mutation and self.mutation_streams is not None:
+            return [self.streams.index(s) for s in sorted(self.mutation_streams)]
+        if self.tap_streams is None or name not in self.tap_streams:
+            return None
+        return [self.streams.index(s) for s in sorted(self.tap_streams[name])]
 
     def get(self, name, for_xcorr=False):
         if name in self.base:
@@ -128,24 +141,33 @@ def _tap_list(backend, with_mask, mask_head, refine):
     return taps
 
 
-def check(cfg, run, sd, precision, backend="tensor", with_mask=True, mask_head=True, refine=True):
+def check(cfg, run, sd, precision, backend="tensor", with_mask=True, mask_head=True, refine=True, stale=None):
     """Check every tap, and that its gate rejects every mutation of the layer; returns (failures, mutations the gate
-    accepts).  The measured numbers go to TABLE."""
+    accepts).  The measured numbers go to TABLE.  stale (optional): stale(name, tap, fetch, streams) -> a fetch that
+    returns the tap's inputs (rows: `streams`) with some rows of the previous engine call in place of this call's, or
+    None; the gate must reject that as well (mutation d)."""
     mode = "exact" if precision == "exact" else "fast"
     fails, insensitive = [], []
     taps = _tap_list(backend, with_mask, mask_head, refine)
     # backbone layers run on both sides under one activation scale
     shared = {t.name for t, p in taps if p} & {t.name for t, p in taps if not p and t.op == "conv"}
     for tap, prefix in taps:
-        def fetch(n, prefix=prefix, tap=tap):
-            if n in ("z", "x", "pos"):
-                return run.get(n)
-            if prefix and n != "z":
-                return run.get(prefix + n)
-            return run.get(n, for_xcorr=tap.op == "xcorr" and n.startswith("template:"))
         name = prefix + tap.name
+
+        def fetcher(sel, prefix=prefix, tap=tap):
+            def fetch(n):
+                if n in ("z", "x", "pos"):
+                    t = run.get(n)
+                elif prefix and n != "z":
+                    t = run.get(prefix + n)
+                else:
+                    t = run.get(n, for_xcorr=tap.op == "xcorr" and n.startswith("template:"))
+                return t if sel is None else t[sel]
+            return fetch
+        sel, msel = run.select(name), run.select(name, mutation=True)
+        fetch = fetcher(sel)
         ref, scale = lr.evaluate(sd, tap, fetch)
-        got = run.get(name)
+        got = run.get(name) if sel is None else run.get(name)[sel]
         fam = lr.family(tap, backend)
         if fam == "exact":
             if not torch.equal(got.float(), ref.float().reshape(got.shape)):
@@ -164,8 +186,13 @@ def check(cfg, run, sd, precision, backend="tensor", with_mask=True, mask_head=T
             fails.append(f"{name} ({fam}/{mode}): measured gamma {raw:.3e}, {gated:.2f} x the gate; worst at {i}: "
                          f"got {float(got.reshape(ref.shape)[i]):.6e} ref {float(ref[i]):.6e} scale "
                          f"{float(scale[i]):.3e} (max|ref| {float(ref.abs().max()):.3e})")
+        if msel != sel:                                           # the mutations at other (fewer) streams
+            fetch = fetcher(msel)
+            ref, scale = lr.evaluate(sd, tap, fetch)
+        stale_fetch = None if stale is None else stale(name, tap, fetch,
+                                                       run.streams if msel is None else [run.streams[i] for i in msel])
         insensitive += [f"{name}: {m}" for m in _mutations_passing(sd, tap, fetch, ref, scale, gamma, rho, tau,
-                                                                    fam, precision)
+                                                                    fam, precision, stale_fetch)
                         if (cfg, name, m[0]) not in SHIFT_DOMINATED]
     return fails, insensitive
 
@@ -175,12 +202,15 @@ def _split(n):
     return n not in ("x", "z", "pos") and n not in lr.F32_OUT
 
 
-def _mutations_passing(sd, tap, fetch, ref, scale, gamma, rho, tau, fam, precision):
+def _mutations_passing(sd, tap, fetch, ref, scale, gamma, rho, tau, fam, precision, stale_fetch=None):
     """Mutations of the layer that its gate fails to reject.  (a) exact mode: the lo plane of every split-fp16 input is
     dropped (the xcorr's search input and kernel separately); (b) exact mode, tensor-core convs: the weight lo plane is
     dropped; (c) one 64-channel k-block of one kernel tap of the (first) conv is missing; for the fp32 SIMT convs and
-    the deconv one input channel, for xcorr one of the 25 taps."""
+    the deconv one input channel, for xcorr one of the 25 taps; (d) with stale_fetch: input rows the previous engine
+    call left behind read in place of this call's."""
     muts = {}
+    if stale_fetch is not None:
+        muts["d: stale rows of the previous call"] = dict(fetch=stale_fetch)
     if precision == "exact":
         if tap.op == "xcorr":
             muts["a: search lo dropped"] = dict(fetch=lambda n: lr.round_sig(fetch(n)) if n == tap.inputs[0]
