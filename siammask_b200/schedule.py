@@ -1,5 +1,5 @@
 """Queue scheduling of (sequence, combination) streams through one engine: the admission plan `VotRunner.open_queue`,
-`ParamSweep.open_queue` and `VideoSegmenter.open_queue` follow.
+`ParamSweep.open_queue` and `VideoSegmenter.open_queue` follow, and the plumbing those classes share (`QueueRun`).
 
 A benchmark run is G sequences x K hyper-parameter combinations, one tracker stream each, and the engine holds at most
 `capacity` of them.  Run in fixed chunks, every stream of a chunk starts on frame 0 and the batch only shrinks, so a
@@ -95,6 +95,53 @@ class Scheduler:
         self._active -= int(sum(self.width[s // self.K] for s in retire))
         self.f += 1
         return Step(need, entry, track, list(new), retire)
+
+
+class QueueRun:
+    """The queue plumbing of `VotRunner`, `ParamSweep` and `VideoSegmenter`, whose `open` / `frame` and `open_queue` /
+    `step` feed one step body per class.  `tracker` is the run's `BatchTracker`; `_sched` is None outside a queue run."""
+
+    _sched = None
+    _plan = None
+
+    @property
+    def pending(self) -> bool:
+        """Whether a queue run has steps left."""
+        return self._sched is not None and self._plan is not None
+
+    def needed(self) -> list:
+        """The distinct (sequence, frame) pairs the next `step` reads, in the order its lists follow."""
+        return list(self._pending_step().need)
+
+    def _pending_step(self, **lists) -> Step:
+        """The next step of the plan; ValueError unless a queue run is pending and every list (frames, annos) holds one
+        entry per needed() entry."""
+        if not self.pending:
+            raise ValueError("no queue step is pending: call open_queue() first; the run has finished")
+        n = len(self._plan.need)
+        for name, v in lists.items():
+            if not isinstance(v, (list, tuple)) or len(v) != n:
+                raise ValueError(f"{name} must be a list of {n} entries, one per needed() entry")
+        return self._plan
+
+    def _queue(self, lengths, K: int, widths=None):
+        """Plans a queue run through min(max_batch, free slots) engine slots and takes its first step."""
+        net = self.tracker.net
+        cap = min(net.max_batch, net.num_slots - self.tracker.slot0)
+        if cap < 1:
+            raise ValueError("the engine has no free slot")
+        self._sched = Scheduler(lengths, K, cap, widths)
+        self._plan = self._sched.step()
+
+    def _advance(self):
+        self._plan = self._sched.step() if not self._sched.done else None
+
+    def _repoint(self, want: list):
+        """Points the tracker's rows at their entries (`want`, in row order) of the step's frame list.  The list moves
+        only after admissions or departures, so the table is uploaded only then."""
+        bt = self.tracker
+        if want != bt._fidx:
+            bt.set_frame_index(bt.ids, want)
 
 
 MAX_LANES = 2         # engine.cu kMaxLanes

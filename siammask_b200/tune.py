@@ -5,12 +5,13 @@ The reference re-runs the whole `siamese_init` / `siamese_track` loop on the sam
 (utils/average_meter_helper.py:71-113): the pasted soft mask thresholded at each of `np.arange(0.3, 0.81, 0.05)`
 against `anno > 0`.  Here the K combinations x G videos are one batch of tracker streams: stream (g, k) reads video g's
 frames in place and carries combination k in the tracker's per-stream hyper-parameter table (`sm_step_slots_hp`,
-`sm_tracker_update_hp`).  Each frame is scored by one fused paste-back + count kernel (`sm_mask_iou`) without
-materialising a frame-sized mask per stream, and the IoU rows stay on the device until `ParamSweep.result`.
+`sm_tracker_update_hp`).  Each frame is scored by one fused paste-back + count kernel (`sm_mask_iou_ragged`, over
+the frame's packed annotations) without materialising a frame-sized mask per stream, and the IoU rows stay on the
+device until `ParamSweep.result`.
 
 `open_queue` / `needed` / `step` run a sweep of any size, with videos of different lengths and frame sizes, through a
-queue of streams (`schedule.Scheduler`); each step is scored by `sm_mask_iou_ragged` over the step's packed
-annotations.
+queue of streams (`schedule.Scheduler`).  `open` / `frame` run G same-size videos as one step of that kind each, all
+streams admitted at once.
 
 The rotated box of `siamese_track` (contours / minAreaRect) is not computed: tune_vos never scores it.
 """
@@ -20,7 +21,7 @@ import numpy as np
 import torch
 
 from . import ops
-from .schedule import Scheduler
+from .schedule import QueueRun, Step
 from .tracker import BatchTracker, FramePacker, TrackerParams
 
 # tools/tune_vos.py's default ranges (--penalty-k 0.0,0.1,0.03 --window-influence 0.3,0.5,0.04 --lr 0.8,1.01,0.05)
@@ -57,15 +58,24 @@ def _check_thresholds(thrs) -> np.ndarray:
     return t
 
 
+def _check_combos(combos) -> np.ndarray:
+    c = np.asarray(combos, dtype=np.float64)
+    if c.ndim != 2 or c.shape[1] != 3 or c.shape[0] == 0:
+        raise ValueError(f"combos must be [K, 3] (penalty_k, window_influence, lr), got {c.shape}")
+    if not np.isfinite(c).all():
+        raise ValueError("combos must be finite")
+    return c
+
+
 def _one_size(frames, fr) -> bool:
     """Whether `frames` (fr: the tracker's `Packed` of them) is a [G,H,W,3] batch or a list of frames of one size:
-    `sm_mask_iou` scores same-size videos only."""
+    `open` / `frame` take same-size videos only."""
     if isinstance(frames, (list, tuple)):
         return None not in fr.shapes and len(set(fr.shapes)) == 1
     return np.ndim(frames) == 4
 
 
-class ParamSweep:
+class ParamSweep(QueueRun):
     """tune_vos's grid search over `combos` (float64 [K,3] = penalty_k, window_influence, lr; default `grid()`) for G
     videos on one engine.  `net` is a `siammask_b200.Custom` whose max_batch and num_slots cover G*K streams; `params`
     holds the settings the combinations do not (context_amount, out_size, ...).  Masks come from the refine module when
@@ -75,21 +85,34 @@ class ParamSweep:
         self.tracker = BatchTracker(net, params)
         self.p = self.tracker.p
         self.dev = self.tracker.dev
-        c = grid() if combos is None else np.asarray(combos, dtype=np.float64)
-        if c.ndim != 2 or c.shape[1] != 3 or c.shape[0] == 0:
-            raise ValueError(f"combos must be [K, 3] (penalty_k, window_influence, lr), got {c.shape}")
-        if not np.isfinite(c).all():
-            raise ValueError("combos must be finite")
-        self.combos = c
+        self.combos = _check_combos(grid() if combos is None else combos)
         self.thrs = _check_thresholds(thrs)
         self._thrs_dev = torch.as_tensor(self.thrs, device=self.dev)
         self.G = 0
         self.f = self.T = 0
-        self._sched = None
 
     @property
     def K(self) -> int:
         return int(self.combos.shape[0])
+
+    def _reset(self, boxes_xywh, lengths):
+        """The state of a run over len(lengths) videos of lengths[g] frames: no stream admitted yet, every IoU row 0."""
+        G, K = len(lengths), self.K
+        boxes = np.asarray(boxes_xywh, dtype=np.float64)
+        if boxes.shape != (G, 4):
+            raise ValueError(f"boxes_xywh must be [{G}, 4]")
+        self._boxes, self._hw = boxes, [None] * G
+        self._video = np.repeat(np.arange(G), K)
+        self._vT = np.asarray(lengths, np.int64)[self._video]
+        self._off = np.concatenate([[0], np.cumsum(self._vT - 2)[:-1]])      # stream s owns IoU rows off[s] ..
+        self._iou = torch.zeros(int((self._vT - 2).sum()), self.thrs.size, dtype=torch.float32, device=self.dev)
+        self._admit = np.full(G * K, -1, np.int64)     # the step at which each stream was templated
+        self._annos = FramePacker(self.dev)
+        self.tracker._clear()
+        self._stream_of, self._id_of = {}, [None] * (G * K)
+        self._sched = self._plan = None
+        self.G, self.f = G, 0
+        self._index_rows()
 
     @torch.no_grad()
     def open(self, frames0, boxes_xywh, num_frames: int):
@@ -100,29 +123,24 @@ class ParamSweep:
         if not _one_size(frames0, fr):
             raise ValueError("frames0 must be [G,H,W,3]")
         G, K, T = len(fr.shapes), self.K, int(num_frames)
-        boxes = np.asarray(boxes_xywh, dtype=np.float64)
-        if boxes.shape != (G, 4):
-            raise ValueError(f"boxes_xywh must be [{G}, 4]")
         if T < 3:
             raise ValueError("num_frames must be >= 3 (the first and the last frame are not scored)")
         net = self.tracker.net
         if G * K > net.max_batch or G * K > net.num_slots - self.tracker.slot0:
             raise ValueError(f"{G} videos x {K} combinations = {G * K} streams exceed the engine's max_batch "
                              f"({net.max_batch}) or free slots ({net.num_slots - self.tracker.slot0}); split the grid")
-        self._sched = None
-        video = np.repeat(np.arange(G), K)
-        self.tracker._clear()
-        self.tracker.add(fr, np.repeat(boxes, K, axis=0), frame_index=video, hp=np.tile(self.combos, (G, 1)))
-        self._video = torch.as_tensor(video.astype(np.int32), device=self.dev)
-        self._iou = torch.zeros(T - 2, G * K, self.thrs.size, dtype=torch.float32, device=self.dev)
-        self.G, self.T, self.f = G, T, 1
+        self._reset(boxes_xywh, [T] * G)
+        self.T = T
+        self._run(fr, None, Step([(g, 0) for g in range(G)], {s: s // K for s in range(G * K)}, [],
+                                 list(range(G * K)), []))
         return self
 
     @torch.no_grad()
     def frame(self, frames, annos=None):
         """Track frame f (the next one) of every video: frames uint8 [G,H,W,3]; annos uint8 [G,H,W] annotation label maps
         of this frame, required when it is scored (0 < f < T-1).  The frame's IoU rows (float32(intersection / union),
-        1 where the union is empty) are written into a device buffer.  Returns the tracker's `TrackResult`."""
+        1 where the union is empty) are written into a device buffer.  Returns the tracker's `TrackResult`.  The streams
+        leave the engine after the last frame."""
         f = self.f
         if self._sched is not None:
             raise ValueError("a queue run advances with step(); frame() belongs to open()")
@@ -132,36 +150,28 @@ class ParamSweep:
         if not _one_size(frames, fr) or len(fr.shapes) != self.G:
             raise ValueError(f"frames must be [{self.G},H,W,3]")
         H, W = fr.shapes[0]
-        scored = f < self.T - 1
         anno = None
-        if scored:
+        if f < self.T - 1:
             if annos is None:
                 raise ValueError(f"frame {f} is scored: annotations are required")
-            anno = torch.as_tensor(annos).to(self.dev).contiguous()
-            if anno.dtype != torch.uint8 or tuple(anno.shape) != (self.G, H, W):
+            a = torch.as_tensor(annos).to(self.dev).contiguous()
+            if a.dtype != torch.uint8 or tuple(a.shape) != (self.G, H, W):
                 raise ValueError(f"annos must be uint8 [{self.G},{H},{W}]")
-        r = self.tracker.track(fr, mask=True, refine=self.p.out_size == 127, paste=False)
-        if scored:
-            cnt = ops._mask_iou(r.extras["mask_prob"], r.extras["maps"], anno, self._video, self._thrs_dev)
-            inter, union = cnt[..., 0].double(), cnt[..., 1].double()
-            # IouMeter.add: intxn / union in float64, stored into a float32 matrix; 1 when the union is empty
-            self._iou[f - 1] = torch.where(union > 0, (inter / union).float(), torch.ones_like(union, dtype=torch.float32))
-        self.f += 1
-        return r
+            anno = self._annos.wrap(a, 1)
+        S, K = self.G * self.K, self.K
+        return self._run(fr, anno, Step([(g, f) for g in range(self.G)], {s: s // K for s in range(S)},
+                                        self._row_streams, [], list(range(S)) if f == self.T - 1 else []))
 
     def result(self):
         """One D2H copy.  Returns (iou_list float32 [G,K,T] = IouMeter.value('mean') of every stream, per-frame IoU
         float32 [num_frames-2, G, K, T]); rows of frames not tracked yet are 0, as in a partly filled IouMeter.  After
         a queue run the per-frame IoU is a list of G arrays float32 [T_g-2, K, T], one per video."""
         G, K, n = self.G, self.K, self.thrs.size
-        if self._sched is not None:
-            flat = self._iou.cpu().numpy()
-            rows = [flat[o:o + m] for o, m in zip(self._off, self._vT - 2)]
-            means = np.stack([iou_mean(r) for r in rows]).reshape(G, K, n)
-            return means, [np.stack(rows[g * K:(g + 1) * K], 1) for g in range(G)]
-        per_frame = self._iou.cpu().numpy()
-        means = np.stack([iou_mean(per_frame[:, s]) for s in range(G * K)]).reshape(G, K, n)
-        return means, per_frame.reshape(-1, G, K, n)
+        flat = self._iou.cpu().numpy()
+        rows = [flat[o:o + m] for o, m in zip(self._off, self._vT - 2)]
+        means = np.stack([iou_mean(r) for r in rows]).reshape(G, K, n)
+        per_video = [np.stack(rows[g * K:(g + 1) * K], 1) for g in range(G)]
+        return means, np.stack(per_video, 1) if np.ndim(self.T) == 0 else per_video
 
     # ------------------------------------------------------------------ queue mode
     @torch.no_grad()
@@ -178,44 +188,15 @@ class ParamSweep:
                            [annos[g][t] if 0 < t < T[g] - 1 else None for g, t in need])
 
         and read `result()`: iou_list [G,K,T] and one per-frame array [T_g-2, K, T] per video."""
-        boxes = np.asarray(boxes_xywh, dtype=np.float64)
         T = np.asarray(num_frames).reshape(-1)
-        G, K = len(T), self.K
-        if G == 0:
+        if T.size == 0:
             raise ValueError("open_queue needs at least one video")
-        if boxes.shape != (G, 4):
-            raise ValueError(f"boxes_xywh must be [{G}, 4]")
         if not np.issubdtype(T.dtype, np.integer) or (T < 3).any():
             raise ValueError("num_frames must be integers >= 3 (the first and the last frame are not scored)")
-        net = self.tracker.net
-        cap = min(net.max_batch, net.num_slots - self.tracker.slot0)
-        if cap < 1:
-            raise ValueError("the engine has no free slot")
-        self._sched = Scheduler(T, K, cap)
-        self._plan = self._sched.step()
-        self._boxes, self._hw = boxes, [None] * G
-        self._qvideo = np.repeat(np.arange(G), K)
-        self._vT = T.astype(np.int64)[self._qvideo]
-        self._off = np.concatenate([[0], np.cumsum(self._vT - 2)[:-1]])      # stream s owns IoU rows off[s] ..
-        self._iou = torch.zeros(int((self._vT - 2).sum()), self.thrs.size, dtype=torch.float32, device=self.dev)
-        self._admit = np.full(G * K, -1, np.int64)
-        self._annos = FramePacker(self.dev)
-        self.tracker._clear()
-        self._stream_of, self._id_of = {}, [None] * (G * K)
-        self.G, self.T, self.f = G, T, 0
-        self._index_rows()
+        self._reset(boxes_xywh, T)
+        self.T = T
+        self._queue(T, self.K)
         return self
-
-    @property
-    def pending(self) -> bool:
-        """Whether a queue run has steps left."""
-        return self._sched is not None and self._plan is not None
-
-    def needed(self) -> list:
-        """The distinct (video, frame) pairs the next `step` reads, in the order its frame and annotation lists follow."""
-        if not self.pending:
-            raise ValueError("no queue step is pending: call open_queue() first; the run has finished")
-        return list(self._plan.need)
 
     def _index_rows(self):
         """Each active tracker row's stream and the IoU row it writes at step 0 (add the step): uploaded only when the
@@ -228,19 +209,12 @@ class ParamSweep:
     def step(self, frames, annos):
         """One step of a queue run: frames[i] / annos[i] are frame t of video g and its uint8 [H,W] annotation for
         (g, t) = needed()[i]; an annotation is required where 0 < t < T_g - 1 and ignored elsewhere (None will do).
-        Tracks every running stream one frame of its own video, scores it with `sm_mask_iou_ragged` against the packed
-        annotations, retires the streams whose video ends, then templates the admitted streams from their frame 0.
-        Returns the tracker's `TrackResult` of the streams that tracked a frame, or None when none did."""
-        if not self.pending:
-            raise ValueError("no queue step is pending: call open_queue() first; the run has finished")
-        st, f, bt = self._plan, self.f, self.tracker
-        n = len(st.need)
-        if not isinstance(frames, (list, tuple)) or len(frames) != n:
-            raise ValueError(f"frames must be a list of {n} frames, one per needed() entry")
-        if not isinstance(annos, (list, tuple)) or len(annos) != n:
-            raise ValueError(f"annos must be a list of {n} entries, one per needed() entry")
+        Tracks every running stream one frame of its own video, scores it against the packed annotations, retires the
+        streams whose video ends, then templates the admitted streams from their frame 0.  Returns the tracker's
+        `TrackResult` of the streams that tracked a frame, or None when none did."""
+        st = self._pending_step(frames=frames, annos=annos)
         scored = [0 < t < self.T[g] - 1 for g, t in st.need]
-        fr = bt._input(frames)
+        fr = self.tracker._input(frames)
         for i, (g, t) in enumerate(st.need):
             hw = fr.shapes[i]
             if self._hw[g] is not None and hw != self._hw[g]:
@@ -252,13 +226,20 @@ class ParamSweep:
                     raise ValueError(f"frame {t} of video {g} is scored: its annotation is required")
                 if a.dtype not in (np.uint8, torch.uint8) or tuple(a.shape) != tuple(hw):
                     raise ValueError(f"the annotation of frame {t} of video {g} must be uint8 [{hw[0]},{hw[1]}]")
+        r = self._run(fr, self._annos.pack([a if s else None for a, s in zip(annos, scored)], 1), st)
+        self._advance()
+        return r
+
+    def _run(self, fr, anno, st):
+        """Step st over the step's frames fr and annotations anno (a `Packed` in frame-list order, skipped where no
+        stream is scored; None when none is): tracks every running stream one frame of its own video, scores the rows
+        that are not on their video's last frame, retires the streams whose video ends, then templates the admitted
+        streams from their frame 0."""
+        f, bt = self.f, self.tracker
         r = None
         if st.track:
-            want = [st.entry[self._stream_of[i]] for i in bt.ids]
-            if want != bt._fidx:                        # the frame list moved: only after admissions or departures
-                bt.set_frame_index(bt.ids, want)
+            self._repoint([st.entry[self._stream_of[i]] for i in bt.ids])
             r = bt.track(fr, mask=True, refine=self.p.out_size == 127, paste=False)
-            anno = self._annos.pack([a if s else None for a, s in zip(annos, scored)], 1)
             masks, maps, video, dest = r.extras["mask_prob"], r.extras["maps"], bt._fidx_dev, self._row_dest + f
             last = set(st.retire)
             if last:                                    # rows on their video's last frame are not scored
@@ -266,29 +247,27 @@ class ParamSweep:
                 sel = torch.tensor(keep, dtype=torch.long, device=self.dev)
                 masks, maps, video, dest = masks[sel], maps[sel], video[sel], dest[sel]
             if dest.numel():
-                hs, ws = zip(*[anno.shapes[i] for i in range(n) if scored[i]])
+                hs, ws = zip(*[s for s in anno.shapes if s is not None])
                 cnt = ops._mask_iou_ragged(masks, maps, anno.data, anno.desc, video, (max(hs), max(ws)),
                                            self._thrs_dev)
                 inter, union = cnt[..., 0].double(), cnt[..., 1].double()
+                # IouMeter.add: intxn / union in float64, stored into a float32 matrix; 1 when the union is empty
                 iou = torch.where(union > 0, (inter / union).float(), torch.ones_like(union, dtype=torch.float32))
                 self._iou.index_copy_(0, dest, iou)
         gone = [self._id_of[s] for s in st.retire if self._id_of[s] is not None]
         if gone:
             bt.remove(gone)
         for s in st.admit:
-            g = int(self._qvideo[s])
+            g = int(self._video[s])
             if self._hw[g] is None:
                 self._hw[g] = fr.shapes[st.entry[s]]
             self._admit[s] = f
-        new = list(st.admit)
-        if new:
-            K = self.K
-            ids = bt.add(fr, self._boxes[self._qvideo[new]], frame_index=[st.entry[s] for s in new],
-                         hp=self.combos[[s % K for s in new]])
-            for s, i in zip(new, ids):
+        if st.admit:
+            ids = bt.add(fr, self._boxes[self._video[st.admit]], frame_index=[st.entry[s] for s in st.admit],
+                         hp=self.combos[[s % self.K for s in st.admit]])
+            for s, i in zip(st.admit, ids):
                 self._stream_of[i], self._id_of[s] = s, i
-        if gone or new:
+        if gone or st.admit:
             self._index_rows()
         self.f += 1
-        self._plan = self._sched.step() if not self._sched.done else None
         return r

@@ -27,8 +27,8 @@ The reference has two branches, both restated as they are:
 
 A whole dataset (videos of any length, frame size and object count) goes through `open_queue` / `needed` / `step`: the
 videos are queued by `schedule.Scheduler`, each holding as many slots as it has objects active at once (`peak_width`)
-from its admission until its last frame, and each admitted video advances one frame of its own per step, exactly as
-`frame` advances it.
+from its admission until its last frame, and each admitted video advances one frame of its own per step.  `frame` is a
+step of the same kind in which every video reads frame f, so one code path runs the loop in both.
 """
 from __future__ import annotations
 
@@ -37,7 +37,7 @@ import torch
 
 from . import ops
 from .ops import OBJ_IDLE, OBJ_INIT, OBJ_TRACKED
-from .schedule import Scheduler
+from .schedule import QueueRun
 from .tracker import BatchTracker, TrackerParams, upload
 from .tune import _check_thresholds
 
@@ -46,9 +46,9 @@ VOS_THRESHOLDS = np.arange(0.3, 0.5, 0.05)         # tools/test.py:30 thrs
 SCORE_MODES = (None, "whole", "spans")
 
 
-def schedule(start, end, f: int) -> np.ndarray:
+def schedule(start, end, f) -> np.ndarray:
     """What each object does at frame f (tools/test.py:492-501): OBJ_INIT where f == start, OBJ_TRACKED where
-    end >= f > start, OBJ_IDLE otherwise.  start, end: per-object frame numbers."""
+    end >= f > start, OBJ_IDLE otherwise.  start, end: per-object frame numbers; f: one frame, or one per object."""
     start, end = np.asarray(start, dtype=np.int64), np.asarray(end, dtype=np.int64)
     kind = np.full(start.shape, OBJ_IDLE, dtype=np.int32)
     kind[(end >= f) & (f > start)] = OBJ_TRACKED
@@ -97,7 +97,7 @@ def score_row(counts, lo: int, hi: int) -> np.ndarray:
     return res
 
 
-class VideoSegmenter:
+class VideoSegmenter(QueueRun):
     """track_vos for G videos on one engine.  `net` is a `siammask_b200.Custom` whose max_batch / num_slots cover the
     largest number of objects tracked at once; `params` the tracker hyper-parameters (seg_thr included)."""
 
@@ -107,7 +107,42 @@ class VideoSegmenter:
         self.dev = self.tracker.dev
         self.objects: list[tuple[int, int, int, int]] = []
         self.score = None
-        self._sched = None
+
+    def _reset(self, objs, G: int, lengths, score, thrs):
+        """The state of a run over objs (checked (video, id, start, end) tuples) in G videos of lengths[g] frames (None:
+        unbounded, without scoring): every object idle, no frame processed.  Checks the per-video object count and the
+        scored ids."""
+        members = [[k for k, o in enumerate(objs) if o[0] == g] for g in range(G)]
+        for g, ks in enumerate(members):
+            if len(ks) > 255:
+                raise ValueError(f"video {g}: at most 255 objects per video (labels are uint8)")
+        if score is not None:
+            self.thrs = _check_thresholds(thrs)
+            target, lo, hi = (np.zeros(len(objs), np.int64) for _ in range(3))
+            for g, ks in enumerate(members):
+                target[ks], lo[ks], hi[ks] = score_windows([objs[k] for k in ks], int(lengths[g]), score)
+                if np.unique(target[ks]).size != len(ks):
+                    raise ValueError(f"video {g}: scored object ids must be unique within a video")
+            self._target, self._lo, self._hi = target, lo, hi
+            n_rows = np.maximum(hi - lo, 0)
+            self._row0 = np.concatenate([[0], np.cumsum(n_rows)[:-1]]).astype(np.int64)
+            self._thrs_dev = torch.as_tensor(self.thrs, device=self.dev)
+            # (intersection, union) of object k at frame lo[k] + j, threshold t: row _row0[k] + j
+            self._rows = torch.zeros(int(n_rows.sum()), self.thrs.size, 2, dtype=torch.int32, device=self.dev)
+        self.objects, self.score, self.G, self._T = objs, score, G, lengths
+        self.order = [k for ks in members for k in ks]          # the objects grouped by video, each video's in order
+        self._members = members
+        self._video = np.array([o[0] for o in objs], np.int64)
+        self._start = np.array([o[2] for o in objs], np.int64)
+        self._end = np.array([o[3] for o in objs], np.int64)
+        self._sid: list[int | None] = [None] * len(objs)     # tracker stream of each object (None: not tracked)
+        self._hw: list = [None] * G                  # frame size of each video, from its frame 0
+        self._admitted = np.full(G, -1, np.int64)   # the step that read each video's frame 0
+        self._done = np.zeros(G, np.int64)          # frames of each video processed
+        self._table_key = self._tid_key = self._off_key = self._copy_key = None
+        self._sched = self._plan = None
+        self.tracker._clear()
+        self.f = 0
 
     def open(self, objects, num_frames: int | None = None, num_videos: int | None = None, score: str | None = None,
              thrs=VOS_THRESHOLDS):
@@ -134,51 +169,25 @@ class VideoSegmenter:
                 # (tools/test.py:502-503), so it could never appear in a label map
                 raise ValueError(f"object {o}: end_frame {o[3]} is before start_frame {o[2]}")
             objs.append(o)
-        self.G = max((o[0] for o in objs), default=-1) + 1 if num_videos is None else int(num_videos)
-        if self.G < 1 or any(o[0] >= self.G for o in objs):
+        G = max((o[0] for o in objs), default=-1) + 1 if num_videos is None else int(num_videos)
+        if G < 1 or any(o[0] >= G for o in objs):
             raise ValueError("every object's video index must be < num_videos")
-        counts = np.bincount([o[0] for o in objs], minlength=self.G)
-        if (counts > 255).any():
-            raise ValueError("at most 255 objects per video (labels are uint8)")
-        # objects grouped by video (stable): entry i of the kernel's table is object order[i]
-        self.order = sorted(range(len(objs)), key=lambda k: objs[k][0])
-        self.objects = objs
-        self._start = np.array([o[2] for o in objs], dtype=np.int64)
-        self._end = np.array([o[3] for o in objs], dtype=np.int64)
-        self._sid: list[int | None] = [None] * len(objs)     # tracker stream of each object (None: not tracked)
-        self._offsets = torch.tensor(np.concatenate([[0], np.cumsum(counts)]), dtype=torch.int32, device=self.dev)
-        self._table_key, self._table = None, None
-        self.score = score
-        if score is not None:
-            if any(o[3] > last for o in objs):
-                raise ValueError(f"scoring: every end_frame must be <= num_frames - 1 ({last})")
-            self.thrs = _check_thresholds(thrs)
-            target, self._lo, self._hi = score_windows(objs, int(num_frames), score)
-            for g in range(self.G):
-                v = target[[k for k in range(len(objs)) if objs[k][0] == g]]
-                if np.unique(v).size != v.size:
-                    raise ValueError(f"video {g}: scored object ids must be unique within a video")
-            self._target = target
-            self._thrs_dev = torch.as_tensor(self.thrs, device=self.dev)
-            self._tid_key, self._tid = None, None
-            # counts of frame f, entry i (kernel order, self.order[i]) and threshold t: (intersection, union)
-            self._counts = torch.zeros(int(num_frames), len(objs), self.thrs.size, 2, dtype=torch.int32, device=self.dev)
-        self._sched = None
-        self.tracker._clear()
-        self.f = 0
+        if score is not None and any(o[3] > last for o in objs):
+            raise ValueError(f"scoring: every end_frame must be <= num_frames - 1 ({last})")
+        self._reset(objs, G, None if num_frames is None else [int(num_frames)] * G, score, thrs)
         return self
 
-    def _target_ids(self, scored, order=None) -> torch.Tensor:
-        key = tuple(int(self._target[k]) if scored[k] else -1 for k in (self.order if order is None else order))
+    def _target_ids(self, scored, order) -> torch.Tensor:
+        key = tuple(int(self._target[k]) if scored[k] else -1 for k in order)
         if key != self._tid_key:              # changes only when an object's window opens or closes
             self._tid_key = key
             self._tid = upload(np.asarray(key, np.int64), torch.int32, self.dev)
         return self._tid
 
-    def _entries(self, kinds, rows, order=None) -> torch.Tensor:
-        """The kernel's object table: one (kind, arg) entry per object of `order` (default: every object, by video)."""
+    def _entries(self, kinds, rows, order) -> torch.Tensor:
+        """The kernel's object table: one (kind, arg) entry per object of `order`."""
         ent = []
-        for k in (self.order if order is None else order):
+        for k in order:
             if kinds[k] == OBJ_TRACKED:
                 ent.append((OBJ_TRACKED, rows[self._sid[k]]))
             elif kinds[k] == OBJ_INIT:
@@ -202,25 +211,21 @@ class VideoSegmenter:
         if self._sched is not None:
             raise ValueError("a queue run advances with step(); frame() belongs to open()")
         f, G = self.f, self.G
-        # the schedule and scoring checks need no frames: they fail before any frame reaches the device
-        kinds = schedule(self._start, self._end, f)
-        starting = [k for k in range(len(self.objects)) if kinds[k] == OBJ_INIT]
-        scored = None
+        # the scoring checks need no frames: they fail before any frame reaches the device
+        scored = False
         if self.score is not None:
-            if f >= self._counts.shape[0]:
-                raise ValueError(f"scoring: at most num_frames ({self._counts.shape[0]}) frames")
-            scored = (self._lo <= f) & (f < self._hi)
-            if scored.any() and annos is None:
+            if f >= self._T[0]:
+                raise ValueError(f"scoring: at most num_frames ({self._T[0]}) frames")
+            scored = bool(((self._lo <= f) & (f < self._hi)).any())
+            if scored and annos is None:
                 raise ValueError(f"frame {f} is scored: annotation label maps are required")
-            if not scored.any():
-                scored = None
         listed = isinstance(frames, (list, tuple))
         fr = self.tracker._input(frames)
         if listed and (len(fr.shapes) != G or any(s is None for s in fr.shapes)):
             raise ValueError(f"frames must be a list of {G} frames")
         if not listed and (np.ndim(frames) != 4 or len(fr.shapes) != G):
             raise ValueError(f"frames must be [{G},H,W,3]")
-        H, W = max(s[0] for s in fr.shapes), max(s[1] for s in fr.shapes)      # the grid of the label kernels
+        H, W = max(s[0] for s in fr.shapes), max(s[1] for s in fr.shapes)
         if listed and annos is not None:                # host check from shapes alone, before any device work
             if not isinstance(annos, (list, tuple)) or len(annos) != G:
                 raise ValueError(f"annos must be a list of {G} label maps, one per frame")
@@ -228,56 +233,20 @@ class VideoSegmenter:
             if shp != [tuple(s) for s in fr.shapes]:
                 raise ValueError(f"each anno must be [H_g, W_g] of its frame: {shp} vs {fr.shapes}")
         anno = None
-        if starting or scored is not None:
+        if scored or (self._start == f).any():
             if annos is None:
                 raise ValueError(f"frame {f}: objects start here, annotation label maps are required")
-            if listed:
+            if listed:                                  # their shapes were checked above
                 pa = self.tracker.packer.pack(annos, 1)
-                if pa.shapes != fr.shapes:
-                    raise ValueError(f"each anno must match its frame's size: {pa.shapes} vs {fr.shapes}")
             else:
                 a = torch.as_tensor(annos)
                 if a.dtype != torch.uint8 or tuple(a.shape) != (G, H, W):
                     raise ValueError(f"annos must be uint8 [{G},{H},{W}]")
                 pa = self.tracker.packer.wrap(a, 1)
             anno = pa.data
-        # sm_image_desc of the G label maps (and annotations)
-        desc, ptable = self.tracker.packer.table(fr.shapes, 1)
-        plane = (desc, int(ptable["offset"][-1]) + fr.shapes[-1][0] * fr.shapes[-1][1])
-        if starting:
-            # init boxes (:494-496): one D2H copy, at init frames only
-            queries = [(self.objects[k][0], self.objects[k][1]) for k in starting]
-            boxes = ops._label_boxes_ragged(anno, desc, G, queries).cpu().numpy()
-            missing = [self.objects[k][:2] for k, b in zip(starting, boxes) if b[2] == 0]
-            if missing:
-                raise ValueError(f"frame {f}: (video, id) {missing} not in the annotation")
-        bt = self.tracker
-        leaving = [k for k, s in enumerate(self._sid) if s is not None and kinds[k] != OBJ_TRACKED]
-        if leaving:
-            bt.remove([self._sid[k] for k in leaving])
-            for k in leaving:
-                self._sid[k] = None
-        masks = maps = None
-        rows = {}
-        if bt.N:
-            r = bt.track(fr, mask=True, refine=self.p.out_size == 127, paste=False)
-            masks, maps = r.extras["mask_prob"], r.extras["maps"]
-            rows = {sid: i for i, sid in enumerate(r.extras["ids"])}
-            self.last = r
-        table = self._entries(kinds, rows)
-        if starting:
-            xywh = boxes.astype(np.float64)
-            ids = bt.add(fr, xywh, frame_index=[self.objects[k][0] for k in starting])
-            for k, sid in zip(starting, ids):
-                self._sid[k] = sid
-        if scored is None:
-            labels = ops._paste_labels(masks, maps, anno, self._offsets, table, (H, W), self.p.seg_thr, ragged=plane)
-        else:
-            labels, _ = ops._paste_labels_iou(masks, maps, anno, self._offsets, table, self._target_ids(scored), (H, W),
-                                              self.p.seg_thr, self._thrs_dev, counts=self._counts[f], ragged=plane)
-        self.f += 1
+        labels, offsets = self._run(fr, anno, [(g, f) for g in range(G)])
         if listed:
-            return [labels[int(o):int(o) + h * w].view(h, w) for o, (h, w) in zip(ptable["offset"], fr.shapes)]
+            return [labels[int(o):int(o) + h * w].view(h, w) for o, (h, w) in zip(offsets, fr.shapes)]
         return labels.view(G, H, W)
 
     def state(self):
@@ -298,16 +267,13 @@ class VideoSegmenter:
         from the integer counts with the reference's float64 arithmetic (`score_row`); NaN for an empty window."""
         if self.score is None:
             raise ValueError("open(..., score='whole' | 'spans') or open_queue(..., score=...) first")
-        if self._sched is not None:
-            return self._queue_result()
-        counts = self._counts.cpu().numpy()
-        entry = {k: i for i, k in enumerate(self.order)}
-        rows = [score_row(counts[:, entry[k]], int(self._lo[k]), min(int(self._hi[k]), self.f))
-                for k in range(len(self.objects))]
+        counts = self._rows.cpu().numpy()
         out = []
-        for g in range(self.G):
-            r = [rows[k] for k in range(len(self.objects)) if self.objects[k][0] == g]
-            out.append(np.stack(r) if r else np.zeros((0, self.thrs.size), np.float32))
+        for g, ks in enumerate(self._members):
+            # frames lo .. min(hi, frames processed) - 1 of each object
+            out.append(np.stack([score_row(counts[self._row0[k]:self._row0[k] + max(self._hi[k] - self._lo[k], 0)], 0,
+                                           min(int(self._hi[k]), int(self._done[g])) - int(self._lo[k]))
+                                 for k in ks]) if ks else np.zeros((0, self.thrs.size), np.float32))
         return out
 
     # ------------------------------------------------------------------ queue mode
@@ -329,8 +295,6 @@ class VideoSegmenter:
         T = np.asarray(num_frames).reshape(-1)
         if T.size == 0 or not np.issubdtype(T.dtype, np.integer) or (T < 1).any():
             raise ValueError("num_frames must be one integer >= 1 per video")
-        if score not in SCORE_MODES:
-            raise ValueError(f"score must be one of {SCORE_MODES}, got {score!r}")
         G = int(T.size)
         objs = []
         for o in objects:
@@ -343,55 +307,12 @@ class VideoSegmenter:
                 raise ValueError(f"object {o}: needs 0 <= start_frame <= end_frame <= {int(T[o[0]]) - 1} "
                                  f"(video {o[0]}'s last frame)")
             objs.append(o)
-        members = [[k for k, o in enumerate(objs) if o[0] == g] for g in range(G)]
-        for g, ks in enumerate(members):
-            if not ks:
-                raise ValueError(f"video {g} has no object")
-            if len(ks) > 255:
-                raise ValueError(f"video {g}: at most 255 objects per video (labels are uint8)")
-        start = np.array([o[2] for o in objs], np.int64)
-        end = np.array([o[3] for o in objs], np.int64)
-        width = np.array([peak_width(start[ks], end[ks]) for ks in members], np.int64)
-        net = self.tracker.net
-        cap = min(net.max_batch, net.num_slots - self.tracker.slot0)
-        if cap < 1:
-            raise ValueError("the engine has no free slot")
-        sched = Scheduler(T, 1, cap, width)          # ValueError for a video wider than the engine
-        if score is not None:
-            self.thrs = _check_thresholds(thrs)
-            target, lo, hi = (np.zeros(len(objs), np.int64) for _ in range(3))
-            for g, ks in enumerate(members):
-                target[ks], lo[ks], hi[ks] = score_windows([objs[k] for k in ks], int(T[g]), score)
-                if np.unique(target[ks]).size != len(ks):
-                    raise ValueError(f"video {g}: scored object ids must be unique within a video")
-            self._target, self._lo, self._hi = target, lo, hi
-            n_rows = np.maximum(hi - lo, 0)
-            self._row0 = np.concatenate([[0], np.cumsum(n_rows)[:-1]]).astype(np.int64)
-            self._thrs_dev = torch.as_tensor(self.thrs, device=self.dev)
-            # (intersection, union) of object k at frame lo[k] + j, threshold t: row _row0[k] + j
-            self._rows = torch.zeros(int(n_rows.sum()), self.thrs.size, 2, dtype=torch.int32, device=self.dev)
-        self.objects, self.score, self.G = objs, score, G
-        self._start, self._end, self._members, self._qT = start, end, members, T.astype(np.int64)
-        self._sid = [None] * len(objs)
-        self._hw: list = [None] * G                  # frame size of each video, from its frame 0
-        self._admitted = np.full(G, -1, np.int64)   # the step that read each video's frame 0
-        self._done = np.zeros(G, np.int64)          # frames of each video processed
-        self._table_key = self._tid_key = self._off_key = self._copy_key = None
-        self._sched, self._plan = sched, sched.step()
-        self.tracker._clear()
-        self.f = 0
+        self._reset(objs, G, T.astype(np.int64), score, thrs)
+        if [] in self._members:
+            raise ValueError(f"video {self._members.index([])} has no object")
+        width = [peak_width(self._start[ks], self._end[ks]) for ks in self._members]
+        self._queue(T, 1, width)                     # ValueError for a video wider than the engine
         return self
-
-    @property
-    def pending(self) -> bool:
-        """Whether a queue run has steps left."""
-        return self._sched is not None and self._plan is not None
-
-    def needed(self) -> list:
-        """The (video g, frame t) pairs the next `step` reads, one per admitted video, in the order of its lists."""
-        if not self.pending:
-            raise ValueError("no queue step is pending: call open_queue() first; the run has finished")
-        return list(self._plan.need)
 
     def _wants_anno(self, g: int, t: int) -> bool:
         ks = self._members[g]
@@ -418,14 +339,7 @@ class VideoSegmenter:
         for every admitted video what `frame` does at its frame t: objects start, are tracked and leave, and the fused
         label map (with the scored objects' counts) comes from one ragged kernel pass over the step's videos.  Returns
         the label maps, a list of uint8 [H_g,W_g] device views in needed() order."""
-        if not self.pending:
-            raise ValueError("no queue step is pending: call open_queue() first; the run has finished")
-        st, f, bt = self._plan, self.f, self.tracker
-        n = len(st.need)
-        if not isinstance(frames, (list, tuple)) or len(frames) != n:
-            raise ValueError(f"frames must be a list of {n} frames, one per needed() entry")
-        if not isinstance(annos, (list, tuple)) or len(annos) != n:
-            raise ValueError(f"annos must be a list of {n} entries, one per needed() entry")
+        st = self._pending_step(frames=frames, annos=annos)
         # every check reads shapes on the host, before any device work
         want = [self._wants_anno(g, t) for g, t in st.need]
         for i, (g, t) in enumerate(st.need):
@@ -442,38 +356,49 @@ class VideoSegmenter:
                                      "required")
                 if a.dtype not in (np.uint8, torch.uint8) or self._size_of(a, "annotation") != hw:
                     raise ValueError(f"the annotation of frame {t} of video {g} must be uint8 [{hw[0]},{hw[1]}]")
-        fr = bt._input(frames)
-        for i, (g, t) in enumerate(st.need):
-            if t == 0:
-                self._hw[g], self._admitted[g] = fr.shapes[i], f
-        order = [k for g, _ in st.need for k in self._members[g]]
-        kinds = np.full(len(self.objects), OBJ_IDLE, np.int32)
-        scored = np.zeros(len(self.objects), bool)
-        for g, t in st.need:
-            ks = self._members[g]
-            kinds[ks] = schedule(self._start[ks], self._end[ks], t)
-            if self.score is not None:
-                scored[ks] = (self._lo[ks] <= t) & (t < self._hi[ks])
-        entry = {g: i for i, (g, _) in enumerate(st.need)}
-        starting = [k for k in order if kinds[k] == OBJ_INIT]
+        fr = self.tracker._input(frames)
         anno = None
-        if starting or scored.any():
+        if any(want):
             # every video of the step gets a map in the frames' layout (the kernels read both through one table)
             fill = [annos[i] if want[i] else
                     (torch.zeros(hw, dtype=torch.uint8, device=frames[i].device) if torch.is_tensor(frames[i])
                      else np.zeros(hw, np.uint8)) for i, hw in enumerate(fr.shapes)]
-            anno = bt.packer.pack(fill, 1).data
+            anno = self.tracker.packer.pack(fill, 1).data
+        labels, offsets = self._run(fr, anno, st.need)
+        self._advance()
+        return [labels[int(o):int(o) + h * w].view(h, w) for o, (h, w) in zip(offsets, fr.shapes)]
+
+    def _run(self, fr, anno, need):
+        """One step over the frames fr of `need` ((video g, frame t) pairs in frame-list order): every video of it does
+        at its frame t what the reference's loop does: objects start, are tracked and leave, and the fused label map
+        (with the scored objects' counts) comes from one ragged kernel pass.  anno: the packed annotations in the
+        frames' layout, None when no object starts or is scored.  Returns (packed labels, each video's offset)."""
+        f, bt, n = self.f, self.tracker, len(need)
+        for i, (g, t) in enumerate(need):
+            if t == 0:
+                self._hw[g], self._admitted[g] = fr.shapes[i], f
+        order = [k for g, _ in need for k in self._members[g]]
+        tv = np.full(self.G, -1, np.int64)
+        tv[[g for g, _ in need]] = [t for _, t in need]
+        t_obj = tv[self._video]                   # each object's frame in this step, -1 where its video is not in it
+        # objects of videos that are not in the step (ended, or not admitted yet) are idle
+        kinds = np.where(t_obj >= 0, schedule(self._start, self._end, t_obj), OBJ_IDLE)
+        scored = np.zeros(len(self.objects), bool)
+        if self.score is not None:
+            scored = (t_obj >= 0) & (self._lo <= t_obj) & (t_obj < self._hi)
+        entry = {g: i for i, (g, _) in enumerate(need)}
+        starting = [k for k in order if kinds[k] == OBJ_INIT]
         desc, ptable = bt.packer.table(fr.shapes, 1)
         plane = (desc, int(ptable["offset"][-1]) + fr.shapes[-1][0] * fr.shapes[-1][1])
-        H, W = max(s[0] for s in fr.shapes), max(s[1] for s in fr.shapes)
+        H, W = max(s[0] for s in fr.shapes), max(s[1] for s in fr.shapes)      # the grid of the label kernels
         if starting:
-            # init boxes: one D2H copy, at steps where objects start
+            # init boxes (:494-496): one D2H copy, at steps where objects start
             queries = [(entry[self.objects[k][0]], self.objects[k][1]) for k in starting]
             boxes = ops._label_boxes_ragged(anno, desc, n, queries).cpu().numpy()
             missing = [self.objects[k][:2] for k, b in zip(starting, boxes) if b[2] == 0]
             if missing:
-                raise ValueError(f"step {f}: (video, id) {missing} not in the annotation")
-        # objects that stopped and the objects of videos that ended in the last step (not in `order`: IDLE) leave
+                raise ValueError(f"(video, id) {missing} not in the annotation of their start frame")
+        # objects that stopped and the objects of videos that ended in the last step leave
         leaving = [k for k, s in enumerate(self._sid) if s is not None and kinds[k] != OBJ_TRACKED]
         if leaving:
             bt.remove([self._sid[k] for k in leaving])
@@ -483,9 +408,7 @@ class VideoSegmenter:
         rows = {}
         if bt.N:
             video = {self._sid[k]: self.objects[k][0] for k in order if self._sid[k] is not None}
-            idx = [entry[video[i]] for i in bt.ids]
-            if idx != bt._fidx:                          # the frame list moved: only after admissions or departures
-                bt.set_frame_index(bt.ids, idx)
+            self._repoint([entry[video[i]] for i in bt.ids])
             r = bt.track(fr, mask=True, refine=self.p.out_size == 127, paste=False)
             masks, maps = r.extras["mask_prob"], r.extras["maps"]
             rows = {sid: i for i, sid in enumerate(r.extras["ids"])}
@@ -495,14 +418,14 @@ class VideoSegmenter:
             ids = bt.add(fr, boxes.astype(np.float64), frame_index=[entry[self.objects[k][0]] for k in starting])
             for k, sid in zip(starting, ids):
                 self._sid[k] = sid
-        per = tuple(len(self._members[g]) for g, _ in st.need)
+        per = tuple(len(self._members[g]) for g, _ in need)
         if per != self._off_key:                         # changes only when a video is admitted or retires
             self._off_key = per
-            self._qoffsets = upload(np.concatenate([[0], np.cumsum(per)]), torch.int32, self.dev)
+            self._offsets = upload(np.concatenate([[0], np.cumsum(per)]), torch.int32, self.dev)
         if not scored.any():
-            labels = ops._paste_labels(masks, maps, anno, self._qoffsets, table, (H, W), self.p.seg_thr, ragged=plane)
+            labels = ops._paste_labels(masks, maps, anno, self._offsets, table, (H, W), self.p.seg_thr, ragged=plane)
         else:
-            labels, cnt = ops._paste_labels_iou(masks, maps, anno, self._qoffsets, table, self._target_ids(scored, order),
+            labels, cnt = ops._paste_labels_iou(masks, maps, anno, self._offsets, table, self._target_ids(scored, order),
                                                 (H, W), self.p.seg_thr, self._thrs_dev, ragged=plane)
             # object k's counts at its frame t = f - admitted go to row _row0[k] + t - lo[k]: a constant plus f
             src = [i for i, k in enumerate(order) if scored[k]]
@@ -513,18 +436,7 @@ class VideoSegmenter:
                 self._copy_src = upload(np.asarray(key[0], np.int64), torch.long, self.dev)
                 self._copy_dst = upload(np.asarray(key[1], np.int64), torch.long, self.dev)
             self._rows.index_copy_(0, self._copy_dst + f, cnt.index_select(0, self._copy_src))
-        for g, t in st.need:
+        for g, t in need:
             self._done[g] = t + 1
         self.f += 1
-        self._plan = self._sched.step() if not self._sched.done else None
-        return [labels[int(o):int(o) + h * w].view(h, w) for o, (h, w) in zip(ptable["offset"], fr.shapes)]
-
-    def _queue_result(self) -> list[np.ndarray]:
-        counts = self._rows.cpu().numpy()
-        out = []
-        for g, ks in enumerate(self._members):
-            # frames lo .. min(hi, frames processed) - 1 of each object, as `result` of a per-video run
-            out.append(np.stack([score_row(counts[self._row0[k]:self._row0[k] + max(self._hi[k] - self._lo[k], 0)], 0,
-                                           min(int(self._hi[k]), int(self._done[g])) - int(self._lo[k]))
-                                 for k in ks]))
-        return out
+        return labels, ptable["offset"]

@@ -25,8 +25,9 @@ Sequences of different frame sizes run in one batch: pass each frame as a list o
 the entry of a sequence that has ended may be None).
 
 A run larger than the engine goes through `open_queue` / `needed` / `step`: the (sequence, combination) streams are
-queued (`schedule.Scheduler`), a freed slot is refilled on the next step, and each stream runs the same protocol from
-its own frame 0; the step's frame list holds one entry per distinct (sequence, frame).
+queued (`schedule.Scheduler`), a freed slot is refilled on the next step, and each stream runs the protocol from its
+own frame 0; the step's frame list holds one entry per distinct (sequence, frame).  `open` / `frame` are steps of the
+same kind in which every stream was admitted at step 0, so one code path runs the protocol in both.
 
 `VotScore` scores finished runs the way tools/eval.py does for VOT2016/2017/2018/2019 ('all' tag): pysot's
 AccuracyRobustnessBenchmark (accuracy, robustness, lost number) and EAOBenchmark (expected-overlap curve and EAO), for
@@ -54,8 +55,9 @@ import numpy as np
 import torch
 
 from . import ops
-from .schedule import Scheduler
+from .schedule import QueueRun, Step
 from .tracker import BatchTracker, TrackerParams
+from .tune import _check_combos
 
 # tools/tune_vot.py's argparse defaults: a 9 x 14 x 3 grid of (penalty_k, window_influence, lr)
 DEFAULT_PENALTY_K = np.arange(0.05, 0.5, 0.05)
@@ -123,7 +125,7 @@ def write_result(path, regions) -> None:
         f.write("".join(line + "\n" for line in lines))
 
 
-class VotRunner:
+class VotRunner(QueueRun):
     """track_vot for G sequences on one engine; their frames may differ in size.  With combos=None
     each sequence is one stream with `params`' hyper-parameters; with combos float64 [K,3] = (penalty_k,
     window_influence, lr) rows (tune_vot's grid is `tune.grid(DEFAULT_PENALTY_K, DEFAULT_WINDOW_INFLUENCE,
@@ -149,17 +151,9 @@ class VotRunner:
         self.tracker = BatchTracker(net, params)
         self.p = self.tracker.p
         self.dev = self.tracker.dev
-        self.combos = None
-        if combos is not None:
-            c = np.asarray(combos, dtype=np.float64)
-            if c.ndim != 2 or c.shape[1] != 3 or c.shape[0] == 0:
-                raise ValueError(f"combos must be [K, 3] (penalty_k, window_influence, lr), got {c.shape}")
-            if not np.isfinite(c).all():
-                raise ValueError("combos must be finite")
-            self.combos = c
+        self.combos = None if combos is None else _check_combos(combos)
         self.G = 0
         self.f = 0
-        self._sched = None
 
     @property
     def K(self) -> int:
@@ -168,24 +162,42 @@ class VotRunner:
     @property
     def ended(self) -> bool:
         """Whether every stream of the run has tracked its sequence's last frame."""
-        if self._sched is not None:
-            return self._plan is None
-        return self.G > 0 and bool((self.T <= self.f).all())
+        return self.G > 0 and bool(((self._admit >= 0) & (self.f - self._admit >= self._video_T)).all())
 
-    def _load_gt(self, gt) -> int:
-        """Checks and uploads every gt row and computes get_axis_aligned_bbox of each on the host, in the reference's
-        arithmetic: self._init (cx, cy, w, h) [G, Tmax, 4]; returns G."""
+    def _reset(self, gt):
+        """Checks and uploads every gt row, computes get_axis_aligned_bbox of each on the host, in the reference's
+        arithmetic (self._init (cx, cy, w, h) [G, Tmax, 4]), and sets up a run of the G sequences with no stream
+        admitted yet."""
         gts = check_gt(gt)
+        G, K = len(gts), self.K
+        if G == 0:
+            raise ValueError("a run needs at least one sequence")
         self.T = np.array([a.shape[0] for a in gts])
-        Tmax = int(self.T.max()) if gts else 0
-        self._init = np.zeros((len(gts), Tmax, 4))
-        polys = np.zeros((len(gts), Tmax, 8), np.float32)
+        S, Tmax = G * K, int(self.T.max())
+        self._init = np.zeros((G, Tmax, 4))
+        polys = np.zeros((G, Tmax, 8), np.float32)
         for g, a in enumerate(gts):
             with np.errstate(divide="ignore", invalid="ignore"):
                 self._init[g, :len(a)] = [get_axis_aligned_bbox(row) for row in a]
             polys[g, :len(a)] = a                            # Polygon() stores C floats
         self._gt = torch.from_numpy(polys).to(self.dev)
-        return len(gts)
+        self._hw = [None] * G                           # each sequence's (H, W), from its frame 0
+        self._video = np.repeat(np.arange(G), K)
+        self._video_T = self.T[self._video]
+        self._admit = np.full(S, -1, np.int64)          # the step at which each stream was templated
+        self.tracker._clear()
+        self._stream_of, self._id_of = {}, [None] * S   # tracker id -> stream, stream -> tracker id
+        # rows [0, Tmax) of stream s: (entry code, location x, y, w, h) of its own frames; row Tmax: (lost_times, 0..)
+        self._rec = torch.zeros(Tmax + 1, S, 5, dtype=torch.float64, device=self.dev)
+        self._rec[0, :, 0] = CODE_INIT
+        self._poly = torch.zeros(Tmax, S, 8, dtype=torch.float64, device=self.dev) if self.mask else None
+        self._start = torch.zeros(S, dtype=torch.int32, device=self.dev)         # in the stream's own frames
+        self._flags = torch.zeros(S, dtype=torch.uint8, device=self.dev)
+        self._pinned = [torch.zeros(S, dtype=torch.uint8).pin_memory() for _ in range(SKIP_FRAMES + 1)]
+        self._events = [None] * (SKIP_FRAMES + 1)       # (step, event) of the flags in each pinned buffer
+        self._sched = self._plan = None
+        self.G, self.f = G, 0
+        self._index_rows()
 
     @torch.no_grad()
     def open(self, frames0, gt):
@@ -197,8 +209,7 @@ class VotRunner:
             raise ValueError("frames0 must be [G,H,W,3]")
         if any(s is None for s in fr.shapes):
             raise ValueError("frames0 must hold frame 0 of every sequence")
-        G, self._hw = len(fr.shapes), list(fr.shapes)
-        K = self.K
+        G, K = len(fr.shapes), self.K
         if len(check_gt(gt)) != G:
             raise ValueError(f"one gt array per sequence expected ({G})")
         net, S = self.tracker.net, G * K
@@ -206,48 +217,20 @@ class VotRunner:
             raise ValueError(f"{G} sequences x {K} combinations = {S} streams exceed the engine's max_batch "
                              f"({net.max_batch}) or free slots ({net.num_slots - self.tracker.slot0}); split the run, "
                              "or queue it with open_queue()")
-        self._sched = None
-        self._load_gt(gt)
-        Tmax = int(self.T.max())
-        video = np.repeat(np.arange(G), K)
-        self._video = video
-        c0 = self._init[video, 0]
-        self.tracker._clear()
-        ids = self.tracker.add_state(fr, c0[:, 0:2], c0[:, 2:4], frame_index=video,
-                                     hp=None if self.combos is None else np.tile(self.combos, (G, 1)))
-        self._stream_of = {i: s for s, i in enumerate(ids)}          # tracker id -> stream
-        self._id_of = ids
-        # rows [0, Tmax) of stream s: (entry code, location x, y, w, h); row Tmax: (lost_times, 0, 0, 0, 0)
-        self._rec = torch.zeros(Tmax + 1, S, 5, dtype=torch.float64, device=self.dev)
-        self._rec[0, :, 0] = CODE_INIT
-        self._poly = torch.zeros(Tmax, S, 8, dtype=torch.float64, device=self.dev) if self.mask else None
-        self._start = torch.zeros(S, dtype=torch.int32, device=self.dev)
-        self._flags = torch.zeros(S, dtype=torch.uint8, device=self.dev)
-        self._pinned = [torch.zeros(S, dtype=torch.uint8).pin_memory() for _ in range(SKIP_FRAMES + 1)]
-        self._events = [None] * (SKIP_FRAMES + 1)
-        self.G, self.f = G, 0
-        self._index_rows()
-        self._retire()
-        self.f = 1
+        self._reset(gt)
+        self._run(fr, Step([(g, 0) for g in range(G)], {s: s // K for s in range(S)}, [], list(range(S)),
+                           np.nonzero(self._video_T == 1)[0].tolist()))
         return self
 
     def _index_rows(self):
-        """Stream and sequence of each active tracker row (and, in a queue run, its admission step): a host list and
-        device indices.  The upload waits for the copy, so it runs only when the set of active streams changes."""
+        """Stream, sequence, frame size and admission step of each active tracker row: a host list and device indices.
+        The upload waits for the copy, so it runs only when the set of active streams changes."""
         self._row_streams = [self._stream_of[i] for i in self.tracker.ids]
         self._row_dev = torch.tensor(self._row_streams, dtype=torch.long, device=self.dev)
         self._row_video = torch.as_tensor(self._video[self._row_streams], dtype=torch.long, device=self.dev)
         wh = [self._hw[self._video[s]][::-1] for s in self._row_streams]     # each row's own (W, H)
         self._row_wh = torch.tensor(wh, dtype=torch.int32, device=self.dev).reshape(-1, 2)
-        if self._sched is not None:
-            self._row_admit = torch.as_tensor(self._admit[self._row_streams], dtype=torch.long, device=self.dev)
-
-    def _retire(self):
-        """Step 5: streams whose sequence ends with frame self.f leave the batch."""
-        done = [i for i in self.tracker.ids if self.T[self._video[self._stream_of[i]]] == self.f + 1]
-        if done:
-            self.tracker.remove(done)
-            self._index_rows()
+        self._row_admit = torch.as_tensor(self._admit[self._row_streams], dtype=torch.long, device=self.dev)
 
     @torch.no_grad()
     def frame(self, frames):
@@ -266,42 +249,9 @@ class VotRunner:
                 raise ValueError(f"frames must be a list of {self.G} frames")
         elif np.ndim(frames) != 4 or len(fr.shapes) != self.G:
             raise ValueError(f"frames must be [{self.G},H,W,3]")
-        rows = self._row_dev
-        # 1. track every active stream (skipped ones too: their outputs are discarded below)
-        # 2. overlap of the gt polygon with the predicted polygon, stored as C floats
-        r, loc, pred = self._predict(fr)
-        ov = ops._vot_overlap_sized(self._gt[self._row_video, f], pred, self._row_wh)
-        # 3. bookkeeping on the device: init / track / skip by the stream's start frame; only an overlap of exactly 0
-        #    is a failure (NaN is truthy)
-        start = self._start[rows]
-        tracking = start < f
-        lost = tracking & (ov == 0)
-        code = torch.where(start == f, CODE_INIT, torch.where(lost, CODE_LOST, CODE_LOCATION * tracking.long()))
-        self._rec[f, rows, 0] = code.double()
-        self._locations()[f * self._rec.shape[1] + rows] = torch.where(tracking & ~lost, 1, 0).unsqueeze(1) * loc
-        self._rec[-1, rows, 0] += lost.double()
-        self._start[rows] = torch.where(lost, f + SKIP_FRAMES, start)
-        self._flags.zero_()
-        self._flags[rows] = lost.to(torch.uint8)
-        slot = f % len(self._pinned)
-        self._pinned[slot].copy_(self._flags, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream(self.dev))
-        self._events[slot] = ev
-        # 4. re-initialise the streams lost at frame f - 5 (their start frame is f), from the gt of frame f
-        if f > SKIP_FRAMES:                              # nothing is lost on frame 0
-            old = (f - SKIP_FRAMES) % len(self._pinned)
-            self._events[old].synchronize()
-            again = np.nonzero(self._pinned[old].numpy())[0]
-            active = set(self._row_streams)
-            again = [int(s) for s in again if int(s) in active]
-            if again:
-                c = self._init[self._video[again], f]
-                self.tracker.reinit([self._id_of[s] for s in again], fr, c[:, 0:2], c[:, 2:4])
-        # 5. sequences that end with this frame leave the batch
-        self._retire()
-        self.f += 1
-        return r
+        K = self.K
+        return self._run(fr, Step([(g, f) for g in range(self.G)], {s: s // K for s in range(self.G * K)},
+                                  self._row_streams, [], np.nonzero(self._video_T == f + 1)[0].tolist()))
 
     def result(self):
         """One D2H copy (two in mask mode).  Returns (regions, lost_times): regions[g][k] is stream (g, k)'s list in the
@@ -310,10 +260,8 @@ class VotRunner:
         rec = self._rec.cpu().numpy()
         poly = self._poly.cpu().numpy() if self.mask else None
         G, K = self.G, self.K
-        if self._sched is None:
-            n = np.repeat(np.minimum(self.T, self.f), K)
-        else:                                           # frames 0 .. f - admission step - 1 of each admitted stream
-            n = np.where(self._admit >= 0, np.minimum(self._video_T, self.f - self._admit), 0)
+        # frames 0 .. f - admission step - 1 of each admitted stream
+        n = np.where(self._admit >= 0, np.minimum(self._video_T, self.f - self._admit), 0)
         regions = [[regions_from_record(rec[:, g * K + k], int(n[g * K + k]),
                                         None if poly is None else poly[:, g * K + k]) for k in range(K)]
                    for g in range(G)]
@@ -333,43 +281,9 @@ class VotRunner:
 
         Frames may differ in size between sequences (not within one); `result()` and `VotScore.add` then work as for
         `open`, stream (g, k) being row g*K + k."""
-        G, K = self._load_gt(gt), self.K
-        if G == 0:
-            raise ValueError("open_queue needs at least one sequence")
-        net = self.tracker.net
-        cap = min(net.max_batch, net.num_slots - self.tracker.slot0)
-        if cap < 1:
-            raise ValueError("the engine has no free slot")
-        S, Tmax = G * K, int(self.T.max())
-        self._sched = Scheduler(self.T, K, cap)
-        self._plan = self._sched.step()
-        self._hw = [None] * G                           # each sequence's (H, W), from its frame 0
-        self._video = np.repeat(np.arange(G), K)
-        self._video_T = self.T[self._video]
-        self._admit = np.full(S, -1, np.int64)          # the step at which each stream was templated
-        self.tracker._clear()
-        self._stream_of, self._id_of = {}, [None] * S
-        self._rec = torch.zeros(Tmax + 1, S, 5, dtype=torch.float64, device=self.dev)
-        self._rec[0, :, 0] = CODE_INIT
-        self._poly = torch.zeros(Tmax, S, 8, dtype=torch.float64, device=self.dev) if self.mask else None
-        self._start = torch.zeros(S, dtype=torch.int32, device=self.dev)         # in the stream's own frames
-        self._flags = torch.zeros(S, dtype=torch.uint8, device=self.dev)
-        self._pinned = [torch.zeros(S, dtype=torch.uint8).pin_memory() for _ in range(SKIP_FRAMES + 1)]
-        self._events = [None] * (SKIP_FRAMES + 1)       # (step, event) of the flags in each pinned buffer
-        self.G, self.f = G, 0
-        self._index_rows()
+        self._reset(gt)
+        self._queue(self.T, self.K)
         return self
-
-    @property
-    def pending(self) -> bool:
-        """Whether a queue run has steps left."""
-        return self._sched is not None and self._plan is not None
-
-    def needed(self) -> list:
-        """The distinct (sequence, frame) pairs the next `step` reads, in the order its frame list must follow."""
-        if not self.pending:
-            raise ValueError("no queue step is pending: call open_queue() first; the run has finished")
-        return list(self._plan.need)
 
     @torch.no_grad()
     def step(self, frames):
@@ -378,26 +292,29 @@ class VotRunner:
         the streams lost 5 frames earlier, retires the streams whose sequence ends, then templates the admitted streams
         from their frame 0.  A step waits for the device only when it re-initialises, admits or retires streams.
         Returns the tracker's `TrackResult` of the streams that tracked a frame, or None when none did."""
-        if not self.pending:
-            raise ValueError("no queue step is pending: call open_queue() first; the run has finished")
-        st, f, bt = self._plan, self.f, self.tracker
-        if not isinstance(frames, (list, tuple)) or len(frames) != len(st.need):
-            raise ValueError(f"frames must be a list of {len(st.need)} frames, one per needed() entry")
-        fr = bt._input(frames)
+        st = self._pending_step(frames=frames)
+        fr = self.tracker._input(frames)
         for i, (g, t) in enumerate(st.need):
             if self._hw[g] is not None and fr.shapes[i] != self._hw[g]:
                 h, w = fr.shapes[i] if fr.shapes[i] is not None else (0, 0)
                 raise ValueError(f"frame {t} of sequence {g} is {h}x{w}, its frame 0 {self._hw[g][0]}x{self._hw[g][1]}")
+        r = self._run(fr, st)
+        self._advance()
+        return r
+
+    def _run(self, fr, st):
+        """Step st over the step's frames fr: steps 1-4 of the module docstring for the running streams, each at its own
+        frame t = f - admission step, then the streams whose sequence ends leave and the admitted streams are templated
+        from their frame 0 (a one-frame sequence is its frame 0's init alone)."""
+        f, bt = self.f, self.tracker
         r = None
         if st.track:
-            want = [st.entry[self._stream_of[i]] for i in bt.ids]
-            if want != bt._fidx:                        # the frame list moved: only after admissions or departures
-                bt.set_frame_index(bt.ids, want)
+            self._repoint([st.entry[self._stream_of[i]] for i in bt.ids])
             r = self._track(fr, f)
         gone = [self._id_of[s] for s in st.retire if self._id_of[s] is not None]
         if gone:
             bt.remove(gone)
-        new = [s for s in st.admit if self._video_T[s] > 1]      # a one-frame sequence is its frame 0's init alone
+        new = [s for s in st.admit if self._video_T[s] > 1]
         for s in st.admit:
             g = int(self._video[s])
             if self._hw[g] is None:
@@ -405,15 +322,13 @@ class VotRunner:
             self._admit[s] = f
         if new:
             c0 = self._init[self._video[new], 0]
-            K = self.K
-            hp = None if self.combos is None else self.combos[[s % K for s in new]]
+            hp = None if self.combos is None else self.combos[[s % self.K for s in new]]
             ids = bt.add_state(fr, c0[:, 0:2], c0[:, 2:4], frame_index=[st.entry[s] for s in new], hp=hp)
             for s, i in zip(new, ids):
                 self._stream_of[i], self._id_of[s] = s, i
         if gone or new:
             self._index_rows()
         self.f += 1
-        self._plan = self._sched.step() if not self._sched.done else None
         return r
 
     def _predict(self, fr):
@@ -434,27 +349,26 @@ class VotRunner:
         loc = torch.stack([x0, y0, st[:, 2], st[:, 3]], 1)
         return r, loc, torch.stack([x0, y0, x1, y0, x1, y1, x0, y1], 1).float()
 
-    def _locations(self) -> torch.Tensor:
-        """The record's location columns as a [(Tmax) * S, 4 or 8] view, row f * S + s: rec[..., 1:5] in box mode,
-        the polygon plane in mask mode."""
-        return self._poly.view(-1, 8) if self.mask else self._rec.view(-1, 5)[:, 1:5]
-
     def _track(self, fr, f: int):
-        """Steps 1-4 of `frame` for the running streams of a queue step f: each row at its own frame t = f - admission
-        step, its record row t and its gt row t."""
+        """Steps 1-4 for the running streams of step f: each row at its own frame t = f - admission step, its record
+        row t and its gt row t."""
         rows = self._row_dev
         S, Tmax = self._rec.shape[1], self._gt.shape[1]
+        # 1. track every active stream (skipped ones too: their outputs are discarded below)
+        # 2. overlap of the gt polygon with the predicted polygon, stored as C floats
         r, loc, pred = self._predict(fr)
         t = f - self._row_admit                          # each row's own frame, on the device
         ov = ops._vot_overlap_sized(self._gt.view(-1, 8)[self._row_video * Tmax + t], pred, self._row_wh)
+        # 3. bookkeeping on the device: init / track / skip by the stream's start frame; only an overlap of exactly 0
+        #    is a failure (NaN is truthy)
         start = self._start[rows].long()
         tracking = start < t
         lost = tracking & (ov == 0)
         code = torch.where(start == t, CODE_INIT, torch.where(lost, CODE_LOST, CODE_LOCATION * tracking.long()))
-        rec = self._rec.view(-1, 5)
         at = t * S + rows
-        rec[at, 0] = code.double()
-        self._locations()[at] = torch.where(tracking & ~lost, 1, 0).unsqueeze(1) * loc
+        self._rec.view(-1, 5)[at, 0] = code.double()
+        locations = self._poly.view(-1, 8) if self.mask else self._rec.view(-1, 5)[:, 1:5]
+        locations[at] = torch.where(tracking & ~lost, 1, 0).unsqueeze(1) * loc
         self._rec[-1, rows, 0] += lost.double()
         self._start[rows] = torch.where(lost, t + SKIP_FRAMES, start).int()
         self._flags.zero_()
@@ -464,8 +378,8 @@ class VotRunner:
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(self.dev))
         self._events[slot] = (f, ev)
-        # re-initialise the streams lost at step f - 5 (every active stream advanced 5 frames since), from the gt of
-        # each one's own frame
+        # 4. re-initialise the streams lost at step f - 5 (every active stream advanced 5 frames since), from the gt of
+        #    each one's own frame
         old = self._events[(f - SKIP_FRAMES) % len(self._pinned)]
         if old is not None and old[0] == f - SKIP_FRAMES:
             if not old[1].query():                       # 5 steps old: as good as always complete
@@ -477,7 +391,6 @@ class VotRunner:
                 c = self._init[self._video[again], f - self._admit[again]]
                 self.tracker.reinit([self._id_of[s] for s in again], fr, c[:, 0:2], c[:, 2:4])
         return r
-
 
 
 # EAOBenchmark's (low, high) per dataset (utils/pysot/evaluation/eao_benchmark.py): EAO averages curve[low-1 .. high-1]

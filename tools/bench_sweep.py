@@ -143,7 +143,8 @@ def main():
     res["frame_ms"] = 1e3 * dt / args.frames
     iou_list, _ = sweep.result()
     res["best_mean_iou"] = float(iou_list.max())
-    res["scoring"] = scoring_legs(r, annos[T - 2], sweep._video, THRESHOLDS, W, H)
+    video = torch.arange(G, dtype=torch.int32, device="cuda").repeat_interleave(K)     # stream g*K + k scores video g
+    res["scoring"] = scoring_legs(r, annos[T - 2], video, THRESHOLDS, W, H)
     res["scoring"]["traffic_bytes_shapes_only"] = {"unfused": 4 * H * W * (1 + len(THRESHOLDS)) * G * K}
     res["serial_b1"] = serial_leg(sd, combos, frames, boxes, args.serial_frames, base)
     if args.baseline_tracker:
